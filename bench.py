@@ -1,10 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- Groth16 withdraw proofs per second on B200 (BASELINE.json metric, config 4).
+"""bench.py -- Groth16 withdraw proofs per second on H100 (BASELINE.json metric, config 4).
 
 A "step" is one pass of the hot path over one batch of 1024 synthetic depth-32 withdraw witnesses:
 MiMC7 Merkle-path witness generation -> A.w/B.w -> 6 NTTs -> 3 fixed-base MSMs -> 256-byte proofs.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+`--dump-outputs DIR`: after the timed steps, rank 0 writes what the last timed step returned -- the proofs and the
+            public inputs, one byte per float32 element -- and the two sums of the sharded MSM leg as DIR/<name>.npy.
+            Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 `value`   : whole-job proofs/s with the secret inputs already resident in HBM (og_*_dev entry points),
             timed with CUDA events on the library's stream, max over ranks.
@@ -39,12 +43,15 @@ UNIT = "proofs/s"
 TOXIC_SEED = 20260922
 
 
+HBM_NOMINAL_GBS = 3350.0      # H100 SXM data sheet (HBM3)
+
+
 def measured_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return HBM_NOMINAL_GBS, "nominal"
 
 
 class ClockSampler:
@@ -121,8 +128,7 @@ def parse_pk_blob(pk: bytes, n_vars, n_pub, log_m):
 
 
 def physical_cores():
-    """Host threads the CPU prover should use: physical cores (SMT siblings slow this integer-bound code down:
-    6.4 proofs/s on 128 threads vs 8.8 on 64 on the round-1 box)."""
+    """Host threads the CPU prover should use: physical cores (SMT siblings slow this integer-bound code down)."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     try:
         import psutil
@@ -131,7 +137,7 @@ def physical_cores():
             n = min(n, phys)
     except Exception:
         pass
-    try:      # a cgroup CPU quota caps what the threads can get whatever the affinity mask says (round 2: 16 of 128 on the bench box)
+    try:      # a cgroup CPU quota caps what the threads can get whatever the affinity mask says
         q, per = open("/sys/fs/cgroup/cpu.max").read().split()
         if q != "max":
             n = max(1, min(n, int(float(q) / float(per) + 0.999)))
@@ -142,7 +148,7 @@ def physical_cores():
 
 def host_cpu_info():
     """What the CPU arm can actually use on this box, so that ratios compare across boxes: affinity mask, cgroup
-    quota, SMT layout, load before the run (round 1 saw 8.6 vs 34 proofs/s on two boxes that both said "64 cores")."""
+    quota, SMT layout, load before the run (two hosts that both report "64 cores" can differ severalfold)."""
     info = {"affinity": len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else None, "os_cpu_count": os.cpu_count()}
     try:
         import psutil
@@ -278,7 +284,8 @@ def sharded_msm_leg(torch, dist, ob, api, ctx, dev, rank, world, log_n, steps=3,
     if dist:
         dist.barrier()
     alg = (64 + 128 + 32) * n
-    return {"workload": f"2^{log_n}-point G1 + G2 MSM, shared scalars, point-range sharded over {world} rank(s) (BASELINE config 5 shape; "
+    sums = {"sharded_msm_g1": out1.cpu().numpy(), "sharded_msm_g2": out2.cpu().numpy()}
+    return sums, {"workload": f"2^{log_n}-point G1 + G2 MSM, shared scalars, point-range sharded over {world} rank(s) (BASELINE config 5 shape; "
                         f"2^24 needs the 8-GPU box, see scripts/bench_sharded_msm.py)",
             "log_n": log_n, "n_gpus": world, "ms": ms, "points_per_s": n / (ms * 1e-3), "algorithmic_bytes": alg,
             "hbm_gbs_aggregate": alg / (ms * 1e-3) / 1e9, "exchange_bytes_per_rank": 192, "ranks_agree": bool(agree.item()),
@@ -342,7 +349,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--no-parity", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--sharded-log-n", type=int, default=22, help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's proofs and public inputs (and the sharded MSM sums) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -443,12 +454,20 @@ def main():
     h2d = len(nul) + len(sec) + len(rec) + len(sib) + 4 * batch + len(rs)
     d2h = 256 * batch + 96 * batch
 
-    sharded = None
+    sharded, sums = None, {}
     if args.sharded_log_n > 0:
         try:
-            sharded = sharded_msm_leg(torch, dist, ob, api, ctx, dev, rank, world, args.sharded_log_n)
+            sums, sharded = sharded_msm_leg(torch, dist, ob, api, ctx, dev, rank, world, args.sharded_log_n, steps=args.steps)
         except Exception as e:      # an extra leg: its failure must not hide the headline
             sharded = {"error": f"{type(e).__name__}: {e}"}
+
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        outs = {"proofs": np.frombuffer(proofs_host, dtype=np.uint8).reshape(batch, 256),
+                "public_inputs": np.frombuffer(pub_host, dtype=np.uint8).reshape(batch, 96), **sums}
+        for name, a in outs.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a.astype(np.float32))
 
     # max over ranks
     times = torch.tensor([dev_ms, wall_ms, e2e_ms], dtype=torch.float64, device=dev)
@@ -472,12 +491,6 @@ def main():
         alg_bytes_per_launch = 96.0 * pairs_per_proof_g1 * batch * args.steps / max(kn, 1)
         avg_ms = kms / max(kn, 1)
         achieved = alg_bytes_per_launch / (avg_ms * 1e-3) / 1e9 if avg_ms > 0 else 0.0
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                traffic = json.load(f).get(kname)
-        except Exception:
-            pass
         pipes = ctx.int_pipe_peaks()
         def cbits(name, dflt):      # mirrors groth16.cu: pk_load (defaults 15 / 15 / 16 bits for A / B / C')
             return int(os.environ.get(name) or os.environ.get("OG_WINDOW_BITS") or dflt)
@@ -537,15 +550,15 @@ def main():
             "config": {"workload": f"groth16 withdraw prove, batch {batch} per GPU, depth-{DEPTH} MiMC7 Merkle witnesses (BASELINE config 4)",
                        "circuit_constraints": info["n_constraints"], "circuit_variables": info["n_vars"], "domain": m,
                        "parallelism": f"replicas x{world} (independent proofs, no data-path collective)",
-                       "l2": "per-step working set (sorted digit lists + window tables, > 2 GB) exceeds the 126 MB L2; no flush needed",
+                       "l2": "per-step working set (sorted digit lists + window tables, > 2 GB) exceeds the 50 MB L2; no flush needed",
                        "timing": "CUDA events on the library stream, max over ranks", "wall_ms_per_step": wall_ms / args.steps,
                        "proofs_verify": bool(verified), "e2e_bytes_equal_device_path": bool(e2e_match), "parity": parity},
             "e2e": {"value": world * batch * args.steps / (e2e_ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(launches),
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
-                         "frac": achieved / hbm_peak if hbm_peak else None, "frac_of_nominal_8tbs": achieved / 8000.0,
-                         "traffic": traffic, "peak_source": peak_kind,
+                         "frac": achieved / hbm_peak if hbm_peak else None, "frac_of_nominal": achieved / HBM_NOMINAL_GBS,
+                         "peak_source": peak_kind,
                          "avg_launch_ms": avg_ms, "launches": kn, "share_of_step": kms / total_prof_ms if total_prof_ms else None,
                          "note": "MSM is bound by the 32-bit integer multiply-add pipe, not HBM (DESIGN.md 5); see `imad`"},
             "imad": {"kernel": kname, "achieved_wide_mad_per_s": wide_rate, "peak_wide_mad_per_s": pipes["imad_wide_carry_chain_per_s"],

@@ -1,4 +1,4 @@
-/* include/owshen_b200.h -- C ABI of the B200-native Groth16 backend (libowshen_b200.so).
+/* include/owshen_b200.h -- C ABI of the H100-native (sm_90a) Groth16 backend (libowshen_b200.so).
  *
  * WHAT THIS REPLACES IN THE REFERENCE.  OwshenNetwork/owshen @ c7b1f00 has no prover, no FFI and no
  * plugin interface for proving (SURVEY.md section 0 / 8b), so there is no reference binding to cite

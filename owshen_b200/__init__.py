@@ -1,4 +1,4 @@
-"""owshen_b200 -- B200-native (sm_100a) Groth16 backend for privacy-pool withdraw proofs over BN254.
+"""owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool withdraw proofs over BN254.
 
 Python is the host language here because the reference's (Rust) toolchain is absent from this image;
 everything below is a thin ctypes veneer over the C ABI in include/owshen_b200.h, which is the real

@@ -29,7 +29,7 @@ class OwshenB200Error(RuntimeError):
 
 
 def build_library(jobs=8):
-    """Compile every CUDA source for sm_100a into owshen_b200/libowshen_b200.so (in-tree)."""
+    """Compile every CUDA source for sm_90a into owshen_b200/libowshen_b200.so (in-tree)."""
     subprocess.run(["make", "-C", os.path.join(_HERE, "csrc"), f"-j{jobs}"], check=True, stdout=subprocess.DEVNULL)
 
 

@@ -1,5 +1,5 @@
 // owshen_b200/csrc/bjj_impl.cuh -- (included at the end of mimc.cu: it shares the MiMC7 round constants)
-// batched BabyJubJub EdDSA-style signature verification on sm_100a.
+// batched BabyJubJub EdDSA-style signature verification on sm_90a.
 //
 // This is the one kernel whose algorithm the reference defines: it follows
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs --

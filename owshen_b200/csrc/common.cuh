@@ -21,7 +21,7 @@ struct NttTables;   // ntt.cu
 
 struct og_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;        // the stream launches go to NOW (OG_LAUNCH); == main_stream outside a lane
     cudaStream_t main_stream = nullptr;   // what og_sync / og_timer_* / the host-pointer copies use
     // the batched prover keeps MAX_LANES chunks in flight: per lane one high-priority stream for the short

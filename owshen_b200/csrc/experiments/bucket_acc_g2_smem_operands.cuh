@@ -1,10 +1,9 @@
 // owshen_b200/csrc/experiments/bucket_acc_g2_smem_operands.cuh -- REJECTED EXPERIMENT, not part of libowshen_b200.so.
 // G2 bucket accumulation with EVERY Fq2 value of the mixed addition in shared memory (VERDICT r1 item 4: "pass Fq2 operands to
-// the out-of-line multiplier through the shared-memory accumulator layout").  Measured in round 2 (profiles/r2_small_ab.md):
-// bit-exact, local-memory traffic per addition 550 -> ~30 accesses, 128 registers, 0.17 KB stack -- and 91.3 instead of 88.4 ms per
-// 1024 proofs, which is exactly what 4 instead of 6 resident CTAs cost the by-value kernel in round 1 (90.4 ms): the spills and the
-// marshalling moves are not what bounds the kernel, the multiplier's own instruction mix is (per Fq2 product 302 IMAD.WIDE + 58 other
-// FMA-pipe instructions + 305 ALU instructions, identical in both forms).  To repeat: paste into msm.cu inside #ifdef OG_MSM_G2 and
+// the out-of-line multiplier through the shared-memory accumulator layout").  Bit-exact, with far less local-memory traffic per
+// addition (128 registers) -- and slower than the shipped kernel, as slow as that kernel at 4 instead of 6 resident CTAs: the
+// spills and the marshalling moves are not what bounds the kernel, the multiplier's own instruction mix is (identical in both
+// forms).  To repeat: paste into msm.cu inside #ifdef OG_MSM_G2 and
 // launch k_bucket_acc_sm2 with 6 * 4 * 128 * 16 bytes of dynamic shared memory instead of k_bucket_acc_sm.
 //
 //     p   = qx ZZ - X                 -> P        (X is dead after q1, r takes its slot; x3 lands in P and the two

@@ -1,11 +1,11 @@
 // owshen_b200/csrc/experiments/bucket_affine.cuh -- REJECTED EXPERIMENT, not part of libowshen_b200.so.
-// Batched-affine bucket accumulation for the prover's MSMs, measured in round 2 against the XYZZ kernel it was meant to
-// replace (profiles/r2_affine_ab.md: bit-exact, but 246-249 ms + 32 ms of inversion kernels against 233 ms per 1024 proofs;
-// ncu: 394 B of DRAM traffic per addition at 41 % of HBM peak, FMA pipe 31 % active).  Kept so that the measurement can be
+// Batched-affine bucket accumulation for the prover's MSMs, compared against the XYZZ kernel it was meant to replace:
+// bit-exact, but slower once its batched inversion kernels are counted (it moves several hundred bytes of DRAM traffic per
+// addition).  Kept so that the measurement can be
 // repeated: build msm.cu with -DOG_EXPERIMENT_AFFINE (it is included from there) and run with OG_AFFINE=1 (G1) / 3 (G1 + G2).
 #pragma once
 
-// ---- 4b: batched-affine bucket accumulation (the batched prover; profiles/r2_affine_ab.md) ------------------------
+// ---- 4b: batched-affine bucket accumulation (the batched prover) ------------------------
 // A mixed XYZZ addition costs 8M + 2S; an affine addition costs 1M + 1S + 1M once 1/(x2 - x1) is known, and Montgomery's
 // trick turns N inversions into one inversion and 3(N-1) products.  With 10^7 buckets per chunk there are 10^7 independent
 // additions available at every step of the bucket lists, so the accumulation runs in ROUNDS: round j adds entry j of every

@@ -1,4 +1,4 @@
-// owshen_b200/csrc/fp.cuh -- 256-bit prime-field arithmetic for sm_100a, 8 x 32-bit limbs in registers.
+// owshen_b200/csrc/fp.cuh -- 256-bit prime-field arithmetic for sm_90a, 8 x 32-bit limbs in registers.
 //
 // Montgomery form with R = 2^256.  The multiplier is the even/odd split CIOS: the running sum is
 // kept in two staggered 8-limb arrays so every 32x32->64 partial product lands in a (lo, hi) pair
@@ -108,7 +108,7 @@ OG_HD void final_sub(uint32_t* r) {
 //    and because s + lo(q*p0) == 0 (mod 2^32) the low product is never computed: its carry is (s != 0),
 //    injected with add.cc(s, 0xffffffff) into the q*p chain on E, which starts at limb 1.
 // No limb ripples through a whole array, so successive rows overlap and the dependency chain per product
-// is short (this kernel family is latency-bound at 4 warps/scheduler; see profiles/).
+// is short (this kernel family is latency-bound at 4 warps/scheduler).
 template <class P>
 OG_HD void mont_row(uint32_t* E, uint32_t* O, const uint32_t* a, uint32_t bi, bool first) {
     CC cc;
@@ -400,9 +400,8 @@ struct alignas(32) Fp {
 
     OG_HD friend Fp operator*(const Fp& a, const Fp& b) { Fp r; mont_mul<P>(r.l, a.l, b.l); return r; }
 #if defined(OG_SQR_INTERLEAVED)
-    // A/B switch: squarings through the interleaved multiplier.  Round 1 built the G1 unit this way (its bucket kernel kept
-    // the accumulator in registers then and was register-bound: 248.9 vs 245.6 ms per 1024 proofs); with the accumulator in
-    // shared memory the wide squarer wins by 0.8 % (231.5 vs 233.3 ms, profiles/r2_small_ab.md) and every unit uses it
+    // A/B switch: squarings through the interleaved multiplier.  The wide squarer is the default in every unit; this
+    // switch keeps the alternative buildable for comparison
     OG_HD Fp sqr() const { Fp r; mont_mul<P>(r.l, l, l); return r; }
 #else
     OG_HD Fp sqr() const { Fp r; uint32_t T[16]; sqr_wide(T, l); mont_reduce_wide<P>(r.l, T); return r; }   // 36 + 64 products
@@ -558,7 +557,7 @@ struct Fq2 {
 #if defined(__CUDA_ARCH__) && defined(OG_FP_MUL_CALL)
 // Translation units whose kernels would inline dozens of Fq2 products per group operation keep ONE copy of
 // the Fq2 multiplier / squarer (arguments and result travel in registers): the fully inlined G2 bucket kernel
-// overflowed the instruction cache (ncu: 30 % of warp samples in "no_instructions", profiles/).
+// overflowed the instruction cache (ncu: warps stalled on "no_instructions").
 static __device__ __noinline__ Fq2 fq2_mul_call(Fq2 a, Fq2 b) { return Fq2::mul_inl(a, b); }
 static __device__ __noinline__ Fq2 fq2_sqr_call(Fq2 a) { return Fq2::sqr_inl(a); }
 OG_HD Fq2 operator*(const Fq2& a, const Fq2& b) { return fq2_mul_call(a, b); }

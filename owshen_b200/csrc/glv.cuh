@@ -4,7 +4,7 @@
 //     k P = k1 P + k2 phi(P),   k = k1 + k2 lambda (mod r),   |k1|, |k2| < 2^127:
 // an n-point MSM with 254-bit scalars becomes a 2n-point MSM with 127-bit scalars -- the same number of bucket additions, but
 // half the windows, i.e. half the bucket sets to reduce and half the ~240 sequential doublings of the final Horner, which are a
-// third of a 2^20-point MSM's time (profiles/r2_msm_oneshot_breakdown.md).  Public technique (Gallant-Lambert-Vanstone, CRYPTO 2001);
+// large share of a 2^20-point MSM's time.  Public technique (Gallant-Lambert-Vanstone, CRYPTO 2001);
 // not in the reference (SURVEY.md section 0).  The short lattice basis comes from the extended Euclid on (r, lambda):
 //     v1 = (A1, -NB1),  v2 = (A2, A1),   a_i + b_i lambda = 0 (mod r)
 // and  c1 = round(b2 k / r), c2 = round(-b1 k / r)  are taken with precomputed  G_i = round(2^256 b / r):  c = (G k + 2^255) >> 256

@@ -1,4 +1,4 @@
-// owshen_b200/csrc/groth16.cu -- batched Groth16 prover for sm_100a (BASELINE config 4) plus the
+// owshen_b200/csrc/groth16.cu -- batched Groth16 prover for sm_90a (BASELINE config 4) plus the
 // development setup.  The reference has no prover (SURVEY.md section 0); conventions are frozen in
 // DESIGN.md section 4 and checked bit-for-bit against oracle/groth16.py and oracle/cpu.
 //
@@ -250,7 +250,8 @@ int32_t pk_load(og_ctx* ctx, const uint8_t* bytes, uint64_t len, og_pk** out) {
     for (uint32_t i = 0; i < nv; i++)
         if (!all_zero(qb1 + 64ull * i, 64) || !all_zero(qb2 + 128ull * i, 128)) supp.push_back(i);
     pk->n_supp = (uint32_t)supp.size();
-    // measured on B200 (profiles/r1_window_sweep.md): 15 bits for A and B, 16 for C' (3x the points); OG_WINDOW_BITS overrides all three, OG_C_A / OG_C_B / OG_C_C one each
+    // 15 bits for A and B, 16 for C' (3x the points): the fastest of the H100 sweep in DESIGN.md section 8;
+    // OG_WINDOW_BITS overrides all three, OG_C_A / OG_C_B / OG_C_C one each
     const uint32_t dflt[3] = {15, 15, 16};
     const char* names[3] = {"OG_C_A", "OG_C_B", "OG_C_C"};
     for (int k = 0; k < 3; k++) {
@@ -459,7 +460,7 @@ static uint32_t chunk_limit(const og_pk* pk) {
     return (uint32_t)(lim < 1 ? 1 : lim);
 }
 
-// OG_CHUNK proofs per chunk (default 1024 = the whole BASELINE batch, ~28 GB of scratch per lane; profiles/r2_lanes_sweep.md), OG_LANES chunks in flight (default 2, 1 = serial)
+// OG_CHUNK proofs per chunk (default 1024 = the whole BASELINE batch, ~28 GB of scratch per lane, which the 80 GB of an H100 holds), OG_LANES chunks in flight (default 2, 1 = serial)
 static uint32_t chunk_size(const og_pk* pk, uint32_t batch) {
     uint32_t c = env_u32("OG_CHUNK", 1024);
     if (c > chunk_limit(pk)) c = chunk_limit(pk);

@@ -1,4 +1,4 @@
-// owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_100a: 2-to-1 node hash, batched Merkle
+// owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
 // paths (BASELINE config 2), level-by-level tree build, and the witness generator of the withdraw
 // statement (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //

@@ -1,5 +1,5 @@
 // owshen_b200/csrc/msm.cu -- bucket-method (Pippenger) multi-scalar multiplication on BN254 G1/G2
-// for sm_100a.  BASELINE configs 3 and 5 and the inner engine of the batched Groth16 prover.
+// for sm_90a.  BASELINE configs 3 and 5 and the inner engine of the batched Groth16 prover.
 //
 // No counterpart in the reference (SURVEY.md section 0).  Pipeline (DESIGN.md section 5.3):
 //   1. k_digits<false>   signed c-bit digits of every scalar, histogram of (group, bucket) keys
@@ -122,9 +122,8 @@ struct DigitIter {
 };
 
 // one thread per scalar, global atomics (one-shot MSMs: up to 2^15 buckets x 16 windows of keys).  The scatter is pure
-// atomic round-trip latency (ncu, profiles/r2_ncu_digits.md: 93 % of the warp samples on the long scoreboard, issue slots 17 %
-// busy); cutting eight windows first and issuing their eight atomics back to back was measured SLOWER (21.3 vs 20.1 ms per 1024
-// proofs, profiles/r2_small_ab.md): the L2 atomic units, not the per-thread dependency, are what the kernel waits for.
+// atomic round-trip latency (warps wait on the long scoreboard); cutting eight windows first and issuing their eight atomics
+// back to back does not help: the L2 atomic units, not the per-thread dependency, are what the kernel waits for.
 template <bool SCATTER>
 __global__ void __launch_bounds__(256) k_digits(DigitPlan P, uint32_t* __restrict__ counts, const uint32_t* __restrict__ offsets,
                                                 uint32_t* __restrict__ cursor, uint32_t* __restrict__ sorted, int* flag) {
@@ -146,9 +145,8 @@ __global__ void __launch_bounds__(256) k_digits(DigitPlan P, uint32_t* __restric
 
 // Tiled histogram for the batched prover (one group per proof, nb <= 32768): a CTA owns a tile of one problem's
 // scalars, counts its digits in shared memory and touches global memory once per bucket instead of once per
-// digit (5x faster than global atomics: 5 vs 24 ms per 1024 proofs).  The scatter stays the plain k_digits<true>:
-// a tiled scatter with run reservation and a one-CTA-per-proof shared-memory sort were both measured slower
-// (39 vs 33 ms and 56.6 vs 29 ms per 1024 proofs, profiles/r1_*; their code was removed in round 2).
+// digit.  The scatter stays the plain k_digits<true>: a tiled scatter with run reservation and a one-CTA-per-proof
+// shared-memory sort were both slower and were removed.
 constexpr uint32_t DIG_TILE = 4096, DIG_THREADS = 256, DIG_MAX_NB_COUNT = 32768;
 
 __global__ void __launch_bounds__(DIG_THREADS) k_digits_count_tiled(DigitPlan P, uint32_t* __restrict__ counts, int* flag) {
@@ -259,7 +257,7 @@ int32_t msm_sort_digits(og_ctx* ctx, const DigitPlan& plan, uint32_t n_keys, uin
 
 // ---- 3b: order the buckets of every group by decreasing load ------------------------------------------------
 // Bucket loads are Poisson-distributed, so a warp of 32 neighbouring buckets waits for its longest list
-// (ncu: 26.5-28.4 of 32 lanes active on G1, 24.8 on G2).  A counting sort of the bucket ids by their count
+// (ncu shows a quarter or more of the lanes idle).  A counting sort of the bucket ids by their count
 // puts equal loads in the same warp and schedules the longest lists first.
 constexpr uint32_t ORDER_BINS = 2048;
 template <class F>   // (template only so that each translation unit gets its own copy)
@@ -317,10 +315,9 @@ struct SmAcc1 {
 };
 
 // 8 CTAs of 128 threads per SM (64 registers); only the next 4-byte ENTRY is read ahead, the 64-byte gather is
-// covered by the other warps (measured against 6/7 CTAs and against a prefetched point: profiles/r1_bucket_acc_smem_sweep.md)
+// covered by the other warps (compared against 6/7 CTAs and against a prefetched point)
 // the two squarings of a mixed addition through ONE out-of-line copy of the wide squarer (8 registers in, 8 out): with the squarer
-// inlined twice next to eight inlined products the kernel outgrew the instruction cache (ncu: 12.7 % of the warp samples waiting
-// for instructions after the wide squarer replaced the interleaved one, profiles/r2_small_ab.md)
+// inlined twice next to eight inlined products the kernel outgrows the instruction cache (ncu: warps waiting for instructions)
 #ifndef OG_SQR_CALL
 #define OG_SQR_CALL 1
 #endif
@@ -387,8 +384,7 @@ __global__ void __launch_bounds__(128, OG_ACC1_MINB) k_bucket_acc_sm1(const Affi
 #ifdef OG_MSM_G2
 // G2 variant with the 256-byte accumulator in shared memory (16-byte chunks interleaved over the CTA's threads, so
 // every access is conflict-free): registers hold only the temporaries of one mixed addition, which buys resident
-// warps in a kernel whose top stall is the fixed-latency wait of the carry chains (4, 5 and 6 resident CTAs were measured
-// in round 1, profiles/r1_bucket_acc_smem_sweep.md; 6 won).
+// warps in a kernel whose top stall is the fixed-latency wait of the carry chains (of 4, 5 and 6 resident CTAs, 6 was fastest).
 struct SmAcc {
     uint4* base;    // [16 chunks][128 threads]
     __device__ __forceinline__ Fq2 ld(int coord) const {
@@ -455,7 +451,7 @@ __global__ void __launch_bounds__(128, 6) k_bucket_acc_sm(const Affine<Fq2>* __r
 
 // Heavy buckets (lists above the cap: witness-like scalars put 30 % of all points into bucket "1" of window 0) are cut
 // into segments of `seg` entries; every segment gets a CTA, a second kernel adds the partial sums of each bucket.
-// Round 1 gave a whole list to ONE CTA: 3*10^5 entries on 256 threads were 5.5 of the 13.9 ms of a witness-like 2^20 MSM.
+// (One CTA per whole list left 3*10^5 entries of a witness-like 2^20 MSM on 256 threads.)
 // heavy[0] = number of heavy buckets, heavy[1 ..] = their keys, heavy[1 + n_keys ..] = first segment of each (+ total).
 template <class F>   // (template only so that each translation unit gets its own copy)
 __global__ void __launch_bounds__(256) k_heavy_plan(uint32_t* __restrict__ heavy, const uint32_t* __restrict__ counts, uint32_t n_keys, uint32_t seg) {
@@ -536,7 +532,7 @@ __global__ void __launch_bounds__(32) k_heavy_combine(const XYZZ<F>* __restrict_
 }
 
 #ifdef OG_EXPERIMENT_AFFINE
-#include "experiments/bucket_affine.cuh"      // rejected in round 2 (profiles/r2_affine_ab.md); not in the shipped library
+#include "experiments/bucket_affine.cuh"      // rejected experiment; not in the shipped library
 #endif
 
 constexpr uint32_t RED_FAN_LOG2 = 3, RED_FAN = 1u << RED_FAN_LOG2;   // 8 children per parent: more threads, shorter chains
@@ -546,11 +542,10 @@ constexpr uint32_t RED_FAN_LOG2 = 3, RED_FAN = 1u << RED_FAN_LOG2;   // 8 childr
 //   S_p = sum S_c;   U_p = sum U_c + 2^w_log2 * sum_c idx(c) * S_c   (running-sum trick for the last term).
 // HAS_U = false is level 0 (children are raw buckets, no weighted part yet): most of the work, and one 4-coordinate
 // accumulator fewer to keep in registers.  (A variant with R and T in shared memory -- 128 instead of 226 registers,
-// twice the resident warps -- was measured slower, 32.7 vs 30.7 ms per step for G1: the R -> T chain, not occupancy,
-// is what this kernel waits on.)
+// twice the resident warps -- was slower for G1: the R -> T chain, not occupancy, is what this kernel waits on.)
 // Group operations of the reduction.  G1: ONE out-of-line copy of add and dbl with operands and result in registers (by
-// value): the fully inlined kernel (three adds and a doubling, ~13k instructions) spent 15 % of its warp samples waiting for
-// instructions (ncu, profiles/r2_ncu_reduce.md) at 8 resident warps per SM.  G2 keeps the inlined group law over the
+// value): the fully inlined kernel (three adds and a doubling, ~13k instructions) stalls waiting for instructions (ncu) at
+// 8 resident warps per SM.  G2 keeps the inlined group law over the
 // out-of-line Fq2 multiplier (128 registers of arguments would not travel in registers).
 template <class F> struct RedOps {
     static __device__ __forceinline__ void add(XYZZ<F>& a, const XYZZ<F>& b) { a.add(b); }
@@ -565,10 +560,10 @@ template <> struct RedOps<Fq> {
 };
 #endif
 
-// measured (profiles/r2_small_ab.md): G1 25.5 (registers, out-of-line ops) vs 29.6 ms (shared memory); G2 25.3 (registers, spilling) vs 24.1 ms
+// G1 is faster with registers and out-of-line ops, G2 (whose register version spills) with shared memory
 template <class F> constexpr bool RED_SM_DEFAULT = sizeof(F) != 32;
 
-// (64 threads, 206 registers for G1: 4 resident CTAs per SM; asking ptxas for 6 or 8 costs spills: 26.4 / 27.6 vs 25.2 ms)
+// (64 threads, 206 registers for G1: 4 resident CTAs per SM; asking ptxas for 6 or 8 costs spills and time)
 template <class F, bool HAS_U>
 __global__ void __launch_bounds__(64) k_reduce_level(const XYZZ<F>* __restrict__ S_in, const XYZZ<F>* __restrict__ U_in,
                                                      uint32_t n_in, uint32_t n_out, uint32_t n_groups, uint32_t w_log2,
@@ -700,7 +695,7 @@ __global__ void __launch_bounds__(64) k_group_total(const XYZZ<F>* __restrict__ 
 
 // ---- 5b: the reduction above level 0 when there are FEW groups (one-shot MSMs: groups = windows) -------------------------
 // Levels 1.. of k_reduce_level then run a few thousand threads that each walk ~23 additions and up to 12 doublings in sequence:
-// four such levels were 0.7 of the 5.3 ms of a 2^20-point G1 MSM and 2 of the 6 ms of a 2^18-point G2 one.  With R_p, T_p the
+// four such levels are a large share of a one-shot 2^20-point G1 or 2^18-point G2 MSM.  With R_p, T_p the
 // level-0 sums of chunk p (2^f buckets each) a group's total is  sum_p (T_p + R_p) + 2^f sum_p p R_p,  and the weighted part
 // is taken bit by bit:  sum_p p R_p = sum_k 2^k Q_k,  Q_k = sum of the R_p whose index has bit k set.  The two plain sums and the
 // log2(n1) sums Q_k are independent tree reductions (one CTA each: a few strided additions per thread, then log2(threads) levels
@@ -822,8 +817,8 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
         uint32_t n_out = (n_in + (1u << fan_log2) - 1) >> fan_log2;
         uint32_t threads = n_groups * n_out;
         const char* rn = sizeof(F) == 32 ? "k_reduce_level_g1" : "k_reduce_level_g2";
-        // G1: running sums in registers, group operations out of line; G2: running sums in shared memory (profiles/r2_small_ab.md;
-        // the losing combination of each was removed from the library after the measurement)
+        // G1: running sums in registers, group operations out of line; G2: running sums in shared memory (the losing
+        // combination of each was removed from the library)
         if constexpr (RED_SM_DEFAULT<F>) {
             if (U_in) { auto k = k_reduce_level_sm<F, true>; OG_LAUNCHN(ctx, rn, k, (threads + 63) / 64, 64, 0, S_in, U_in, n_in, n_out, n_groups, w_log2, fan_log2, bufS[pp], bufU[pp]); }
             else { auto k = k_reduce_level_sm<F, false>; OG_LAUNCHN(ctx, rn, k, (threads + 63) / 64, 64, 0, S_in, U_in, n_in, n_out, n_groups, w_log2, fan_log2, bufS[pp], bufU[pp]); }
@@ -886,7 +881,7 @@ size_t msm_aff_scratch_bytes_g2(uint64_t) { return 0; }
 
 // ---- 6: one-shot MSM = Horner over the window totals ------------------------------------------------------
 // sum_w 2^(c w) T_w needs c (W - 1) ~ 240 SEQUENTIAL doublings whatever the order, and one thread's multiplier issues a
-// product every ~630 cycles, so round 1's single-thread Horner cost 0.7 ms (G1) / 2.2 ms (G2) of every one-shot MSM.
+// product every ~630 cycles, so a single-thread Horner is a visible share of every one-shot MSM.
 // The nine products of an XYZZ doubling form three dependency levels of (2, 4, 3) independent products; four warps -- which
 // sit on the SM's four schedulers -- take one product each per level and meet at barriers:
 //   level 1: v = (2y)^2, xx = x^2     level 2: w = 2y v, s = x v, mm = (3xx)^2, zz' = v zz
@@ -954,8 +949,8 @@ __global__ void __launch_bounds__(128) k_horner(const XYZZ<F>* __restrict__ tota
 #ifdef OG_MSM_G1
 // GLV front end of the one-shot G1 MSM (glv.cuh): (P_i, k_i) -> (+-P_i, |k1_i|) at index i and (+-phi(P_i), |k2_i|) at index n + i;
 // the signs go into the points.  phi(P_i) is MATERIALISED: applying beta at fetch time instead (entries >= n standing for phi of
-// point index - n, signs in the scalars) keeps the table at 64 MB but costs a product per phi entry in the accumulation kernel and
-// measured 3.61 vs 3.27 ms of accumulation at 2^20 points (profiles/r2_msm_oneshot_breakdown.md)
+// point index - n, signs in the scalars) keeps the table at 64 MB but costs a product per phi entry in the accumulation kernel,
+// which made the accumulation slower
 __global__ void __launch_bounds__(128) k_glv_expand(const uint8_t* __restrict__ scalars, uint64_t n, Fq beta, Affine<Fq>* __restrict__ pts,
                                                     uint32_t* __restrict__ sc2, int* flag) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -40,7 +40,7 @@ int32_t msm_buckets_g2(og_ctx* ctx, const G2Affine* d_table, const uint32_t* d_s
                        const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, G2XYZZ* d_buckets,
                        G2XYZZ* d_lvl, uint32_t* d_heavy, uint32_t* d_perm, G2XYZZ* d_totals, void* aff_scratch = nullptr);
 // aff_scratch: experiment builds only (-DOG_EXPERIMENT_AFFINE): non-null selects the rejected batched-affine accumulation
-// (csrc/experiments/bucket_affine.cuh, profiles/r2_affine_ab.md); the shipped library ignores it and the sizes are 0
+// (csrc/experiments/bucket_affine.cuh); the shipped library ignores it and the sizes are 0
 size_t msm_aff_scratch_bytes_g1(uint64_t n_keys);
 size_t msm_aff_scratch_bytes_g2(uint64_t n_keys);
 static inline size_t msm_lvl_elems(uint32_t n_groups, uint32_t nb) { return 4 * ((size_t)n_groups * ((nb + 7) / 8) + 16); }   // RED_FAN = 8

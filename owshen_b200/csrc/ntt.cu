@@ -1,4 +1,4 @@
-// owshen_b200/csrc/ntt.cu -- batched radix-2 NTT over BN254 Fr for sm_100a.
+// owshen_b200/csrc/ntt.cu -- batched radix-2 NTT over BN254 Fr for sm_90a.
 //
 // No counterpart in the reference (SURVEY.md section 0); convention follows its field generator 7
 // (/root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:9): omega_n = 7^((r-1)/n),
@@ -84,10 +84,10 @@ __device__ __forceinline__ uint32_t bitrev(uint32_t x, uint32_t bits) { return _
 
 // ---- the pass kernel ------------------------------------------------------------------------------------
 // Three things taken from the ncu capture of the first version (one level per barrier, plain array-of-structures
-// tile; profiles/r1_*; its code was removed in round 2): (1) two butterfly levels per
+// tile; its code was removed): (1) two butterfly levels per
 // barrier with the four operands in registers (half the shared-memory round trips and barriers); (2) the 32-byte
 // elements are stored as two 16-byte chunks whose position is XOR-swizzled with bit 2 of the element index, which
-// removes the 2-way bank conflict of the plain array-of-structures layout (58 % of the wavefronts were replays);
+// removes the 2-way bank conflict of the plain array-of-structures layout;
 // (3) the first level of the first pass has twiddle 1 everywhere and skips its products.
 __device__ __forceinline__ uint32_t sw_chunk(uint32_t e, uint32_t h) { return ((e << 1) | h) ^ ((e >> 2) & 1); }
 __device__ __forceinline__ Fr sm_get(const uint4* sm, uint32_t e) {
@@ -105,8 +105,7 @@ __device__ __forceinline__ void sm_put(uint4* sm, uint32_t e, const Fr& v) {
 // non-first passes a tile is made of 256-byte runs of 8 consecutive elements -- so when the PREVIOUS pass stores those
 // elements with their halves swapped, the tile in shared memory is a byte-for-byte copy of its runs in global memory, and
 // one warp can fetch it with 256-byte cp.async.bulk copies that complete on an mbarrier while no thread issues a load.
-// 3 resident CTAs of 256 threads per SM (80 registers): measured 35.7 -> 31.9 ms per 1024 proofs against 2 CTAs,
-// 4 CTAs (64 registers) was equal
+// 3 resident CTAs of 256 threads per SM (80 registers): faster than 2 CTAs; 4 CTAs (64 registers) was no faster
 __global__ void __launch_bounds__(256, 3) k_ntt_pass2(PassPlan P, const Fr* __restrict__ in, Fr* __restrict__ out,
                                                    const Fr* __restrict__ t2, const Fr* __restrict__ t2n, Fr n_inv) {
     extern __shared__ __align__(32) unsigned char smem_raw[];
@@ -278,8 +277,8 @@ int32_t ntt_mont_dev(og_ctx* ctx, Fr* data, Fr* tmp, uint32_t log_n, uint32_t ba
         plans[np++] = p;
     }
     plans[np - 1].last = 1;
-    // OG_NTT_TMA=1: intermediates pre-swizzled + TMA bulk tile loads in the non-first passes.  Measured equal in the prover (32.4 vs
-    // 32.4 ms per step) and 0.6-3.6 % slower standalone (profiles/r2_ntt_tma_ab.md), hence not the default
+    // OG_NTT_TMA=1: intermediates pre-swizzled + TMA bulk tile loads in the non-first passes.  No faster than plain loads in
+    // the prover and slower standalone, hence not the default
     const int use_tma = [] { const char* e = getenv("OG_NTT_TMA"); return e ? atoi(e) : 0; }();     // read per call: tests toggle it
     for (int i = 0; i < np; i++) plans[i].tma = (use_tma && np > 1) ? 1 : 0;
     for (int i = 0; i < np; i++) {

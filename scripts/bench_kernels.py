@@ -5,10 +5,10 @@
   NTT       2^20 forward, and the prover's shape (3072 x 2^15)
 Inputs are resident in HBM (the `_dev` C-ABI entry points), timing is CUDA events on the library stream,
 W warm-ups then K timed repetitions; inputs exceed or are re-generated so L2 does not serve them warm
-(each repetition streams > 126 MB of scratch through L2 for the MSM/NTT; config 2 flushes explicitly).
+(each repetition streams more scratch than the 50 MB L2 holds through L2 for the MSM/NTT; config 2 flushes explicitly).
 Every line reports the algorithmic HBM fraction SURVEY.md section 8d asks for AND the integer-pipe
 fraction (32x32->64 multiply-adds per second against og_int_pipe_peaks), which is the bound that binds.
-Usage: python scripts/bench_kernels.py [--reps K] > profiles/rNN_kernels.jsonl
+Usage: python scripts/bench_kernels.py [--reps K] > kernels.jsonl
 """
 import argparse
 import json
@@ -30,7 +30,7 @@ def hbm_peak():
     try:
         return float(json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "nominal"      # H100 SXM data sheet (HBM3)
 
 
 def fr_bytes(rng, n):
@@ -143,7 +143,7 @@ def main():
             line(f"msm_{curve}_2^{log_n}_{kind} (config 3)", ms, per_pair * n, muls,
                  {"points_per_s": n / (ms * 1e-3), "window_bits": c, "windows": windows,
                   "kernels_ms_one_run": {k: round(v[1], 3) for k, v in sorted(prof.items(), key=lambda kv: -kv[1][1])[:8]},
-                  "l2": "sorted digit lists + buckets (> 126 MB) stream through L2 every repetition"})
+                  "l2": "sorted digit lists + buckets (> 50 MB) stream through L2 every repetition"})
 
     # ---- NTT ------------------------------------------------------------------------------------
     for log_n, batch in ((20, 1), (15, 3072), (24, 1)):

@@ -1,5 +1,5 @@
 #!/bin/bash
-# re-entry sanity run of HEAD on a fresh B200: gpu tests, smoke, bench (both arms)
+# sanity run of HEAD: gpu tests, smoke, bench (both arms)
 mkdir -p gpurun_out/c20
 python -m pytest tests -m gpu -x -q > gpurun_out/c20/gputest.log 2>&1; echo "pytest rc=$?" >> gpurun_out/c20/gputest.log
 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/c20/smoke.log 2>&1; echo "smoke rc=$?" >> gpurun_out/c20/smoke.log

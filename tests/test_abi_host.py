@@ -29,6 +29,17 @@ def test_every_declared_symbol_is_exported():
     assert L.og_abi_version() == 1
 
 
+def test_library_is_built_for_sm90a_only():
+    """The kernels are compiled for the H100 (sm_90a) and nothing else: code for another architecture does not load
+    there, and a stale build for one would fail only at the first kernel launch."""
+    import shutil
+    import subprocess
+    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    out = subprocess.run([tool, "--list-elf", api._LIB_PATH], capture_output=True, text=True, check=True).stdout
+    archs = set(re.findall(r"\.(sm_\w+)\.cubin", out))
+    assert archs == {"sm_90a"}, out
+
+
 def test_header_prototypes_match_the_ctypes_mirror():
     """Parameter counts (and pointer-ness of every parameter) of include/owshen_b200.h against api.ABI_SYMBOLS:
     a drifted mirror would pass garbage across the boundary without any loader error."""

@@ -1,9 +1,10 @@
-"""bench.py's reference arm runs on the CPU: check its one-line JSON contract here (the GPU arm's line is checked
-by the driver on the GPU box)."""
+"""bench.py's reference arm runs on the CPU: check its one-line JSON contract here (the GPU arm needs an H100)."""
 import json
 import os
 import subprocess
 import sys
+
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -27,14 +28,32 @@ def test_reference_arm_other_ranks_exit_quietly():
     assert out.returncode == 0 and out.stdout.strip() == ""
 
 
+@pytest.mark.gpu
+def test_gpu_arm_dump_outputs(tmp_path):
+    """--dump-outputs writes what the last timed step returned (proofs, public inputs) and the sharded MSM sums as float32
+    .npy files of byte values; --steps sets the number of timed steps."""
+    import numpy as np
+    out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", "2", "--warmup", "1",
+                          "--batch", "4", "--no-cpu-baseline", "--no-parity", "--sharded-log-n", "12", "--dump-outputs", str(tmp_path)],
+                         capture_output=True, text=True, timeout=900, cwd=ROOT)
+    assert out.returncode == 0, out.stderr[-2000:]
+    line = json.loads(out.stdout.strip().splitlines()[-1])
+    assert line["steps"] == 2 and line["config"]["proofs_verify"] and line["sharded_msm"]["steps"] == 2
+    shapes = {"proofs": (4, 256), "public_inputs": (4, 96), "sharded_msm_g1": (64,), "sharded_msm_g2": (128,)}
+    for name, shape in shapes.items():
+        a = np.load(tmp_path / f"{name}.npy")
+        assert a.dtype == np.float32 and a.shape == shape, name
+        assert np.all((a >= 0) & (a <= 255) & (a == np.round(a))) and a.any(), name
+
+
 def test_launch_list_tool_reads_the_committed_ncu_csv(tmp_path):
-    """tools/launch_list_summary.py turns the committed ncu launch list into the table under profiles/: the dominant kernel of
-    the bench command must come out on top (this is the evidence the roofline share is checked against)."""
+    """tools/launch_list_summary.py turns an ncu launch list of the benchmark (the committed fixture under tests/golden/)
+    into a per-kernel table: the dominant kernel of the bench command must come out on top."""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     out = tmp_path / "ll.md"
     subprocess.run([sys.executable, os.path.join(root, "tools", "launch_list_summary.py"),
-                    os.path.join(root, "profiles", "r2_launches_bench_steps2.csv"), str(out), "t"], check=True)
+                    os.path.join(root, "tests", "golden", "ncu_launch_list.csv"), str(out), "t"], check=True)
     rows = [l for l in out.read_text().splitlines() if l.startswith("| `")]
     assert rows and rows[0].startswith("| `k_bucket_acc_sm1"), rows[:2]

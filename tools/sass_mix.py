@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Static SASS instruction mix of the hot kernels of libowshen_b200.so (cuobjdump -sass), as a markdown table:
 IMAD.WIDE (the 32x32->64 multiply-add the integer roofline counts), other IMAD, IADD3, local-memory traffic (LDL/STL =
-spills and stack), shared / global accesses, shuffles, barriers -- and the Blackwell/Hopper-only opcodes (UTMALDG, UBLKCP,
-UTCxMMA, LDTM ...) whose absence or presence the judge asked to see.  Callees that ptxas kept out of line (e.g. the Fq2
+spills and stack), shared / global accesses, shuffles, barriers -- and the opcodes of the Hopper-generation units (TMA:
+UTMALDG, UBLKCP; mbarrier: SYNCS; HGMMA), to show which of them the library uses.  Callees that ptxas kept out of line (e.g. the Fq2
 multiplier of the G2 unit) are listed inside the kernel that contains them, so counts are per kernel image, not per call.
-Usage: python tools/sass_mix.py [lib.so] > profiles/rNN_sass_mix.md"""
+Usage: python tools/sass_mix.py [lib.so] > sass_mix.md"""
 import collections
 import re
 import subprocess
@@ -52,7 +52,7 @@ def main():
                 mix[fn][c] += 1
             if op.startswith(BLACKWELL):
                 bw[op.split(".")[0]] += 1
-    print(f"# SASS instruction mix of the hot kernels ({lib}, sm_100a, static counts per kernel image)\n")
+    print(f"# SASS instruction mix of the hot kernels ({lib}, sm_90a, static counts per kernel image)\n")
     print("| kernel | " + " | ".join(COLS) + " |")
     print("|---|" + "---|" * len(COLS))
     for fn in sorted(mix):
@@ -62,10 +62,10 @@ def main():
         print(f"| `{short}` | " + " | ".join(str(mix[fn][c]) for c in COLS) + " |")
     print()
     if bw:
-        print("Blackwell/Hopper-only opcodes present: " + ", ".join(f"{k} x{v}" for k, v in sorted(bw.items())))
+        print("TMA / mbarrier / wgmma opcodes present: " + ", ".join(f"{k} x{v}" for k, v in sorted(bw.items())))
     else:
-        print("Blackwell/Hopper-only opcodes (UTMALDG, UTMASTG, UBLKCP, UTC*MMA, LDTM/STTM, SYNCS, HGMMA): **none in the library** -- "
-              "no TMA, no tcgen05: the hot path is 256-bit modular integer arithmetic with 32/64-byte gathers (DESIGN.md 5, 8).")
+        print("TMA / mbarrier / wgmma opcodes (UTMALDG, UTMASTG, UBLKCP, SYNCS, HGMMA): **none in the library** -- "
+              "the hot path is 256-bit modular integer arithmetic with 32/64-byte gathers (DESIGN.md 5).")
 
 
 if __name__ == "__main__":
