@@ -811,7 +811,7 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
     int pp = 0;
     // level 0 (raw buckets) is most of the work: a wider fan there spends fewer additions per bucket (2 - 1/fan)
     // and leaves less for the levels above, at the price of longer serial chains; OG_RED_FAN0 = 3, 4 or 5
-    static const uint32_t fan0 = [] { const char* v = getenv("OG_RED_FAN0"); int x = v ? atoi(v) : 0; return (uint32_t)(x >= 3 && x <= 5 ? x : RED_FAN_LOG2); }();
+    const uint32_t fan0 = [] { const char* v = getenv("OG_RED_FAN0"); int x = v ? atoi(v) : 0; return (uint32_t)(x >= 3 && x <= 5 ? x : RED_FAN_LOG2); }();   // read per call: tests toggle it
     do {
         uint32_t fan_log2 = U_in ? RED_FAN_LOG2 : fan0;
         uint32_t n_out = (n_in + (1u << fan_log2) - 1) >> fan_log2;
@@ -832,7 +832,7 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
         w_log2 += fan_log2;
         if (few_groups && w_log2 == fan_log2 && n_in >= 64 && (n_in & (n_in - 1)) == 0) {
             // one-shot MSM: everything above level 0 as independent tree sums + one Horner per group (5b above)
-            static const bool tail = [] { const char* v = getenv("OG_MSM_TAIL"); return !(v && v[0] == '0' && v[1] == 0); }();
+            const bool tail = [] { const char* v = getenv("OG_MSM_TAIL"); return !(v && v[0] == '0' && v[1] == 0); }();   // read per call: tests toggle it
             if (tail) {
                 uint32_t n_bits = 0;
                 while ((1u << n_bits) < n_in) n_bits++;
@@ -996,7 +996,7 @@ static int32_t msm_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_sc
     if (n == 0) { OG_CUDA(ctx, cudaMemsetAsync(d_out, 0, PB, ctx->stream)); return OG_OK; }
     // G1: GLV halves the scalar length (2n points, 127-bit scalars): same bucket additions, half the windows to reduce and half
     // the sequential doublings of the Horner (OG_GLV=0 switches it off for A/B)
-    static const bool glv_on = [] { const char* v = getenv("OG_GLV"); return !(v && v[0] == '0' && v[1] == 0); }();
+    const bool glv_on = [] { const char* v = getenv("OG_GLV"); return !(v && v[0] == '0' && v[1] == 0); }();   // read per call: tests toggle it
     const bool glv = sizeof(F) == 32 && glv_on && n >= 1024;
     const uint64_t n_in = n;
     if (glv) n = 2 * n;

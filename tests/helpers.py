@@ -22,6 +22,25 @@ def pk_blob(cs, pkb: dict, depth: int) -> bytes:
     return blob
 
 
+_KEYS32 = None
+
+
+def withdraw_keys32(ctx):
+    """Depth-32 withdraw keys from the library's setup and from the oracle's: (pk, vk, r1cs, oracle pk bytes, oracle vk bytes).
+    Made once per process, so every module that proves at depth 32 shares one setup."""
+    global _KEYS32
+    if _KEYS32 is None:
+        import owshen_b200 as ob
+        from oracle import withdraw_circuit as wc
+        rng = random.Random(10)
+        tw = [rng.randrange(1, R) for _ in range(5)]
+        pk, vk = ob.setup_withdraw(ctx, 32, *tw)
+        cs = wc.build_r1cs(32)
+        pkb, vkb = cport.setup_bytes(cs, *tw)
+        _KEYS32 = (pk, vk, cs, pkb, vkb)
+    return _KEYS32
+
+
 def rand_inputs(rng: random.Random, batch: int, depth: int):
     nul = cport.frs([rng.randrange(R) for _ in range(batch)])
     sec = cport.frs([rng.randrange(R) for _ in range(batch)])

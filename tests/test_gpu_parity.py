@@ -12,7 +12,7 @@ from owshen_b200 import api
 from oracle import bn254 as bn
 from oracle import cport, mimc7
 from oracle import withdraw_circuit as wc
-from tests.helpers import pk_blob, rand_fr_bytes, rand_g1, rand_g2, rand_inputs, vk_blob
+from tests.helpers import pk_blob, rand_fr_bytes, rand_g1, rand_g2, rand_inputs, vk_blob, withdraw_keys32
 
 pytestmark = pytest.mark.gpu
 R, P = bn.R, bn.P
@@ -264,12 +264,7 @@ def test_withdraw_witness(ctx):
 
 @pytest.fixture(scope="module")
 def keys32(ctx):
-    rng = random.Random(10)
-    tw = [rng.randrange(1, R) for _ in range(5)]
-    pk, vk = ob.setup_withdraw(ctx, 32, *tw)
-    cs = wc.build_r1cs(32)
-    pkb, vkb = cport.setup_bytes(cs, *tw)
-    return pk, vk, cs, pkb, vkb
+    return withdraw_keys32(ctx)
 
 
 def test_setup_matches_oracle(ctx, keys32):
