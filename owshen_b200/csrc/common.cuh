@@ -44,7 +44,6 @@ struct og_ctx {
     void* g1_fixed = nullptr;        // fixed-base tables of the generators (setup only)
     void* g2_fixed = nullptr;
     void* bjj_fixed = nullptr;       // window multiples of the BabyJubJub BASE (bjj_impl.cuh)
-    bool digits_smem_opt_in = false; // cudaFuncSetAttribute(k_digits_count_tiled) done for this device
 
     // optional per-kernel timing: CUDA events around every launch of this library (og_profile)
     bool prof_on = false;
@@ -103,6 +102,7 @@ enum Slot {
     // lane 1 copies of the per-chunk prover scratch (same order as S_PR_ABC .. S_PR_HEAVY) and of S_MSM_MISC
     S_L1_ABC, S_L1_SCALARS, S_L1_SORTED, S_L1_COUNTS, S_L1_OFFSETS, S_L1_CURSOR, S_L1_BUCKETS, S_L1_SEG, S_L1_HEAVY, S_L1_MSM_MISC,
     S_PR_AFF, S_L1_AFF, S_MSM_AFF,
+    S_PR_SORT_STAGE, S_L1_SORT_STAGE, S_PR_SORT_TILES, S_L1_SORT_TILES,   // only for keys whose sort scratch outgrows bk2 / heavy
     S_COUNT
 };
 static_assert(S_COUNT <= N_SLOTS, "grow N_SLOTS");

@@ -330,6 +330,7 @@ void pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m
 struct ChunkBufs {
     Fr *W, *rs_m, *abc, *ntt_tmp, *bsc, *csc;
     uint32_t *counts, *offsets, *cursor, *sorted, *heavy;
+    uint32_t *sort_stage, *sort_tiles;    // scratch of the digit sort (msm.cuh): inside bk2 and heavy unless a key outgrows them
     G1XYZZ *bk1, *lvl1, *totA, *totC;
     G2XYZZ *bk2, *lvl2, *totB;
     void *aff1, *aff2;                    // batched-affine scratch (nullptr = XYZZ accumulation): G1 MSMs / G2 MSM
@@ -379,6 +380,15 @@ static int32_t alloc_chunk(og_ctx* ctx, const og_pk* pk, uint32_t batch, uint32_
     }
     b.ntt_tmp = b.abc + (size_t)B * 3 * m;
     b.csc = b.bsc + (size_t)B * b.bsc_stride;
+    // The sort's staging lives in the bucket array: nothing writes it before the accumulation of the same MSM, and the
+    // previous MSM's reduction, which reads it, runs earlier on the same stream.  Its per-tile counters live in the heavy-bucket
+    // scratch, which msm_buckets uses only after the sort.
+    const uint32_t n_pts[3] = {pk->nA, pk->nB, pk->nC};
+    size_t stage = msm_sort_stage_bytes((size_t)B * max_pts * pk->max_windows), tiles = 0;
+    for (int k = 0; k < 3; k++) { size_t t = msm_sort_tile_bytes(B, pk->nb[k], n_pts[k]); if (t > tiles) tiles = t; }
+    b.sort_stage = stage <= sizeof(G2XYZZ) * n_keys ? (uint32_t*)b.bk2 : (uint32_t*)ctx->slot(S(S_PR_SORT_STAGE, S_L1_SORT_STAGE), stage);
+    b.sort_tiles = tiles <= 4 * (2 * n_keys + 4) ? b.heavy : (uint32_t*)ctx->slot(S(S_PR_SORT_TILES, S_L1_SORT_TILES), tiles);
+    if (!b.sort_stage || !b.sort_tiles) return OG_E_NOMEM;
     b.bk1 = reinterpret_cast<G1XYZZ*>(b.bk2);       // the G1 and G2 MSMs of a chunk run one after another
     b.lvl1 = reinterpret_cast<G1XYZZ*>(b.lvl2);
     b.totC = b.totA + batch;
@@ -395,7 +405,7 @@ static int32_t run_msm_g1(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
     plan.key_stride_problem = 1; plan.key_stride_window = 0; plan.tidx_window_stride = n_pts;
     plan.montgomery = 1;
     uint32_t n_keys = B * pk->nb[which];
-    OG_TRY(msm_sort_digits(ctx, plan, n_keys, b.counts, b.offsets, b.cursor, b.sorted));
+    OG_TRY(msm_sort_digits(ctx, plan, n_keys, b.counts, b.offsets, nullptr, b.sorted, b.sort_stage, b.sort_tiles));
     return msm_buckets_g1(ctx, table, b.sorted, b.offsets, b.counts, B, pk->nb[which], (uint64_t)B * n_pts * pk->n_windows[which], b.bk1, b.lvl1, b.heavy, b.cursor, totals, b.aff1);
 }
 static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b, uint32_t B, const G2Affine* table, uint32_t n_pts,
@@ -407,7 +417,7 @@ static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
     plan.key_stride_problem = 1; plan.key_stride_window = 0; plan.tidx_window_stride = n_pts;
     plan.montgomery = 1;
     uint32_t n_keys = B * pk->nb[which];
-    OG_TRY(msm_sort_digits(ctx, plan, n_keys, b.counts, b.offsets, b.cursor, b.sorted));
+    OG_TRY(msm_sort_digits(ctx, plan, n_keys, b.counts, b.offsets, nullptr, b.sorted, b.sort_stage, b.sort_tiles));
     return msm_buckets_g2(ctx, table, b.sorted, b.offsets, b.counts, B, pk->nb[which], (uint64_t)B * n_pts * pk->n_windows[which], b.bk2, b.lvl2, b.heavy, b.cursor, totals, b.aff2);
 }
 

@@ -5,6 +5,8 @@
 //   1. k_digits<false>   signed c-bit digits of every scalar, histogram of (group, bucket) keys
 //   2. k_scan            exclusive prefix sum of the histogram
 //   3. k_digits<true>    counting-sort scatter of (point index, sign) entries  -> coalesced bucket lists
+//      (the batched prover sorts with a two-pass partitioned counting sort instead: k_sort_part_count, k_sort_part_scatter,
+//      k_sort_local)
 //   4. k_bucket_acc      one thread per bucket: XYZZ += affine point (8M+2S), accumulator in registers
 //      k_bucket_heavy    buckets above a cap get a whole CTA (witness-like scalars: 0/1 pile-ups)
 //   5. k_reduce_level    sum_b (b+1) B_b by 32-way running sums, log_32(nb) levels
@@ -104,9 +106,34 @@ struct DigitIter {
         s[8] = 0;
         return (s[0] | s[1] | s[2] | s[3] | s[4] | s[5] | s[6] | s[7]) != 0;
     }
-    // calls f(window, magnitude - 1, negative) for every non-zero signed digit
+    __device__ __forceinline__ void clear() {
+#pragma unroll
+        for (int j = 0; j < 9; j++) s[j] = 0;
+    }
+    // load() in two halves, so that a loop can issue the next scalar's loads before it works on the current one
+    // (32-byte aligned scalars: the prover's Fr vectors)
+    static __device__ __forceinline__ void fetch(const DigitPlan& P, uint32_t prob, uint64_t i, uint32_t raw[8]) {
+        const uint4* sp = reinterpret_cast<const uint4*>(P.scalars + ((uint64_t)prob * P.scalar_stride + i) * 8);
+        const uint4 a = sp[0], b = sp[1];
+        raw[0] = a.x; raw[1] = a.y; raw[2] = a.z; raw[3] = a.w; raw[4] = b.x; raw[5] = b.y; raw[6] = b.z; raw[7] = b.w;
+    }
+    __device__ __forceinline__ bool from_raw(const DigitPlan& P, const uint32_t raw[8], int* flag) {
+        if (P.montgomery) {
+            Fr v;
+#pragma unroll
+            for (int j = 0; j < 8; j++) v.l[j] = raw[j];
+            v.to_canonical(s);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 8; j++) s[j] = raw[j];
+            if (!Fr::canonical_lt_mod(s)) { atomicOr(flag, 1); return false; }
+        }
+        s[8] = 0;
+        return (s[0] | s[1] | s[2] | s[3] | s[4] | s[5] | s[6] | s[7]) != 0;
+    }
+    // calls f(window, magnitude, negative) for every window, zero digits included
     template <class Fn>
-    __device__ __forceinline__ void for_each(const DigitPlan& P, Fn f) const {
+    __device__ __forceinline__ void windows(const DigitPlan& P, Fn f) const {
         const uint32_t c = P.c, half = 1u << (c - 1), mask = (1u << c) - 1;
         uint32_t carry = 0;
         for (uint32_t w = 0; w < P.n_windows; w++) {
@@ -116,8 +143,13 @@ struct DigitIter {
             uint32_t neg = v > half;
             uint32_t mag = neg ? (1u << c) - v : v;
             carry = neg;
-            if (mag) f(w, mag - 1, neg);
+            f(w, mag, neg);
         }
+    }
+    // calls f(window, magnitude - 1, negative) for every non-zero signed digit
+    template <class Fn>
+    __device__ __forceinline__ void for_each(const DigitPlan& P, Fn f) const {
+        windows(P, [&](uint32_t w, uint32_t mag, uint32_t neg) { if (mag) f(w, mag - 1, neg); });
     }
 };
 
@@ -141,28 +173,6 @@ __global__ void __launch_bounds__(256) k_digits(DigitPlan P, uint32_t* __restric
             sorted[pos] = (((uint32_t)i + w * P.tidx_window_stride) << 1) | neg;
         }
     });
-}
-
-// Tiled histogram for the batched prover (one group per proof, nb <= 32768): a CTA owns a tile of one problem's
-// scalars, counts its digits in shared memory and touches global memory once per bucket instead of once per
-// digit.  The scatter stays the plain k_digits<true>: a tiled scatter with run reservation and a one-CTA-per-proof
-// shared-memory sort were both slower and were removed.
-constexpr uint32_t DIG_TILE = 4096, DIG_THREADS = 256, DIG_MAX_NB_COUNT = 32768;
-
-__global__ void __launch_bounds__(DIG_THREADS) k_digits_count_tiled(DigitPlan P, uint32_t* __restrict__ counts, int* flag) {
-    extern __shared__ uint32_t hist[];                    // nb counters (dynamic: up to 128 KB)
-    const uint32_t prob = blockIdx.y, nb = P.nb;
-    const uint64_t lo = (uint64_t)blockIdx.x * DIG_TILE;
-    const uint64_t hi = lo + DIG_TILE < P.n ? lo + DIG_TILE : P.n;
-    const uint32_t key0 = prob * P.key_stride_problem * nb;          // key_stride_window == 0 in this mode
-    for (uint32_t b = threadIdx.x; b < nb; b += DIG_THREADS) hist[b] = 0;
-    __syncthreads();
-    for (uint64_t i = lo + threadIdx.x; i < hi; i += DIG_THREADS) {
-        DigitIter it;
-        if (it.load(P, prob, i, flag)) it.for_each(P, [&](uint32_t, uint32_t b, uint32_t) { atomicAdd(&hist[b], 1u); });
-    }
-    __syncthreads();
-    for (uint32_t b = threadIdx.x; b < nb; b += DIG_THREADS) if (hist[b]) atomicAdd(&counts[key0 + b], hist[b]);
 }
 
 // ---- 2: exclusive scan: tile sums -> scan of the tile sums (one CTA) -> tile rescan with offsets ----------
@@ -221,34 +231,214 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_apply(const uint32_t* __r
     uint32_t run = tile_sums[blockIdx.x] + block_exclusive_scan(s, &total);
 #pragma unroll
     for (uint32_t k = 0; k < SCAN_PER_THREAD; k++) {      // the scatter's cursors start at the offsets: one random access per entry fewer
-        if (base + k < n) { offsets[base + k] = run; cursor[base + k] = run; }
+        if (base + k < n) { offsets[base + k] = run; if (cursor) cursor[base + k] = run; }
         run += c[k];
     }
 }
 
+// offsets[n] receives the grand total; cursor (optional) a copy of the offsets
+static int32_t exclusive_scan(og_ctx* ctx, const uint32_t* d_counts, uint32_t n, uint32_t* d_offsets, uint32_t* d_cursor) {
+    uint32_t n_tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
+    OG_SLOT(ctx, tile_sums, uint32_t, ctx->lane ? S_L1_MSM_MISC : S_MSM_MISC, 4 * (size_t)n_tiles);
+    OG_LAUNCH(ctx, k_scan_tiles, n_tiles, SCAN_THREADS, 0, d_counts, n, tile_sums);
+    OG_LAUNCH(ctx, k_scan_tile_sums, 1, SCAN_THREADS, 0, tile_sums, n_tiles, d_offsets + n);
+    OG_LAUNCH(ctx, k_scan_apply, n_tiles, SCAN_THREADS, 0, d_counts, n, tile_sums, d_offsets, d_cursor);
+    return OG_OK;
+}
+
+// ---- the batched prover's sort (one group per proof): a two-pass partitioned counting sort --------------------------------
+// A scatter with one global cursor atomic per entry into 2^15 buckets per proof waits on L2 atomic round trips and writes
+// 4-byte entries to random places.  Instead each proof's entries are first split into P coarse partitions (the top bits of
+// the bucket id), then every partition is sorted by the remaining bits on its own:
+//   k_sort_part_count    per (tile of SORT_TILE scalars, proof): digits per partition, counted in shared memory
+//   exclusive_scan       of those counts in (proof, partition, tile) order: each (tile, partition) gets a run, and the runs of
+//                        one (proof, partition) are adjacent -- they span that partition's window of the final list
+//   k_sort_part_scatter  the digits again: entry + fine bucket id (bucket mod nb/P, one byte) into the tile's runs of a
+//                        staging array, ranked by shared-memory cursors (no global atomics; runs of ~2 KB for C')
+//   k_sort_local         per (proof, partition): histogram of the fine ids -> counts and offsets of the partition's buckets,
+//                        then the entries into the partition's window of the list (~35 KB for C'), whose stores L2 combines
+// Any digit distribution works: every loop is bounded by the tile or the partition, not by a bin's load, and lanes of a
+// warp that hit the same shared counter add once (a 0/1 witness puts nearly every digit in one bucket).
+// P = 128 and tiles of 4096 scalars were the fastest of the sweep in DESIGN.md section 8.
+constexpr uint32_t SORT_PARTS = 128, SORT_TILE = 4096, SORT_THREADS = 256;
+constexpr uint32_t SORT_MAX_NB = 32768, SORT_MAX_FINE = SORT_MAX_NB / SORT_PARTS;     // c <= 16
+constexpr uint32_t NO_BIN = 0xFFFFFFFFu;
+static_assert(SORT_THREADS == SCAN_THREADS, "k_sort_local scans with block_exclusive_scan");
+static_assert(SORT_PARTS <= SORT_THREADS && SORT_MAX_FINE <= SORT_THREADS && SORT_TILE % SORT_THREADS == 0, "sort shape");
+static_assert(SORT_MAX_FINE <= 256, "fine bucket ids are staged as one byte");
+
+static uint32_t sort_parts(uint32_t nb) { return nb < SORT_PARTS ? nb : SORT_PARTS; }
+static uint32_t sort_shift(uint32_t nb) { uint32_t s = 0; while ((sort_parts(nb) << s) < nb) s++; return s; }
+static uint64_t sort_tiles(uint64_t n) { return (n + SORT_TILE - 1) / SORT_TILE; }
+
+// Called by all 32 lanes of a warp; bin NO_BIN adds nothing.  Returns the lane's slot: the bin's old value plus the lane's
+// rank in the warp.  When every lane with a bin has the same one (skewed digits: a 0/1 witness puts nearly every digit in
+// one bucket), the warp adds with one atomic instead of 32 on one address; otherwise each lane adds its own (cheaper than
+// grouping the lanes by bin with __match_any_sync, which made the uniform case slower).
+__device__ __forceinline__ uint32_t warp_bin_add(uint32_t* bins, uint32_t bin) {
+    const uint32_t lane = threadIdx.x & 31, valid = __ballot_sync(0xffffffffu, bin != NO_BIN);
+    if (!valid) return 0;
+    const uint32_t leader = __ffs(valid) - 1, first = __shfl_sync(0xffffffffu, bin, leader);
+    if (__all_sync(0xffffffffu, bin == NO_BIN || bin == first)) {
+        uint32_t base = 0;
+        if (lane == leader) base = atomicAdd(&bins[first], (uint32_t)__popc(valid));
+        return __shfl_sync(0xffffffffu, base, leader) + __popc(valid & ((1u << lane) - 1));
+    }
+    return bin != NO_BIN ? atomicAdd(&bins[bin], 1u) : 0;
+}
+
+// tile_counts[(proof * parts + partition) * n_tiles + tile]
+__global__ void __launch_bounds__(SORT_THREADS) k_sort_part_count(DigitPlan P, uint32_t shift, uint32_t n_tiles,
+                                                                  uint32_t* __restrict__ tile_counts, int* flag) {
+    __shared__ uint32_t hist[SORT_PARTS];
+    const uint32_t prob = blockIdx.y, tile = blockIdx.x, parts = P.nb >> shift;
+    for (uint32_t p = threadIdx.x; p < parts; p += SORT_THREADS) hist[p] = 0;
+    __syncthreads();
+    const uint64_t lo = (uint64_t)tile * SORT_TILE, hi = lo + SORT_TILE < P.n ? lo + SORT_TILE : P.n;
+    uint32_t raw[8];
+    if (lo + threadIdx.x < hi) DigitIter::fetch(P, prob, lo + threadIdx.x, raw);
+    for (uint64_t i0 = lo; i0 < hi; i0 += SORT_THREADS) {          // the same trip count for every lane: warp_bin_add needs all 32
+        const uint64_t i = i0 + threadIdx.x;
+        DigitIter it;
+        if (!(i < hi && it.from_raw(P, raw, flag))) it.clear();
+        if (i + SORT_THREADS < hi) DigitIter::fetch(P, prob, i + SORT_THREADS, raw);     // in flight while this scalar is cut
+        it.windows(P, [&](uint32_t, uint32_t mag, uint32_t) { warp_bin_add(hist, mag ? (mag - 1) >> shift : NO_BIN); });
+    }
+    __syncthreads();
+    for (uint32_t p = threadIdx.x; p < parts; p += SORT_THREADS) tile_counts[((size_t)prob * parts + p) * n_tiles + tile] = hist[p];
+}
+
+// tile_offs: exclusive scan of tile_counts = where the (proof, partition, tile) run starts in the staging (and in the list).
+// Written straight from the digit loop, every lane's store went to another partition (32 sectors per warp store): the kernel
+// was slower than the atomic scatter it replaces.  So each round of SORT_THREADS scalars (up to SORT_ROUND_WINDOWS windows)
+// is first ordered by partition in shared memory and then copied out: consecutive lanes store consecutive slots of a run.
+constexpr uint32_t SORT_ROUND_WINDOWS = 24, SORT_ROUND = SORT_THREADS * SORT_ROUND_WINDOWS;   // 36 KB per round: 5 CTAs per SM
+__global__ void __launch_bounds__(SORT_THREADS) k_sort_part_scatter(DigitPlan P, uint32_t shift, uint32_t n_tiles,
+                                                                    const uint32_t* __restrict__ tile_offs, uint32_t* __restrict__ stage_e,
+                                                                    uint8_t* __restrict__ stage_f, int* flag) {
+    __shared__ uint32_t sm_e[SORT_ROUND];
+    __shared__ uint16_t sm_b[SORT_ROUND];                           // bucket (< nb <= 2^15)
+    __shared__ uint32_t cnt[SORT_PARTS], lbase[SORT_PARTS], cur[SORT_PARTS];
+    const uint32_t tid = threadIdx.x, prob = blockIdx.y, tile = blockIdx.x, parts = P.nb >> shift, fmask = (1u << shift) - 1;
+    for (uint32_t p = tid; p < parts; p += SORT_THREADS) { cur[p] = tile_offs[((size_t)prob * parts + p) * n_tiles + tile]; cnt[p] = 0; }
+    __syncthreads();
+    const uint64_t lo = (uint64_t)tile * SORT_TILE, hi = lo + SORT_TILE < P.n ? lo + SORT_TILE : P.n;
+    uint32_t raw[8];
+    if (lo + tid < hi) DigitIter::fetch(P, prob, lo + tid, raw);
+    for (uint64_t i0 = lo; i0 < hi; i0 += SORT_THREADS) {
+        const uint64_t i = i0 + tid;
+        DigitIter it;
+        if (!(i < hi && it.from_raw(P, raw, flag))) it.clear();
+        if (i + SORT_THREADS < hi) DigitIter::fetch(P, prob, i + SORT_THREADS, raw);     // in flight during the round
+        for (uint32_t w0 = 0; w0 < P.n_windows; w0 += SORT_ROUND_WINDOWS) {
+            auto bin_of = [&](uint32_t w, uint32_t mag) { return mag && w >= w0 && w < w0 + SORT_ROUND_WINDOWS ? (mag - 1) >> shift : NO_BIN; };
+            it.windows(P, [&](uint32_t w, uint32_t mag, uint32_t) { warp_bin_add(cnt, bin_of(w, mag)); });
+            __syncthreads();
+            uint32_t n_round, b = block_exclusive_scan(tid < parts ? cnt[tid] : 0, &n_round);
+            if (tid < parts) { lbase[tid] = b; cnt[tid] = b; }      // cnt: the round's cursors from here on
+            __syncthreads();
+            it.windows(P, [&](uint32_t w, uint32_t mag, uint32_t neg) {
+                const uint32_t bin = bin_of(w, mag), pos = warp_bin_add(cnt, bin);
+                if (bin != NO_BIN) { sm_e[pos] = (((uint32_t)i + w * P.tidx_window_stride) << 1) | neg; sm_b[pos] = (uint16_t)(mag - 1); }
+            });
+            __syncthreads();
+            for (uint32_t k = tid; k < n_round; k += SORT_THREADS) {
+                const uint32_t bk = sm_b[k], p = bk >> shift, dst = cur[p] + k - lbase[p];
+                stage_e[dst] = sm_e[k];
+                stage_f[dst] = (uint8_t)(bk & fmask);
+            }
+            __syncthreads();
+            if (tid < parts) { cur[tid] += cnt[tid] - lbase[tid]; cnt[tid] = 0; }
+            __syncthreads();
+        }
+    }
+}
+
+// one CTA per (proof, partition) g; its buckets are keys g * 2^shift + f.  A partition of up to SORT_LOCAL_CAP entries is
+// assembled in shared memory and written out in order; a larger one (skewed digits) is scattered straight into the list.
+// Each thread loads SORT_LOCAL_ITEMS entries before it ranks any of them: with one load per rank the kernel waited on
+// memory latency.
+constexpr uint32_t SORT_LOCAL_CAP = 10240;                          // 40 KB (5 CTAs per SM); C' partitions average ~8.7k entries
+constexpr uint32_t SORT_LOCAL_ITEMS = 8, SORT_LOCAL_STEP = SORT_THREADS * SORT_LOCAL_ITEMS;
+__global__ void __launch_bounds__(SORT_THREADS) k_sort_local(const uint32_t* __restrict__ tile_offs, uint32_t n_tiles, uint32_t n_parts,
+                                                             uint32_t shift, const uint32_t* __restrict__ total,
+                                                             const uint32_t* __restrict__ stage_e, const uint8_t* __restrict__ stage_f,
+                                                             uint32_t* __restrict__ counts, uint32_t* __restrict__ offsets,
+                                                             uint32_t* __restrict__ sorted) {
+    __shared__ uint32_t bins[SORT_THREADS];                         // >= SORT_MAX_FINE fine buckets
+    __shared__ uint32_t sm_out[SORT_LOCAL_CAP];
+    const uint32_t g = blockIdx.x, F = 1u << shift, tid = threadIdx.x;
+    const uint32_t start = tile_offs[(size_t)g * n_tiles], end = g + 1 < n_parts ? tile_offs[(size_t)(g + 1) * n_tiles] : *total;
+    if (g + 1 == n_parts && tid == 0) offsets[(size_t)n_parts * F] = end;          // offsets[n_keys] = the total
+    bins[tid] = 0;
+    __syncthreads();
+    for (uint32_t j0 = start; j0 < end; j0 += SORT_LOCAL_STEP) {
+        uint32_t f[SORT_LOCAL_ITEMS];
+#pragma unroll
+        for (uint32_t k = 0; k < SORT_LOCAL_ITEMS; k++) { const uint32_t j = j0 + k * SORT_THREADS + tid; f[k] = j < end ? stage_f[j] : NO_BIN; }
+#pragma unroll
+        for (uint32_t k = 0; k < SORT_LOCAL_ITEMS; k++) warp_bin_add(bins, f[k]);
+    }
+    __syncthreads();
+    const uint32_t c = tid < F ? bins[tid] : 0;
+    uint32_t tot;
+    const uint32_t run = start + block_exclusive_scan(c, &tot);      // (ends with a barrier: every bin has been read)
+    if (tid < F) {
+        const size_t key = (size_t)g * F + tid;
+        counts[key] = c; offsets[key] = run; bins[tid] = run;
+    }
+    __syncthreads();
+    const bool staged = end - start <= SORT_LOCAL_CAP;             // the same for the whole CTA
+    for (uint32_t j0 = start; j0 < end; j0 += SORT_LOCAL_STEP) {
+        uint32_t f[SORT_LOCAL_ITEMS], e[SORT_LOCAL_ITEMS];
+#pragma unroll
+        for (uint32_t k = 0; k < SORT_LOCAL_ITEMS; k++) {
+            const uint32_t j = j0 + k * SORT_THREADS + tid;
+            f[k] = j < end ? stage_f[j] : NO_BIN;
+            e[k] = j < end ? stage_e[j] : 0;
+        }
+#pragma unroll
+        for (uint32_t k = 0; k < SORT_LOCAL_ITEMS; k++) {
+            const uint32_t pos = warp_bin_add(bins, f[k]);
+            if (f[k] != NO_BIN) { if (staged) sm_out[pos - start] = e[k]; else sorted[pos] = e[k]; }
+        }
+    }
+    if (staged) {
+        __syncthreads();
+        for (uint32_t k = tid; k < end - start; k += SORT_THREADS) sorted[start + k] = sm_out[k];
+    }
+}
+
+size_t msm_sort_stage_bytes(uint64_t n_entries) { return 5 * n_entries; }
+size_t msm_sort_tile_bytes(uint32_t n_problems, uint32_t nb, uint64_t n) { return 8 * (size_t)n_problems * sort_parts(nb) * sort_tiles(n) + 4; }
+
 int32_t msm_sort_digits(og_ctx* ctx, const DigitPlan& plan, uint32_t n_keys, uint32_t* d_counts, uint32_t* d_offsets,
-                        uint32_t* d_cursor, uint32_t* d_sorted) {
-    OG_CUDA(ctx, cudaMemsetAsync(d_counts, 0, sizeof(uint32_t) * (size_t)n_keys, ctx->stream));
+                        uint32_t* d_cursor, uint32_t* d_sorted, uint32_t* d_stage, uint32_t* d_tiles) {
     if (plan.n == 0 || plan.n_problems == 0) {
+        OG_CUDA(ctx, cudaMemsetAsync(d_counts, 0, sizeof(uint32_t) * (size_t)n_keys, ctx->stream));
         OG_CUDA(ctx, cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * ((size_t)n_keys + 1), ctx->stream));
         return OG_OK;
     }
-    const bool tiled = plan.key_stride_window == 0 && plan.nb <= DIG_MAX_NB_COUNT;
-    if (tiled && !ctx->digits_smem_opt_in) {      // per device, hence per context
-        OG_CUDA(ctx, cudaFuncSetAttribute(k_digits_count_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * DIG_MAX_NB_COUNT)));
-        ctx->digits_smem_opt_in = true;
+    if (plan.key_stride_window == 0) {            // batched prover: one group per proof
+        if (!d_stage || !d_tiles || plan.key_stride_problem != 1 || plan.nb > SORT_MAX_NB || n_keys != plan.n_problems * plan.nb) return OG_E_INVALID;
+        const uint32_t parts = sort_parts(plan.nb), shift = sort_shift(plan.nb), n_tiles = (uint32_t)sort_tiles(plan.n);
+        const uint32_t n_parts = plan.n_problems * parts, n_runs = n_parts * n_tiles;
+        uint32_t* tile_counts = d_tiles;
+        uint32_t* tile_offs = d_tiles + n_runs;       // n_runs + 1 (the grand total)
+        uint32_t* stage_e = d_stage;
+        uint8_t* stage_f = reinterpret_cast<uint8_t*>(d_stage + (uint64_t)plan.n_problems * plan.n * plan.n_windows);
+        dim3 tgrid(n_tiles, plan.n_problems);
+        OG_LAUNCH(ctx, k_sort_part_count, tgrid, SORT_THREADS, 0, plan, shift, n_tiles, tile_counts, ctx->d_flag);
+        OG_TRY(exclusive_scan(ctx, tile_counts, n_runs, tile_offs, nullptr));
+        OG_LAUNCH(ctx, k_sort_part_scatter, tgrid, SORT_THREADS, 0, plan, shift, n_tiles, tile_offs, stage_e, stage_f, ctx->d_flag);
+        OG_LAUNCH(ctx, k_sort_local, n_parts, SORT_THREADS, 0, tile_offs, n_tiles, n_parts, shift, tile_offs + n_runs, stage_e, stage_f,
+                  d_counts, d_offsets, d_sorted);
+        return OG_OK;
     }
+    OG_CUDA(ctx, cudaMemsetAsync(d_counts, 0, sizeof(uint32_t) * (size_t)n_keys, ctx->stream));
     dim3 grid((unsigned)((plan.n + 255) / 256), plan.n_problems);
-    dim3 tgrid((unsigned)((plan.n + DIG_TILE - 1) / DIG_TILE), plan.n_problems);
-    if (tiled) OG_LAUNCH(ctx, k_digits_count_tiled, tgrid, DIG_THREADS, 4 * (size_t)plan.nb, plan, d_counts, ctx->d_flag);
-    else OG_LAUNCHN(ctx, "k_digits_count", k_digits<false>, grid, 256, 0, plan, d_counts, nullptr, nullptr, nullptr, ctx->d_flag);
-    {   // offsets[n_keys] receives the grand total; cursor[k] = offsets[k] for the scatter
-        uint32_t n_tiles = (n_keys + SCAN_TILE - 1) / SCAN_TILE;
-        OG_SLOT(ctx, tile_sums, uint32_t, ctx->lane ? S_L1_MSM_MISC : S_MSM_MISC, 4 * (size_t)n_tiles);
-        OG_LAUNCH(ctx, k_scan_tiles, n_tiles, SCAN_THREADS, 0, d_counts, n_keys, tile_sums);
-        OG_LAUNCH(ctx, k_scan_tile_sums, 1, SCAN_THREADS, 0, tile_sums, n_tiles, d_offsets + n_keys);
-        OG_LAUNCH(ctx, k_scan_apply, n_tiles, SCAN_THREADS, 0, d_counts, n_keys, tile_sums, d_offsets, d_cursor);
-    }
+    OG_LAUNCHN(ctx, "k_digits_count", k_digits<false>, grid, 256, 0, plan, d_counts, nullptr, nullptr, nullptr, ctx->d_flag);
+    OG_TRY(exclusive_scan(ctx, d_counts, n_keys, d_offsets, d_cursor));
     OG_LAUNCHN(ctx, "k_digits_scatter", k_digits<true>, grid, 256, 0, plan, d_counts, d_offsets, d_cursor, d_sorted, ctx->d_flag);
     return OG_OK;
 }

@@ -24,10 +24,17 @@ struct DigitPlan {
 
 static inline uint32_t msm_windows(uint32_t c) { return (255 + c - 1) / c; }
 
-// counts[n_keys] must be zero on entry; fills counts, offsets (exclusive scan), sorted entries.
-// Returns total number of entries through *d_total (device pointer inside offsets[n_keys]).
+// Fills counts[key], offsets[key] (exclusive scan; offsets[n_keys] = the total number of entries) and sorted[]: the entries
+// of each bucket are contiguous, in no particular order.
+// One-shot MSMs (key_stride_window != 0): d_cursor is n_keys u32 of scratch; d_stage and d_tiles are unused.
+// Batched prover (key_stride_window == 0, key_stride_problem == 1, nb <= 2^15): a partitioned sort that needs
+//   d_stage: msm_sort_stage_bytes(n_problems * n * n_windows) of staging and d_tiles: msm_sort_tile_bytes(n_problems, nb, n);
+//   d_cursor is unused.
 int32_t msm_sort_digits(og_ctx* ctx, const DigitPlan& plan, uint32_t n_keys, uint32_t* d_counts,
-                        uint32_t* d_offsets /* n_keys + 1 */, uint32_t* d_cursor, uint32_t* d_sorted);
+                        uint32_t* d_offsets /* n_keys + 1 */, uint32_t* d_cursor, uint32_t* d_sorted,
+                        uint32_t* d_stage = nullptr, uint32_t* d_tiles = nullptr);
+size_t msm_sort_stage_bytes(uint64_t n_entries);
+size_t msm_sort_tile_bytes(uint32_t n_problems, uint32_t nb, uint64_t n);
 
 // Accumulate every bucket and reduce each group to sum_b (b+1) * bucket_b.
 // d_buckets: n_groups * nb XYZZ scratch; d_lvl: msm_lvl_elems(n_groups, nb) XYZZ scratch;
