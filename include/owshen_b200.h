@@ -163,16 +163,37 @@ int32_t og_withdraw_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifie
                             const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
                             uint32_t batch, uint8_t* witnesses);
 
+/* ---- the deposit statement (DESIGN.md section 3): commitment = MultiMiMC7([nullifier, secret], 0) -- */
+/* public inputs (commitment, depositor); 735 variables, 731 constraints, domain 2^10 */
+int32_t og_deposit_r1cs_info(uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_deposit_r1cs_export(int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU */
+int32_t og_deposit_witness(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* depositors,
+                           uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
  * call with pk_out == NULL to get the sizes. */
 int32_t og_groth16_setup_withdraw(og_ctx* ctx, uint32_t depth, const uint8_t* toxic160,
                                   uint8_t* pk_out, uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len);
+/* The same setup for any R1CS: matrices A, B, C as CSR (row_ptr: n_constraints + 1 entries starting at 0, col < n_vars,
+ * coefficients 32 B canonical), variable 0 = ONE, variables 1..n_pub the public inputs.  The key records depth 0.
+ * OG_E_INVALID for a malformed CSR, n_constraints == 0, n_pub + 1 > n_vars, n_pub > 2^16, a domain above 2^24, or a
+ * tau that puts tau or tau/g in the domain; OG_E_ENCODING for a coefficient >= r.  pk_out == NULL returns the sizes. */
+int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
+                         const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
+                         const uint32_t* b_row_ptr, const uint32_t* b_col, const uint8_t* b_coeffs,
+                         const uint32_t* c_row_ptr, const uint32_t* c_col, const uint8_t* c_coeffs,
+                         const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len);
 /* parse a pk blob, upload it and build the fixed-base window tables in HBM */
 int32_t og_load_pk(og_ctx* ctx, const uint8_t* pk_bytes, uint64_t len, og_pk** out);
 void og_free_pk(og_pk* pk);
 int32_t og_pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m, uint32_t* depth);
+/* window bits of the A (G1), B (G2) and C' (G1) MSMs the key proves with: chosen from the key's size when it was
+ * loaded (OG_WINDOW_BITS / OG_C_A / OG_C_B / OG_C_C override) */
+int32_t og_pk_window_bits(const og_pk* pk, uint32_t* c3);
 
 /* batch of proofs from full witnesses (batch * n_vars * 32 B); rs = batch * (r || s) */
 int32_t og_groth16_prove(og_ctx* ctx, const og_pk* pk, const uint8_t* witnesses, uint32_t batch,
@@ -188,6 +209,15 @@ int32_t og_groth16_prove_withdraw_dev(og_ctx* ctx, const og_pk* pk, const uint8_
                                       const uint8_t* d_secrets, const uint8_t* d_recipients,
                                       const uint8_t* d_siblings, const uint32_t* d_path_bits, uint32_t batch,
                                       const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of deposit proofs from the secret inputs, witness generation on the GPU.  OG_E_INVALID unless the key has the
+ * deposit statement's shape.  public_out (optional): batch * 2 * 32 B = commitment, depositor. */
+int32_t og_groth16_prove_deposit(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets,
+                                 const uint8_t* depositors, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
+                                 uint8_t* public_out);
+/* same with every buffer already in HBM; no synchronisation */
+int32_t og_groth16_prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                     const uint8_t* d_depositors, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
+                                     uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

@@ -80,13 +80,21 @@ _SIGS = {
     "og_withdraw_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_withdraw_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_withdraw_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p]),
+    "og_deposit_r1cs_info": (C.c_int32, [C.POINTER(C.c_uint32)] * 4),
+    "og_deposit_r1cs_export": (C.c_int32, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_deposit_witness": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
+                         + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_load_pk": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]),
     "og_free_pk": (None, [C.c_void_p]),
     "og_pk_info": (C.c_int32, [C.c_void_p] + [C.POINTER(C.c_uint32)] * 4),
+    "og_pk_window_bits": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint32)]),
     "og_groth16_prove": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_withdraw": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_withdraw_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_deposit": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_deposit_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
 }
@@ -365,6 +373,16 @@ class Context:
         _check(lib().og_withdraw_witness(self._h, depth, nullifiers, secrets, recipients, siblings, _bits_array(path_bits), n, out), self)
         return out.raw
 
+    def deposit_witness(self, nullifiers: bytes, secrets: bytes, depositors: bytes) -> bytes:
+        """Full assignments of the deposit statement, n_vars * 32 bytes per deposit, computed on the GPU."""
+        _need(len(nullifiers) % 32 == 0, "deposit_witness: nullifiers must be a multiple of 32 bytes")
+        n = len(nullifiers) // 32
+        _need(len(secrets) == 32 * n and len(depositors) == 32 * n, "deposit_witness: secrets / depositors do not match the batch")
+        nv = deposit_r1cs_info()["n_vars"]
+        out = C.create_string_buffer(32 * n * nv)
+        _check(lib().og_deposit_witness(self._h, nullifiers, secrets, depositors, n, out), self)
+        return out.raw
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -390,6 +408,58 @@ def r1cs_export(depth: int, which: str):
     val = C.create_string_buffer(32 * nnz.value)
     _check(lib().og_withdraw_r1cs_export(depth, w, ptr, col, val, C.byref(nnz)))
     return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+
+
+def deposit_r1cs_info() -> dict:
+    v = [C.c_uint32() for _ in range(4)]
+    _check(lib().og_deposit_r1cs_info(*[C.byref(x) for x in v]))
+    return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+
+
+def deposit_r1cs_export(which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's deposit R1CS."""
+    w = "ABC".index(which)
+    nnz = C.c_uint64()
+    _check(lib().og_deposit_r1cs_export(w, None, None, None, C.byref(nnz)))
+    nc = deposit_r1cs_info()["n_constraints"]
+    ptr = (C.c_uint32 * (nc + 1))()
+    col = (C.c_uint32 * nnz.value)()
+    val = C.create_string_buffer(32 * nnz.value)
+    _check(lib().og_deposit_r1cs_export(w, ptr, col, val, C.byref(nnz)))
+    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+
+
+def setup_r1cs(ctx: Context, n_vars: int, n_pub: int, A, B, C_, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of any R1CS -> (pk_bytes, vk_bytes).  A, B, C_ are (row_ptr, col_idx, coeffs) triples as
+    r1cs_export returns them (coefficients as ints or 32-byte little-endian values); variable 0 is ONE and variables
+    1..n_pub are the public inputs.  The key records depth 0, so it proves through prove_witnesses."""
+    mats = []
+    n_constraints = None
+    for name, M in (("A", A), ("B", B), ("C", C_)):
+        _need(len(M) == 3, f"setup_r1cs: {name} must be a (row_ptr, col_idx, coeffs) triple")
+        ptr, col, val = M
+        _need(len(ptr) >= 2, f"setup_r1cs: {name}.row_ptr needs n_constraints + 1 >= 2 entries")
+        _need(n_constraints is None or len(ptr) == n_constraints + 1, f"setup_r1cs: {name}.row_ptr length differs from A's")
+        n_constraints = len(ptr) - 1
+        _need(len(col) == len(val), f"setup_r1cs: {name}.col_idx and {name}.coeffs differ in length")
+        _need(ptr[-1] == len(col), f"setup_r1cs: {name}.row_ptr ends at {ptr[-1]}, but there are {len(col)} terms")
+        _need(all(0 <= x < 1 << 32 for x in ptr) and all(0 <= x < 1 << 32 for x in col), f"setup_r1cs: {name} indices must be 32-bit")
+        cb = b"".join(bytes(x) if isinstance(x, (bytes, bytearray)) else int(x).to_bytes(32, "little") for x in val)
+        _need(len(cb) == 32 * len(val), f"setup_r1cs: {name} coefficients are 32 bytes each")
+        mats += [(C.c_uint32 * len(ptr))(*ptr), (C.c_uint32 * max(1, len(col)))(*col), cb]
+    toxic = b"".join(fr_bytes(x) for x in (tau, alpha, beta, gamma, delta))
+    pl, vl = C.c_uint64(), C.c_uint64()
+    _check(lib().og_groth16_setup(ctx._h, n_constraints, n_vars, n_pub, *mats, toxic, None, C.byref(pl), None, C.byref(vl)), ctx)
+    pk = C.create_string_buffer(pl.value)
+    vk = C.create_string_buffer(vl.value)
+    _check(lib().og_groth16_setup(ctx._h, n_constraints, n_vars, n_pub, *mats, toxic, pk, C.byref(pl), vk, C.byref(vl)), ctx)
+    return pk.raw[:pl.value], vk.raw[:vl.value]
+
+
+def setup_deposit(ctx: Context, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the deposit statement -> (pk_bytes, vk_bytes): its exported R1CS through setup_r1cs."""
+    info = deposit_r1cs_info()
+    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(deposit_r1cs_export(m) for m in "ABC"), tau, alpha, beta, gamma, delta)
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -426,6 +496,13 @@ class ProvingKey:
         except Exception:
             pass
 
+    @property
+    def window_bits(self):
+        """(A, B, C') window bits of the prover's three MSMs for this key."""
+        c = (C.c_uint32 * 3)()
+        _check(lib().og_pk_window_bits(self._h, c))
+        return tuple(c)
+
     def h_evals(self, witness: bytes) -> bytes:
         _need(len(witness) == 32 * self.n_vars, f"h_evals: a witness is {32 * self.n_vars} bytes")
         out = C.create_string_buffer(32 << self.log_m)
@@ -453,6 +530,19 @@ class ProvingKey:
         pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
         _check(lib().og_groth16_prove_withdraw(self.ctx._h, self._h, _ptr(nullifiers), _ptr(secrets), _ptr(recipients),
                                                _ptr(siblings), _ptr(bits), batch, _ptr(rs), proofs, pub), self.ctx)
+        return proofs.raw, (pub.raw if want_public else None)
+
+    def prove_deposit(self, nullifiers, secrets, depositors, rs, want_public=True):
+        """Batch of deposit proofs from the secret inputs (witness generation on the GPU).  Buffers as in prove_withdraw;
+        returns (proofs, public_inputs) with public inputs (commitment, depositor) per proof."""
+        _need(_blen(rs) is not None and _blen(rs) % 64 == 0, "prove_deposit: rs must be a buffer of 64 bytes (r, s) per proof")
+        batch = _blen(rs) // 64
+        for name, buf in (("nullifiers", nullifiers), ("secrets", secrets), ("depositors", depositors)):
+            _need_len(buf, 32 * batch, f"prove_deposit: {name}")
+        proofs = C.create_string_buffer(PROOF_BYTES * batch)
+        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
+        _check(lib().og_groth16_prove_deposit(self.ctx._h, self._h, _ptr(nullifiers), _ptr(secrets), _ptr(depositors), batch,
+                                              _ptr(rs), proofs, pub), self.ctx)
         return proofs.raw, (pub.raw if want_public else None)
 
 

@@ -3,6 +3,7 @@
 // stream, truly asynchronous when the caller's memory is pinned) and return after the result has
 // landed; `_dev` entry points only enqueue.  No entry point has a CPU implementation.
 #include <stdlib.h>
+#include <new>
 #include "common.cuh"
 #include "groth16.cuh"
 #include "mimc.cuh"
@@ -818,7 +819,61 @@ int32_t og_withdraw_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifie
     return check_flag(ctx);
 }
 
+// ---- deposit statement ----------------------------------------------------------------------------------------
+int32_t og_deposit_r1cs_info(uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    DepositLayout L = DepositLayout::make();
+    if (n_constraints) *n_constraints = L.n_constraints;
+    if (n_vars) *n_vars = L.n_vars;
+    if (n_pub) *n_pub = DEPOSIT_N_PUB;
+    if (log_m) *log_m = groth16_domain_log(L.n_constraints, DEPOSIT_N_PUB);
+    return OG_OK;
+}
+int32_t og_deposit_r1cs_export(int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    if (which < 0 || which > 2 || !nnz) return OG_E_INVALID;
+    R1cs cs = DepositBuilder::build();
+    const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
+    *nnz = M.col.size();
+    if (!row_ptr || !col_idx || !coeffs) return OG_OK;
+    memcpy(row_ptr, M.row_ptr.data(), 4 * M.row_ptr.size());
+    memcpy(col_idx, M.col.data(), 4 * M.col.size());
+    for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
+    return OG_OK;
+}
+int32_t og_deposit_witness(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* depositors, uint32_t batch,
+                           uint8_t* witnesses) {
+    OG_ENTER(ctx);
+    if (!ctx || !nullifiers || !secrets || !depositors || !witnesses) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    DepositLayout L = DepositLayout::make();
+    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32ull * batch);
+    OG_SLOT(ctx, dsx, uint8_t, S_IO_B, 32ull * batch);
+    OG_SLOT(ctx, dd, uint8_t, S_IO_C, 32ull * batch);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dn, nullifiers, 32ull * batch); H2D(ctx, dsx, secrets, 32ull * batch); H2D(ctx, dd, depositors, 32ull * batch);
+    OG_TRY(deposit_witness_bytes_dev(ctx, dn, dsx, dd, batch, dout));
+    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
+    return check_flag(ctx);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
+int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
+                         const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
+                         const uint32_t* b_row_ptr, const uint32_t* b_col, const uint8_t* b_coeffs,
+                         const uint32_t* c_row_ptr, const uint32_t* c_col, const uint8_t* c_coeffs,
+                         const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len) {
+    OG_ENTER(ctx);
+    if (!ctx || !pk_len || !vk_len || ((pk_out || vk_out) && !toxic160)) return OG_E_INVALID;
+    const uint32_t* row_ptr[3] = {a_row_ptr, b_row_ptr, c_row_ptr};
+    const uint32_t* col[3] = {a_col, b_col, c_col};
+    const uint8_t* coeffs[3] = {a_coeffs, b_coeffs, c_coeffs};
+    try {
+        return setup_generic(ctx, n_constraints, n_vars, n_pub, row_ptr, col, coeffs, toxic160, pk_out, pk_len, vk_out, vk_len);
+    } catch (const std::bad_alloc&) {           // a shape whose host-side QAP evaluation does not fit in memory
+        snprintf(ctx->err, sizeof(ctx->err), "setup: host allocation failed");
+        return OG_E_NOMEM;
+    }
+}
 int32_t og_groth16_setup_withdraw(og_ctx* ctx, uint32_t depth, const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len,
                                   uint8_t* vk_out, uint64_t* vk_len) {
     OG_ENTER(ctx);
@@ -834,6 +889,12 @@ void og_free_pk(og_pk* pk) { pk_free(pk); }
 int32_t og_pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m, uint32_t* depth) {
     if (!pk) return OG_E_INVALID;
     pk_info(pk, n_vars, n_pub, log_m, depth);
+    return OG_OK;
+}
+
+int32_t og_pk_window_bits(const og_pk* pk, uint32_t* c3) {
+    if (!pk || !c3) return OG_E_INVALID;
+    pk_window_bits(pk, c3);
     return OG_OK;
 }
 
@@ -885,6 +946,37 @@ int32_t og_groth16_prove_withdraw(og_ctx* ctx, const og_pk* pk, const uint8_t* n
     OG_TRY(prove_withdraw_dev(ctx, pk, dn, dsx, dr, dsib, dbits, batch, drs, dpr, public_out ? dpub : nullptr));
     D2H(ctx, proofs, dpr, 256ull * batch);
     if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * n_pub);
+    return check_flag(ctx);
+}
+
+int32_t og_groth16_prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                     const uint8_t* d_depositors, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
+                                     uint8_t* d_public_out) {
+    OG_ENTER(ctx);
+    if (!ctx || !pk || !d_nullifiers || !d_secrets || !d_depositors || !d_rs || !d_proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    return prove_deposit_dev(ctx, pk, d_nullifiers, d_secrets, d_depositors, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_deposit(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* depositors,
+                                 uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
+    OG_ENTER(ctx);
+    if (!ctx || !pk || !nullifiers || !secrets || !depositors || !rs || !proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    if (!pk_is_deposit(pk)) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32ull * batch);
+    OG_SLOT(ctx, dsx, uint8_t, S_IO_B, 32ull * batch);
+    OG_SLOT(ctx, dd, uint8_t, S_IO_C, 32ull * batch);
+    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
+    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
+    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * DEPOSIT_N_PUB);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dn, nullifiers, 32ull * batch); H2D(ctx, dsx, secrets, 32ull * batch); H2D(ctx, dd, depositors, 32ull * batch);
+    H2D(ctx, drs, rs, 64ull * batch);
+    OG_TRY(prove_deposit_dev(ctx, pk, dn, dsx, dd, batch, drs, dpr, public_out ? dpub : nullptr));
+    D2H(ctx, proofs, dpr, 256ull * batch);
+    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * DEPOSIT_N_PUB);
     return check_flag(ctx);
 }
 

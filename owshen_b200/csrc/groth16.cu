@@ -2,7 +2,8 @@
 // development setup.  The reference has no prover (SURVEY.md section 0); conventions are frozen in
 // DESIGN.md section 4 and checked bit-for-bit against oracle/groth16.py and oracle/cpu.
 //
-// Once per batch:  witness  k_withdraw_witness (mimc.cu): MiMC7 Merkle path + every round value -> W[batch][n_vars+2]
+// Once per batch:  witness  k_withdraw_witness / k_deposit_witness (mimc.cu): every MiMC7 round value -> W[batch][n_vars+2]
+//                  (or full witnesses from the caller)
 // Per chunk of B proofs (default 1024; everything stays in HBM, nothing returns to the host until the proofs):
 //   a, b, c      k_abc: sparse A.w, B.w over the CSR kept in L2, c = a*b
 //   h            3 iNTT + 3 coset NTT (ntt.cu), k_pointwise: d = a'b' - c' written straight into
@@ -220,6 +221,19 @@ static int32_t upload_csr(og_ctx* ctx, Reader& rd, uint32_t n_rows, uint32_t n_v
     return OG_OK;
 }
 
+// The c in [2, 16] that minimises the additions of one proof's fixed-base MSM over n points: n * ceil(255 / c) bucket
+// additions (one per point and window; all windows share one bucket set) plus 2.3 additions per each of the 2^(c-1)
+// buckets in the reduction (DESIGN.md section 5.3).  Costs are compared in tenths, exactly; ties go to the smaller c.
+static uint32_t prover_window_bits(uint32_t n) {
+    uint32_t best = 2;
+    uint64_t best_cost = ~0ull;
+    for (uint32_t c = 2; c <= 16; c++) {
+        uint64_t cost = 10ull * n * msm_windows(c) + 23ull * (1ull << (c - 1));
+        if (cost < best_cost) { best = c; best_cost = cost; }
+    }
+    return best;
+}
+
 void pk_free(og_pk* pk) {
     if (!pk) return;
     if (pk->device >= 0) cudaSetDevice(pk->device);    // the key may outlive the context that loaded it
@@ -250,18 +264,19 @@ int32_t pk_load(og_ctx* ctx, const uint8_t* bytes, uint64_t len, og_pk** out) {
     for (uint32_t i = 0; i < nv; i++)
         if (!all_zero(qb1 + 64ull * i, 64) || !all_zero(qb2 + 128ull * i, 128)) supp.push_back(i);
     pk->n_supp = (uint32_t)supp.size();
-    // 15 bits for A and B, 16 for C' (3x the points): the fastest of the H100 sweep in DESIGN.md section 8;
-    // OG_WINDOW_BITS overrides all three, OG_C_A / OG_C_B / OG_C_C one each
-    const uint32_t dflt[3] = {15, 15, 16};
+    pk->nA = nv + 2; pk->nB = pk->n_supp + 2; pk->nC = n_priv + pk->n_supp + m + 1;
+    // window bits from the key's size (DESIGN.md section 6): 15, 15, 16 for the depth-32 withdraw key, the fastest of the
+    // H100 sweep in section 8.  OG_WINDOW_BITS overrides all three, OG_C_A / OG_C_B / OG_C_C one each.
+    const uint32_t n_pts[3] = {pk->nA, pk->nB, pk->nC};
     const char* names[3] = {"OG_C_A", "OG_C_B", "OG_C_C"};
     for (int k = 0; k < 3; k++) {
-        uint32_t c = env_u32(names[k], env_u32("OG_WINDOW_BITS", dflt[k]));
-        if (c < 2 || c > 16) c = dflt[k];
+        const uint32_t dflt = prover_window_bits(n_pts[k]);
+        uint32_t c = env_u32(names[k], env_u32("OG_WINDOW_BITS", dflt));
+        if (c < 2 || c > 16) c = dflt;
         pk->c[k] = c; pk->n_windows[k] = msm_windows(c); pk->nb[k] = 1u << (c - 1);
         if (pk->nb[k] > pk->max_nb) pk->max_nb = pk->nb[k];
         if (pk->n_windows[k] > pk->max_windows) pk->max_windows = pk->n_windows[k];
     }
-    pk->nA = nv + 2; pk->nB = pk->n_supp + 2; pk->nC = n_priv + pk->n_supp + m + 1;
 
     // assemble the base-point lists in boundary bytes, then convert + extend on the GPU
     std::vector<uint8_t> hA(64ull * pk->nA), hB(128ull * pk->nB), hC(64ull * pk->nC);
@@ -315,6 +330,8 @@ int32_t pk_load(og_ctx* ctx, const uint8_t* bytes, uint64_t len, og_pk** out) {
 }
 
 bool pk_on_device_of(const og_pk* pk, const og_ctx* ctx) { return pk && ctx && pk->device == ctx->device; }
+
+void pk_window_bits(const og_pk* pk, uint32_t* c3) { for (int k = 0; k < 3; k++) c3[k] = pk->c[k]; }
 
 void pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m, uint32_t* depth) {
     if (n_vars) *n_vars = pk->n_vars;
@@ -423,9 +440,12 @@ static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
 
 // where a chunk's witness rows come from
 struct WitnessSource {
-    const uint8_t *d_null = nullptr, *d_sec = nullptr, *d_rec = nullptr, *d_sib = nullptr;   // secret inputs (prove_withdraw)
+    enum Kind { WITHDRAW, DEPOSIT, FULL } kind = FULL;
+    const uint8_t *d_null = nullptr, *d_sec = nullptr;                       // secret inputs (prove_withdraw, prove_deposit)
+    const uint8_t *d_rec = nullptr, *d_sib = nullptr;                        // withdraw: recipients, siblings
     const uint32_t* d_bits = nullptr;
-    const uint8_t* d_wit = nullptr;                                                         // or full witnesses (prove)
+    const uint8_t* d_dep = nullptr;                                          // deposit: depositors
+    const uint8_t* d_wit = nullptr;                                          // or full witnesses (prove)
     uint8_t* d_public = nullptr;
 };
 
@@ -435,13 +455,17 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
     const uint32_t m = 1u << pk->log_m, n_priv = pk->n_vars - pk->n_pub - 1;
     Fr* W = b.W + (size_t)off * b.w_stride;
     Fr* rs_m = b.rs_m + 2 * (size_t)off;
-    if (src.d_wit) {
+    if (src.kind == WitnessSource::FULL) {
         uint64_t tot = (uint64_t)B * pk->n_vars;
         OG_LAUNCH(ctx, k_witness_in, (unsigned)((tot + 127) / 128), 128, 0, src.d_wit + 32ull * off * pk->n_vars, B, pk->n_vars, b.w_stride, W, ctx->d_flag);
     } else {
-        WithdrawLayout L = WithdrawLayout::make(pk->depth);
-        OG_TRY(withdraw_witness_strided_dev(ctx, L, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_rec + 32ull * off,
-                                            src.d_sib + 32ull * off * pk->depth, src.d_bits + off, B, W));
+        if (src.kind == WitnessSource::WITHDRAW) {
+            WithdrawLayout L = WithdrawLayout::make(pk->depth);
+            OG_TRY(withdraw_witness_strided_dev(ctx, L, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_rec + 32ull * off,
+                                                src.d_sib + 32ull * off * pk->depth, src.d_bits + off, B, W));
+        } else {
+            OG_TRY(deposit_witness_strided_dev(ctx, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_dep + 32ull * off, B, W));
+        }
         if (src.d_public) OG_LAUNCH(ctx, k_public_out, (B * pk->n_pub + 127) / 128, 128, 0, W, b.w_stride, B, pk->n_pub, src.d_public + 32ull * off * pk->n_pub);
     }
     OG_LAUNCH(ctx, k_extras, (B + 127) / 128, 128, 0, d_rs + 64ull * off, B, pk->n_vars, b.w_stride, W, rs_m, ctx->d_flag);
@@ -516,13 +540,30 @@ int32_t prove_withdraw_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, 
     WithdrawLayout L = WithdrawLayout::make(pk->depth);
     if (L.n_vars != pk->n_vars) return OG_E_INVALID;
     WitnessSource src;
+    src.kind = WitnessSource::WITHDRAW;
     src.d_null = d_null; src.d_sec = d_sec; src.d_rec = d_rec; src.d_sib = d_sib; src.d_bits = d_bits; src.d_public = d_public;
+    return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
+}
+
+bool pk_is_deposit(const og_pk* pk) {
+    DepositLayout L = DepositLayout::make();
+    return pk->n_vars == L.n_vars && pk->n_pub == DEPOSIT_N_PUB && pk->n_constraints == L.n_constraints;
+}
+
+int32_t prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
+                          const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public) {
+    if (!pk_is_deposit(pk)) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    WitnessSource src;
+    src.kind = WitnessSource::DEPOSIT;
+    src.d_null = d_null; src.d_sec = d_sec; src.d_dep = d_dep; src.d_public = d_public;
     return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
 }
 
 int32_t prove_witness_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs) {
     if (batch == 0) return OG_OK;
     WitnessSource src;
+    src.kind = WitnessSource::FULL;
     src.d_wit = d_wit;
     return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
 }
@@ -547,6 +588,17 @@ int32_t withdraw_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const uint8_t* d
     Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
     if (!W) return OG_E_NOMEM;
     OG_TRY(withdraw_witness_strided_dev(ctx, L, L.n_vars, d_null, d_sec, d_rec, d_sib, d_bits, batch, W));
+    uint64_t tot = (uint64_t)batch * L.n_vars;
+    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
+    return OG_OK;
+}
+
+int32_t deposit_witness_bytes_dev(og_ctx* ctx, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
+                                  uint8_t* d_out) {
+    DepositLayout L = DepositLayout::make();
+    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
+    if (!W) return OG_E_NOMEM;
+    OG_TRY(deposit_witness_strided_dev(ctx, L.n_vars, d_null, d_sec, d_dep, batch, W));
     uint64_t tot = (uint64_t)batch * L.n_vars;
     OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
     return OG_OK;

@@ -1,6 +1,6 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
-// paths (BASELINE config 2), level-by-level tree build, and the witness generator of the withdraw
-// statement (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
+// paths (BASELINE config 2), level-by-level tree build, and the witness generators of the withdraw
+// and deposit statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -155,6 +155,24 @@ __global__ void __launch_bounds__(32) k_withdraw_witness(WithdrawLayout L, uint3
     w[1] = cur;
 }
 
+// Witness of the deposit statement, layout of DESIGN.md section 3 (== oracle/deposit_circuit.py).
+// One thread per proof; row p starts at W + p * w_stride, Montgomery form.
+__global__ void __launch_bounds__(32) k_deposit_witness(DepositLayout L, uint32_t w_stride, const uint8_t* __restrict__ nullifiers,
+                                                        const uint8_t* __restrict__ secrets, const uint8_t* __restrict__ depositors,
+                                                        uint32_t batch, Fr* __restrict__ W, int* flag) {
+    uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= batch) return;
+    Fr* w = W + (uint64_t)p * w_stride;
+    Fr nu = load_canonical<Fr>(nullifiers + 32ull * p, flag);
+    Fr se = load_canonical<Fr>(secrets + 32ull * p, flag);
+    Fr de = load_canonical<Fr>(depositors + 32ull * p, flag);
+    w[0] = Fr::one(); w[2] = de; w[3] = nu; w[4] = se;
+    w[5] = de.sqr();
+    Fr cm = mimc7_hash2<true>(nu, se, w + L.cm_base, w + L.cm_base + L.perm);
+    w[L.cm_out] = cm;
+    w[1] = cm;
+}
+
 // ---- host side ------------------------------------------------------------------------------------
 void mimc_constants_host(Fr* out91) { mimc7_round_constants(out91); }
 
@@ -219,6 +237,15 @@ int32_t withdraw_witness_strided_dev(og_ctx* ctx, const WithdrawLayout& L, uint3
     if (batch == 0) return OG_OK;
     if (w_stride < L.n_vars) return OG_E_INVALID;
     OG_LAUNCH(ctx, k_withdraw_witness, (batch + 31) / 32, 32, 0, L, w_stride, d_null, d_sec, d_rec, d_sib, d_bits, batch, d_W, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep,
+                                    uint32_t batch, Fr* d_W) {
+    if (batch == 0) return OG_OK;
+    DepositLayout L = DepositLayout::make();
+    if (w_stride < L.n_vars) return OG_E_INVALID;
+    OG_LAUNCH(ctx, k_deposit_witness, (batch + 31) / 32, 32, 0, L, w_stride, d_null, d_sec, d_dep, batch, d_W, ctx->d_flag);
     return OG_OK;
 }
 

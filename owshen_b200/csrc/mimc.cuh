@@ -1,5 +1,6 @@
-// owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layout of the
-// withdraw statement (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout).
+// owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
+// withdraw and deposit statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout
+// and oracle/deposit_circuit.py: Layout).
 #pragma once
 #include "common.cuh"
 
@@ -23,6 +24,22 @@ struct WithdrawLayout {
     }
 };
 
+constexpr uint32_t DEPOSIT_N_PUB = 2;
+
+// 0 ONE | 1 commitment | 2 depositor | 3 nullifier | 4 secret | 5 depositor_sq | 6.. perm1 perm2 out
+struct DepositLayout {
+    uint32_t perm, cm_base, cm_out, n_vars, n_constraints;
+    static DepositLayout make(uint32_t n_rounds = 91) {
+        DepositLayout L;
+        L.perm = 4 * n_rounds;
+        L.cm_base = 6;
+        L.cm_out = L.cm_base + 2 * L.perm;
+        L.n_vars = L.cm_out + 1;
+        L.n_constraints = 1 + (2 * L.perm + 1) + 1;
+        return L;
+    }
+};
+
 int32_t mimc_hash2_dev(og_ctx* ctx, const uint8_t* d_l, const uint8_t* d_r, uint64_t n, uint8_t* d_out);
 int32_t mimc_merkle_paths_dev(og_ctx* ctx, const uint8_t* d_leaves, const uint8_t* d_siblings, const uint32_t* d_bits,
                               uint32_t n_paths, uint32_t depth, uint8_t* d_out);
@@ -33,6 +50,8 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
 // W rows are w_stride elements apart (the prover keeps two extra scalars after every witness)
 int32_t withdraw_witness_strided_dev(og_ctx* ctx, const WithdrawLayout& L, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec,
                                      const uint8_t* d_rec, const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, Fr* d_W);
+int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep,
+                                    uint32_t batch, Fr* d_W);
 
 // BabyJubJub batch verification (bjj_impl.cuh); out[i] in {0, 1, 2 = public key does not decompress}
 int32_t bjj_verify_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_odd, const uint8_t* d_msgs, const uint8_t* d_sigs,

@@ -1,8 +1,8 @@
-// owshen_b200/csrc/setup.cu -- development Groth16 setup for the withdraw statement ("toxic waste in
+// owshen_b200/csrc/setup.cu -- development Groth16 setup for the withdraw statement or any caller's R1CS ("toxic waste in
 // the clear": tau, alpha, beta, gamma, delta are inputs, so that every pk/vk byte is reproducible and
 // can be compared with oracle/groth16.py).  A production deployment would load a ceremony's key with
-// og_load_pk instead.  QAP evaluation at tau is ~10^5 host field operations; the ~1.6*10^5
-// fixed-base scalar multiplications run on the GPU (msm.cu: fixed_base_mul_*).
+// og_load_pk instead.  QAP evaluation at tau is ~10^5 host field operations for the depth-32 withdraw key;
+// its ~1.6*10^5 fixed-base scalar multiplications run on the GPU (msm.cu: fixed_base_mul_*).
 // Conventions: DESIGN.md section 4 (domain, input-consistency rows, coset-Lagrange H query).
 #include "groth16.cuh"
 #include "msm.cuh"
@@ -60,17 +60,14 @@ static void put_csr(std::vector<uint8_t>& v, const Csr& M) {
     for (const Fr& c : M.val) { uint8_t b[32]; host_store(b, c); put_bytes(v, b, 32); }
 }
 
-int32_t setup_withdraw(og_ctx* ctx, uint32_t depth, const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len,
-                       uint8_t* vk_out, uint64_t* vk_len) {
-    if (depth == 0 || depth > 32 || !pk_len || !vk_len) return OG_E_INVALID;
-    WithdrawLayout L = WithdrawLayout::make(depth);
-    const uint32_t nv = L.n_vars, n_pub = WITHDRAW_N_PUB, n_priv = nv - n_pub - 1;
-    const uint32_t log_m = groth16_domain_log(L.n_constraints, n_pub), m = 1u << log_m;
+// The setup of any R1CS in the library's conventions (variable 0 = ONE, 1..n_pub public).  `cs` must be well formed:
+// setup_withdraw builds it, setup_generic validates the caller's.  depth is recorded in the key (0 = not a withdraw key).
+static int32_t setup_r1cs(og_ctx* ctx, const R1cs& cs, uint32_t depth, const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len,
+                          uint8_t* vk_out, uint64_t* vk_len) {
+    const uint32_t nv = cs.n_vars, n_pub = cs.n_pub, n_priv = nv - n_pub - 1;
+    const uint32_t log_m = groth16_domain_log(cs.n_constraints(), n_pub), m = 1u << log_m;
     // sizes first, so callers can allocate
-    uint64_t csr_bound = 0;   // filled after the build; the size query needs the build as well (cheap)
-    R1cs cs = WithdrawBuilder::build(depth);
-    if (cs.n_constraints() != L.n_constraints) return OG_E_INVALID;
-    csr_bound = 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.A.col.size() + 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.B.col.size();
+    const uint64_t csr_bound = 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.A.col.size() + 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.B.col.size();
     const uint64_t need_pk = 8 + 20 + 64 + 64 + 128 + 64 + 128 + 64ull * nv * 2 + 128ull * nv + 64ull * n_priv + 64ull * m + csr_bound;
     const uint64_t need_vk = 8 + 4 + 64 + 128 + 128 + 128 + 64ull * (n_pub + 1);
     if (!pk_out || !vk_out) { *pk_len = need_pk; *vk_len = need_vk; return OG_OK; }
@@ -150,6 +147,42 @@ int32_t setup_withdraw(og_ctx* ctx, uint32_t depth, const uint8_t* toxic160, uin
     memcpy(pk_out, pk.data(), pk.size()); *pk_len = pk.size();
     memcpy(vk_out, vk.data(), vk.size()); *vk_len = vk.size();
     return OG_OK;
+}
+
+int32_t setup_withdraw(og_ctx* ctx, uint32_t depth, const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len,
+                       uint8_t* vk_out, uint64_t* vk_len) {
+    if (depth == 0 || depth > 32 || !pk_len || !vk_len) return OG_E_INVALID;
+    R1cs cs = WithdrawBuilder::build(depth);
+    if (cs.n_constraints() != WithdrawLayout::make(depth).n_constraints) return OG_E_INVALID;
+    return setup_r1cs(ctx, cs, depth, toxic160, pk_out, pk_len, vk_out, vk_len);
+}
+
+// one matrix of the caller's R1CS: row_ptr starts at 0 and never decreases, columns < n_vars, coefficients < r
+static int32_t load_csr(uint32_t n_rows, uint32_t n_vars, const uint32_t* row_ptr, const uint32_t* col, const uint8_t* coeffs, Csr& M) {
+    if (!row_ptr || row_ptr[0] != 0) return OG_E_INVALID;
+    for (uint32_t i = 0; i < n_rows; i++) if (row_ptr[i] > row_ptr[i + 1]) return OG_E_INVALID;
+    const uint32_t nnz = row_ptr[n_rows];
+    if (nnz && (!col || !coeffs)) return OG_E_INVALID;
+    for (uint32_t k = 0; k < nnz; k++) if (col[k] >= n_vars) return OG_E_INVALID;
+    M.row_ptr.assign(row_ptr, row_ptr + n_rows + 1);
+    M.col.assign(col, col + nnz);
+    M.val.resize(nnz);
+    for (uint32_t k = 0; k < nnz; k++) if (!host_load(M.val[k], coeffs + 32ull * k)) return OG_E_ENCODING;
+    return OG_OK;
+}
+
+int32_t setup_generic(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub, const uint32_t* const row_ptr[3],
+                      const uint32_t* const col[3], const uint8_t* const coeffs[3], const uint8_t* toxic160, uint8_t* pk_out,
+                      uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len) {
+    // the limits og_load_pk enforces: n_pub <= 2^16, n_pub + 1 <= n_vars, a domain of at most 2^24
+    if (!pk_len || !vk_len || n_constraints == 0 || n_pub > (1u << 16) || (uint64_t)n_pub + 1 > n_vars ||
+        (uint64_t)n_constraints + n_pub + 1 > (1ull << 24)) return OG_E_INVALID;
+    R1cs cs;
+    cs.n_vars = n_vars;
+    cs.n_pub = n_pub;
+    Csr* M[3] = {&cs.A, &cs.B, &cs.C};
+    for (int k = 0; k < 3; k++) OG_TRY(load_csr(n_constraints, n_vars, row_ptr[k], col[k], coeffs[k], *M[k]));
+    return setup_r1cs(ctx, cs, 0, toxic160, pk_out, pk_len, vk_out, vk_len);
 }
 
 }  // namespace og

@@ -1,12 +1,18 @@
-// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builder of the withdraw statement's R1CS
-// (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); this is the
-// product's own definition and tests/test_circuit_parity.py checks it entry for entry against the
-// independently written oracle/withdraw_circuit.py through og_withdraw_r1cs_export.
+// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw and deposit statements'
+// R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these are the
+// product's own definitions, checked entry for entry against the independently written
+// oracle/withdraw_circuit.py and oracle/deposit_circuit.py through og_withdraw_r1cs_export and
+// og_deposit_r1cs_export.
 //
+// withdraw
 //   public : root, nullifier_hash, recipient
 //   private: nullifier, secret, siblings[depth], bits[depth]
 //   nullifier_hash = MultiMiMC7([nullifier], key 1); commitment = MultiMiMC7([nullifier, secret], 0);
 //   root = Merkle root from commitment with node = MultiMiMC7([left, right], 0); recipient^2 bound.
+// deposit
+//   public : commitment, depositor
+//   private: nullifier, secret
+//   commitment = MultiMiMC7([nullifier, secret], 0) (the withdraw statement's leaf); depositor^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -48,10 +54,13 @@ struct R1cs {
     uint32_t n_constraints() const { return A.rows(); }
 };
 
-struct WithdrawBuilder {
+// the MiMC7 gadgets both statements are made of
+struct Mimc7Builder {
     R1cs cs;
     Fr consts[MIMC_ROUNDS];
     uint32_t n_rounds;
+
+    explicit Mimc7Builder(uint32_t rounds) : n_rounds(rounds) { mimc7_round_constants(consts); }
 
     // MiMC7 permutation rounds over x with key k; returns the LC of hash(x, k) = perm + k
     LC perm(const LC& x, const LC& k, uint32_t base) {
@@ -76,11 +85,11 @@ struct WithdrawBuilder {
         LC r2 = lc_sum({&r1, &right, &h2});
         cs.add(r2, lc_var(0), lc_var(out));
     }
+};
 
+struct WithdrawBuilder {
     static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
-        WithdrawBuilder b;
-        b.n_rounds = n_rounds;
-        mimc7_round_constants(b.consts);
+        Mimc7Builder b(n_rounds);
         WithdrawLayout L = WithdrawLayout::make(depth, n_rounds);
         b.cs.n_vars = L.n_vars;
         b.cs.n_pub = WITHDRAW_N_PUB;
@@ -106,6 +115,21 @@ struct WithdrawBuilder {
         }
         LC vcur = lc_var(cur), nroot = lc_neg_var(V_ROOT);
         b.cs.add(lc_sum({&vcur, &nroot}), lc_var(V_ONE), LC());
+        return b.cs;
+    }
+};
+
+struct DepositBuilder {
+    static R1cs build(uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        DepositLayout L = DepositLayout::make(n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = DEPOSIT_N_PUB;
+        const uint32_t V_ONE = 0, V_CM = 1, V_DEP = 2, V_NULL = 3, V_SECRET = 4, V_DSQ = 5;
+        b.cs.add(lc_var(V_DEP), lc_var(V_DEP), lc_var(V_DSQ));
+        b.hash2(lc_var(V_NULL), lc_var(V_SECRET), L.cm_base, L.cm_base + L.perm, L.cm_out);
+        LC vout = lc_var(L.cm_out), ncm = lc_neg_var(V_CM);
+        b.cs.add(lc_sum({&vout, &ncm}), lc_var(V_ONE), LC());
         return b.cs;
     }
 };
