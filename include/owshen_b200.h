@@ -172,6 +172,25 @@ int32_t og_deposit_r1cs_export(int32_t which, uint32_t* row_ptr, uint32_t* col_i
 int32_t og_deposit_witness(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* depositors,
                            uint32_t batch, uint8_t* witnesses);
 
+/* ---- the transfer statement (DESIGN.md section 3): two value notes in, two out, a public amount --------------- */
+/* note = (nullifier, secret, token, amount < 2^64), commitment = MultiMiMC7([nullifier, secret, token, amount], 0),
+ * nullifier hash = MultiMiMC7([nullifier], 1).  Public inputs (root, public_amount, token, recipient, nullifier_hash[2],
+ * out_commitment[2]); public_amount = out amounts - in amounts (mod r).  depth 1..32; at depth 32: 53 683 variables,
+ * 53 609 constraints, domain 2^16. */
+int32_t og_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: roots / tokens / recipients 32 B each;
+ * in_* and out_* hold note 0 then note 1 (nullifiers and secrets 2 * 32 B, amounts 2 * uint64); in_siblings holds
+ * 2 * depth elements (input 0's path, then input 1's) and in_path_bits 2 words.  root is the caller's: an input of nonzero
+ * amount that does not reach it, or two inputs with one nullifier, give a witness that does not satisfy the R1CS. */
+int32_t og_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                            const uint8_t* in_nullifiers, const uint8_t* in_secrets, const uint64_t* in_amounts,
+                            const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                            const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
+                            uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -194,6 +213,9 @@ int32_t og_pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t*
 /* window bits of the A (G1), B (G2) and C' (G1) MSMs the key proves with: chosen from the key's size when it was
  * loaded (OG_WINDOW_BITS / OG_C_A / OG_C_B / OG_C_C override) */
 int32_t og_pk_window_bits(const og_pk* pk, uint32_t* c3);
+/* how the prover runs `batch` proofs with this key: proofs per chunk, chunks in flight, and the scratch bytes of one lane.
+ * Without OG_CHUNK the chunk is min(1024, 28 GiB / the scratch of one proof); OG_CHUNK / OG_LANES override. */
+int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane);
 
 /* batch of proofs from full witnesses (batch * n_vars * 32 B); rs = batch * (r || s) */
 int32_t og_groth16_prove(og_ctx* ctx, const og_pk* pk, const uint8_t* witnesses, uint32_t batch,
@@ -218,6 +240,20 @@ int32_t og_groth16_prove_deposit(og_ctx* ctx, const og_pk* pk, const uint8_t* nu
 int32_t og_groth16_prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
                                      const uint8_t* d_depositors, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
                                      uint8_t* d_public_out);
+/* batch of transfer proofs from the notes, witness generation on the GPU; inputs as in og_transfer_witness.  OG_E_INVALID
+ * unless the key has a transfer statement's shape (the depth is recognised from it).  public_out (optional):
+ * batch * 8 * 32 B = root, public_amount, token, recipient, nullifier_hash[2], out_commitment[2]. */
+int32_t og_groth16_prove_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens,
+                                  const uint8_t* recipients, const uint8_t* in_nullifiers, const uint8_t* in_secrets,
+                                  const uint64_t* in_amounts, const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                  const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
+                                  uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out);
+/* same with every buffer already in HBM; no synchronisation */
+int32_t og_groth16_prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
+                                      const uint8_t* d_recipients, const uint8_t* d_in_nullifiers, const uint8_t* d_in_secrets,
+                                      const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
+                                      const uint8_t* d_out_nullifiers, const uint8_t* d_out_secrets, const uint64_t* d_out_amounts,
+                                      uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

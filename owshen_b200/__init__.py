@@ -1,4 +1,4 @@
-"""owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool deposit and withdraw proofs over BN254.
+"""owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool deposit, withdraw and transfer proofs over BN254.
 
 Python is the host language here because the reference's (Rust) toolchain is absent from this image;
 everything below is a thin ctypes veneer over the C ABI in include/owshen_b200.h, which is the real
@@ -7,8 +7,9 @@ anywhere, but creating a Context without a CUDA device raises.
 """
 from .kvstore import KvStore, MirrorKvStore, RamKvStore
 from .api import (Context, ProvingKey, MerkleTree, OwshenB200Error, lib, build_library, prove, verify,
-                  setup_withdraw, setup_r1cs, setup_deposit, deposit_r1cs_info, deposit_r1cs_export, FR_MODULUS, PROOF_BYTES)
+                  setup_withdraw, setup_r1cs, setup_deposit, deposit_r1cs_info, deposit_r1cs_export,
+                  setup_transfer, transfer_r1cs_info, transfer_r1cs_export, FR_MODULUS, PROOF_BYTES)
 
 __all__ = ["Context", "ProvingKey", "MerkleTree", "OwshenB200Error", "lib", "build_library", "prove", "verify",
            "setup_withdraw", "setup_r1cs", "setup_deposit", "deposit_r1cs_info", "deposit_r1cs_export",
-           "FR_MODULUS", "PROOF_BYTES", "KvStore", "RamKvStore", "MirrorKvStore"]
+           "setup_transfer", "transfer_r1cs_info", "transfer_r1cs_export", "FR_MODULUS", "PROOF_BYTES", "KvStore", "RamKvStore", "MirrorKvStore"]

@@ -83,6 +83,9 @@ _SIGS = {
     "og_deposit_r1cs_info": (C.c_int32, [C.POINTER(C.c_uint32)] * 4),
     "og_deposit_r1cs_export": (C.c_int32, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_deposit_witness": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p]),
+    "og_transfer_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_transfer_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_transfer_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -95,6 +98,9 @@ _SIGS = {
     "og_groth16_prove_withdraw_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_deposit": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_deposit_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_transfer": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
 }
@@ -165,6 +171,36 @@ def _need_len(x, n, name):
 
 def _bits_array(bits):
     return (C.c_uint32 * len(bits))(*[int(b) & 0xFFFFFFFF for b in bits])
+
+
+def _u64_array(xs):
+    """Amounts as a buffer of little-endian uint64: bytes-like, a uint64 array / tensor, or a sequence of ints < 2^64."""
+    if _blen(xs) is not None or isinstance(xs, int):
+        return xs
+    vals = [int(x) for x in xs]
+    _need(all(0 <= x < 1 << 64 for x in vals), "amounts must be integers in [0, 2^64)")
+    return (C.c_uint64 * len(vals))(*vals)
+
+
+def _u32_array(xs):
+    return xs if _blen(xs) is not None or isinstance(xs, int) else _bits_array(xs)
+
+
+def _transfer_args(fn, batch, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
+                   out_nullifiers, out_secrets, out_amounts):
+    """Length checks of a transfer batch's eleven input arrays -> their pointers in C ABI order."""
+    amounts = [_u64_array(in_amounts), _u64_array(out_amounts)]
+    bits = _u32_array(in_path_bits)
+    for name, buf, size in (("roots", roots, 32), ("tokens", tokens, 32), ("recipients", recipients, 32),
+                            ("in_nullifiers", in_nullifiers, 64), ("in_secrets", in_secrets, 64), ("in_amounts", amounts[0], 16),
+                            ("in_siblings", in_siblings, 64 * depth), ("in_path_bits", bits, 8),
+                            ("out_nullifiers", out_nullifiers, 64), ("out_secrets", out_secrets, 64), ("out_amounts", amounts[1], 16)):
+        if isinstance(buf, C.Array):        # converted from a sequence above
+            _need(C.sizeof(buf) == size * batch, f"{fn}: {name}: expected {size * batch // C.sizeof(buf._type_)} values, got {len(buf)}")
+        else:
+            _need_len(buf, size * batch, f"{fn}: {name}")
+    return [_ptr(x) for x in (roots, tokens, recipients, in_nullifiers, in_secrets, amounts[0], in_siblings, bits,
+                              out_nullifiers, out_secrets, amounts[1])]
 
 
 def fr_bytes(x: int) -> bytes:
@@ -383,6 +419,22 @@ class Context:
         _check(lib().og_deposit_witness(self._h, nullifiers, secrets, depositors, n, out), self)
         return out.raw
 
+    def transfer_witness(self, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
+                         out_nullifiers, out_secrets, out_amounts) -> bytes:
+        """Full assignments of the depth-`depth` transfer statement, n_vars * 32 bytes per transfer, computed on the GPU.
+        Per transfer: roots / tokens / recipients 32 bytes each; in_* / out_* note 0 then note 1 (nullifiers and secrets
+        2 x 32 bytes, amounts 2 x uint64 as 8-byte little-endian buffers, uint64 arrays or ints); in_siblings 2 * depth
+        elements (input 0's path, then input 1's); in_path_bits 2 words."""
+        _need(1 <= depth <= 32 and _blen(roots) is not None and _blen(roots) % 32 == 0,
+              "transfer_witness: depth must be 1..32 and roots a multiple of 32 bytes")
+        n = _blen(roots) // 32
+        args = _transfer_args("transfer_witness", n, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts,
+                              in_siblings, in_path_bits, out_nullifiers, out_secrets, out_amounts)
+        nv = transfer_r1cs_info(depth)["n_vars"]
+        out = C.create_string_buffer(32 * n * nv)
+        _check(lib().og_transfer_witness(self._h, depth, *args, n, out), self)
+        return out.raw
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -429,6 +481,25 @@ def deposit_r1cs_export(which: str):
     return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
 
 
+def transfer_r1cs_info(depth: int) -> dict:
+    v = [C.c_uint32() for _ in range(4)]
+    _check(lib().og_transfer_r1cs_info(depth, *[C.byref(x) for x in v]))
+    return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+
+
+def transfer_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` transfer R1CS."""
+    w = "ABC".index(which)
+    nnz = C.c_uint64()
+    _check(lib().og_transfer_r1cs_export(depth, w, None, None, None, C.byref(nnz)))
+    nc = transfer_r1cs_info(depth)["n_constraints"]
+    ptr = (C.c_uint32 * (nc + 1))()
+    col = (C.c_uint32 * nnz.value)()
+    val = C.create_string_buffer(32 * nnz.value)
+    _check(lib().og_transfer_r1cs_export(depth, w, ptr, col, val, C.byref(nnz)))
+    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+
+
 def setup_r1cs(ctx: Context, n_vars: int, n_pub: int, A, B, C_, tau: int, alpha: int, beta: int, gamma: int, delta: int):
     """Development setup of any R1CS -> (pk_bytes, vk_bytes).  A, B, C_ are (row_ptr, col_idx, coeffs) triples as
     r1cs_export returns them (coefficients as ints or 32-byte little-endian values); variable 0 is ONE and variables
@@ -460,6 +531,14 @@ def setup_deposit(ctx: Context, tau: int, alpha: int, beta: int, gamma: int, del
     """Development setup of the deposit statement -> (pk_bytes, vk_bytes): its exported R1CS through setup_r1cs."""
     info = deposit_r1cs_info()
     return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(deposit_r1cs_export(m) for m in "ABC"), tau, alpha, beta, gamma, delta)
+
+
+def setup_transfer(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` transfer statement -> (pk_bytes, vk_bytes): its exported R1CS through
+    setup_r1cs.  The key records depth 0; the prover recognises it as a transfer key by its shape."""
+    info = transfer_r1cs_info(depth)
+    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(transfer_r1cs_export(depth, m) for m in "ABC"),
+                      tau, alpha, beta, gamma, delta)
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -544,6 +623,39 @@ class ProvingKey:
         _check(lib().og_groth16_prove_deposit(self.ctx._h, self._h, _ptr(nullifiers), _ptr(secrets), _ptr(depositors), batch,
                                               _ptr(rs), proofs, pub), self.ctx)
         return proofs.raw, (pub.raw if want_public else None)
+
+    @property
+    def transfer_depth(self):
+        """The depth d whose transfer statement has this key's shape (transfer_r1cs_info), or None."""
+        for d in range(1, 33):
+            info = transfer_r1cs_info(d)
+            if (info["n_vars"], info["n_pub"]) == (self.n_vars, self.n_pub):
+                return d
+        return None
+
+    def prove_transfer(self, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
+                       out_nullifiers, out_secrets, out_amounts, rs, want_public=True):
+        """Batch of transfer proofs from the notes (witness generation on the GPU).  Inputs as in Context.transfer_witness;
+        returns (proofs, public_inputs) with public inputs (root, public_amount, token, recipient, nullifier_hash[2],
+        out_commitment[2]) per proof."""
+        depth = self.transfer_depth
+        if depth is None:
+            raise OwshenB200Error(OG_E_INVALID, "prove_transfer: this key was not made for a transfer statement")
+        _need(_blen(rs) is not None and _blen(rs) % 64 == 0, "prove_transfer: rs must be a buffer of 64 bytes (r, s) per proof")
+        batch = _blen(rs) // 64
+        args = _transfer_args("prove_transfer", batch, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts,
+                              in_siblings, in_path_bits, out_nullifiers, out_secrets, out_amounts)
+        proofs = C.create_string_buffer(PROOF_BYTES * batch)
+        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
+        _check(lib().og_groth16_prove_transfer(self.ctx._h, self._h, *args, batch, _ptr(rs), proofs, pub), self.ctx)
+        return proofs.raw, (pub.raw if want_public else None)
+
+    def prover_plan(self, batch: int) -> dict:
+        """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and
+        scratch_bytes_per_lane.  OG_CHUNK / OG_LANES in the environment override the defaults."""
+        c, l, s = C.c_uint32(), C.c_uint32(), C.c_uint64()
+        _check(lib().og_pk_prover_plan(self._h, batch, C.byref(c), C.byref(l), C.byref(s)))
+        return dict(chunk=c.value, lanes=l.value, scratch_bytes_per_lane=s.value)
 
 
 def prove(pk: ProvingKey, nullifiers, secrets, recipients, siblings, path_bits, rs):

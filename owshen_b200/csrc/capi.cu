@@ -856,6 +856,69 @@ int32_t og_deposit_witness(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t
     return check_flag(ctx);
 }
 
+// ---- transfer statement ---------------------------------------------------------------------------------------
+int32_t og_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    if (depth == 0 || depth > 32) return OG_E_INVALID;
+    TransferLayout L = TransferLayout::make(depth);
+    if (n_constraints) *n_constraints = L.n_constraints;
+    if (n_vars) *n_vars = L.n_vars;
+    if (n_pub) *n_pub = TRANSFER_N_PUB;
+    if (log_m) *log_m = groth16_domain_log(L.n_constraints, TRANSFER_N_PUB);
+    return OG_OK;
+}
+int32_t og_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    if (depth == 0 || depth > 32 || which < 0 || which > 2 || !nnz) return OG_E_INVALID;
+    R1cs cs = TransferBuilder::build(depth);
+    const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
+    *nnz = M.col.size();
+    if (!row_ptr || !col_idx || !coeffs) return OG_OK;
+    memcpy(row_ptr, M.row_ptr.data(), 4 * M.row_ptr.size());
+    memcpy(col_idx, M.col.data(), 4 * M.col.size());
+    for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
+    return OG_OK;
+}
+
+// the eleven host input arrays of a transfer batch, copied into one device slot (each array 256-byte aligned)
+static int32_t stage_transfer_inputs(og_ctx* ctx, uint32_t depth, uint32_t batch, const uint8_t* roots, const uint8_t* tokens,
+                                     const uint8_t* recipients, const uint8_t* in_nullifiers, const uint8_t* in_secrets,
+                                     const uint64_t* in_amounts, const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                     const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
+                                     TransferInputs& d) {
+    const uint64_t b = batch;
+    const void* src[11] = {roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
+                           out_nullifiers, out_secrets, out_amounts};
+    const uint64_t bytes[11] = {32 * b, 32 * b, 32 * b, 64 * b, 64 * b, 16 * b, 64ull * depth * b, 8 * b, 64 * b, 64 * b, 16 * b};
+    uint64_t off[11], tot = 0;
+    for (int k = 0; k < 11; k++) { off[k] = tot; tot += (bytes[k] + 255) & ~255ull; }
+    OG_SLOT(ctx, base, uint8_t, S_IO_TRANSFER, tot);
+    for (int k = 0; k < 11; k++) H2D(ctx, base + off[k], src[k], bytes[k]);
+    d.roots = base + off[0]; d.tokens = base + off[1]; d.recipients = base + off[2];
+    d.in_null = base + off[3]; d.in_sec = base + off[4]; d.in_amounts = (const uint64_t*)(base + off[5]);
+    d.in_sib = base + off[6]; d.in_bits = (const uint32_t*)(base + off[7]);
+    d.out_null = base + off[8]; d.out_sec = base + off[9]; d.out_amounts = (const uint64_t*)(base + off[10]);
+    return OG_OK;
+}
+
+int32_t og_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                            const uint8_t* in_nullifiers, const uint8_t* in_secrets, const uint64_t* in_amounts,
+                            const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                            const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
+                            uint32_t batch, uint8_t* witnesses) {
+    OG_ENTER(ctx);
+    if (depth == 0 || depth > 32 || !roots || !tokens || !recipients || !in_nullifiers || !in_secrets || !in_amounts || !in_siblings ||
+        !in_path_bits || !out_nullifiers || !out_secrets || !out_amounts || !witnesses) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    TransferLayout L = TransferLayout::make(depth);
+    TransferInputs d;
+    OG_TRY(stage_transfer_inputs(ctx, depth, batch, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
+                                 in_path_bits, out_nullifiers, out_secrets, out_amounts, d));
+    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
+    OG_TRY(clear_flag(ctx));
+    OG_TRY(transfer_witness_bytes_dev(ctx, depth, d, batch, dout));
+    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
+    return check_flag(ctx);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -978,6 +1041,52 @@ int32_t og_groth16_prove_deposit(og_ctx* ctx, const og_pk* pk, const uint8_t* nu
     D2H(ctx, proofs, dpr, 256ull * batch);
     if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * DEPOSIT_N_PUB);
     return check_flag(ctx);
+}
+
+int32_t og_groth16_prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
+                                      const uint8_t* d_recipients, const uint8_t* d_in_nullifiers, const uint8_t* d_in_secrets,
+                                      const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
+                                      const uint8_t* d_out_nullifiers, const uint8_t* d_out_secrets, const uint64_t* d_out_amounts,
+                                      uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    OG_ENTER(ctx);
+    if (!pk || !d_roots || !d_tokens || !d_recipients || !d_in_nullifiers || !d_in_secrets || !d_in_amounts || !d_in_siblings ||
+        !d_in_path_bits || !d_out_nullifiers || !d_out_secrets || !d_out_amounts || !d_rs || !d_proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    TransferInputs d{d_roots, d_tokens, d_recipients, d_in_nullifiers, d_in_secrets, d_in_amounts, d_in_siblings, d_in_path_bits,
+                     d_out_nullifiers, d_out_secrets, d_out_amounts};
+    return prove_transfer_dev(ctx, pk, d, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                  const uint8_t* in_nullifiers, const uint8_t* in_secrets, const uint64_t* in_amounts,
+                                  const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                  const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
+                                  uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
+    OG_ENTER(ctx);
+    if (!pk || !roots || !tokens || !recipients || !in_nullifiers || !in_secrets || !in_amounts || !in_siblings || !in_path_bits ||
+        !out_nullifiers || !out_secrets || !out_amounts || !rs || !proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    const uint32_t depth = pk_transfer_depth(pk);
+    if (depth == 0) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    TransferInputs d;
+    OG_TRY(stage_transfer_inputs(ctx, depth, batch, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
+                                 in_path_bits, out_nullifiers, out_secrets, out_amounts, d));
+    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
+    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
+    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * TRANSFER_N_PUB);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, drs, rs, 64ull * batch);
+    OG_TRY(prove_transfer_dev(ctx, pk, d, batch, drs, dpr, public_out ? dpub : nullptr));
+    D2H(ctx, proofs, dpr, 256ull * batch);
+    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * TRANSFER_N_PUB);
+    return check_flag(ctx);
+}
+
+int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {
+    if (!pk) return OG_E_INVALID;
+    pk_prover_plan(pk, batch, chunk, lanes, scratch_bytes_per_lane);
+    return OG_OK;
 }
 
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out) {

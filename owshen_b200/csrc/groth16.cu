@@ -2,9 +2,9 @@
 // development setup.  The reference has no prover (SURVEY.md section 0); conventions are frozen in
 // DESIGN.md section 4 and checked bit-for-bit against oracle/groth16.py and oracle/cpu.
 //
-// Once per batch:  witness  k_withdraw_witness / k_deposit_witness (mimc.cu): every MiMC7 round value -> W[batch][n_vars+2]
-//                  (or full witnesses from the caller)
-// Per chunk of B proofs (default 1024; everything stays in HBM, nothing returns to the host until the proofs):
+// Once per batch:  witness  k_withdraw_witness / k_deposit_witness / k_transfer_witness (mimc.cu): every MiMC7 round value
+//                  -> W[batch][n_vars+2] (or full witnesses from the caller)
+// Per chunk of B proofs (default min(1024, the lane budget / one proof's scratch); everything stays in HBM, nothing returns to the host until the proofs):
 //   a, b, c      k_abc: sparse A.w, B.w over the CSR kept in L2, c = a*b
 //   h            3 iNTT + 3 coset NTT (ntt.cu), k_pointwise: d = a'b' - c' written straight into
 //                the scalar vector of the C multi-scalar multiplication
@@ -362,49 +362,80 @@ static uint32_t affine_mode() { return env_u32("OG_AFFINE", 0); }
 static uint32_t affine_mode() { return 0; }
 #endif
 
+// Bytes of the prover's scratch for `batch` proofs in chunks of B: what one lane allocates for its chunk, and what the
+// batch shares (witness rows, (r, s), per-proof MSM totals).  alloc_chunk allocates exactly these and the chunk rule
+// (prover_plan) budgets with them.
+struct ProverScratch {
+    size_t abc, scalars, sorted, counts, offsets, cursor, heavy, buckets, seg, aff;      // per lane
+    size_t stage, tiles;   // per lane, 0 when the sort's staging / tile counters fit in the buckets / heavy scratch
+    size_t wit, misc, sums;                                                               // per batch
+    size_t lane() const { return abc + scalars + sorted + counts + offsets + cursor + heavy + buckets + seg + aff + stage + tiles; }
+};
+
+static ProverScratch prover_scratch(const og_pk* pk, uint32_t batch, uint32_t B) {
+    const uint32_t m = 1u << pk->log_m;
+    const size_t max_pts = pk->nC > pk->nA ? pk->nC : pk->nA;
+    const size_t n_keys = (size_t)B * pk->max_nb;
+    ProverScratch s;
+    s.wit = sizeof(Fr) * (size_t)batch * (pk->n_vars + 2);
+    s.misc = sizeof(Fr) * 2 * (size_t)batch;
+    s.sums = (sizeof(G1XYZZ) * 2 + sizeof(G2XYZZ)) * (size_t)batch;
+    s.abc = sizeof(Fr) * (size_t)B * 3 * m * 2;
+    s.scalars = sizeof(Fr) * (size_t)B * (pk->nB + pk->nC);
+    s.sorted = 4 * (size_t)B * max_pts * pk->max_windows;
+    s.counts = 4 * n_keys;
+    s.offsets = 4 * (n_keys + 1);
+    s.cursor = 4 * n_keys;
+    s.heavy = 4 * (2 * n_keys + 4);
+    s.buckets = sizeof(G2XYZZ) * n_keys;
+    s.seg = sizeof(G2XYZZ) * msm_lvl_elems(B, pk->max_nb);
+    s.aff = 0;
+    if (affine_mode() & 1) s.aff = msm_aff_scratch_bytes_g1(n_keys);
+    if ((affine_mode() & 2) && msm_aff_scratch_bytes_g2((size_t)B * pk->nb[1]) > s.aff) s.aff = msm_aff_scratch_bytes_g2((size_t)B * pk->nb[1]);
+    // The sort's staging lives in the bucket array: nothing writes it before the accumulation of the same MSM, and the
+    // previous MSM's reduction, which reads it, runs earlier on the same stream.  Its per-tile counters live in the heavy-bucket
+    // scratch, which msm_buckets uses only after the sort.  Only a key that outgrows either gets its own slot.
+    const uint32_t n_pts[3] = {pk->nA, pk->nB, pk->nC};
+    size_t stage = msm_sort_stage_bytes((size_t)B * max_pts * pk->max_windows), tiles = 0;
+    for (int k = 0; k < 3; k++) { size_t t = msm_sort_tile_bytes(B, pk->nb[k], n_pts[k]); if (t > tiles) tiles = t; }
+    s.stage = stage <= s.buckets ? 0 : stage;
+    s.tiles = tiles <= s.heavy ? 0 : tiles;
+    return s;
+}
+
 // W, rs_m and the per-proof totals cover the whole batch; everything else is per chunk of B proofs and per lane
 static int32_t alloc_chunk(og_ctx* ctx, const og_pk* pk, uint32_t batch, uint32_t B, int lane, ChunkBufs& b) {
     const uint32_t m = 1u << pk->log_m;
+    const ProverScratch s = prover_scratch(pk, batch, B);
     b.w_stride = pk->n_vars + 2;
     b.bsc_stride = pk->nB;
     b.csc_stride = pk->nC;
-    size_t max_pts = pk->nC > pk->nA ? pk->nC : pk->nA;
-    size_t n_keys = (size_t)B * pk->max_nb;
     auto S = [&](int id0, int id1) { return lane ? id1 : id0; };
-    b.W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * b.w_stride);
-    b.rs_m = (Fr*)ctx->slot(S_PR_MISC, sizeof(Fr) * 2 * (size_t)batch);
-    b.abc = (Fr*)ctx->slot(S(S_PR_ABC, S_L1_ABC), sizeof(Fr) * (size_t)B * 3 * m * 2);
-    b.bsc = (Fr*)ctx->slot(S(S_PR_SCALARS, S_L1_SCALARS), sizeof(Fr) * (size_t)B * (b.bsc_stride + b.csc_stride));
-    b.sorted = (uint32_t*)ctx->slot(S(S_PR_SORTED, S_L1_SORTED), 4 * (size_t)B * max_pts * pk->max_windows);
-    b.counts = (uint32_t*)ctx->slot(S(S_PR_COUNTS, S_L1_COUNTS), 4 * n_keys);
-    b.offsets = (uint32_t*)ctx->slot(S(S_PR_OFFSETS, S_L1_OFFSETS), 4 * (n_keys + 1));
-    b.cursor = (uint32_t*)ctx->slot(S(S_PR_CURSOR, S_L1_CURSOR), 4 * n_keys);
-    b.heavy = (uint32_t*)ctx->slot(S(S_PR_HEAVY, S_L1_HEAVY), 4 * (2 * n_keys + 4));
-    b.bk2 = (G2XYZZ*)ctx->slot(S(S_PR_BUCKETS, S_L1_BUCKETS), sizeof(G2XYZZ) * n_keys);
-    b.lvl2 = (G2XYZZ*)ctx->slot(S(S_PR_SEG, S_L1_SEG), sizeof(G2XYZZ) * msm_lvl_elems(B, pk->max_nb));
-    b.totA = (G1XYZZ*)ctx->slot(S_PR_SUMS, (sizeof(G1XYZZ) * 2 + sizeof(G2XYZZ)) * (size_t)batch);
+    b.W = (Fr*)ctx->slot(S_PR_WIT, s.wit);
+    b.rs_m = (Fr*)ctx->slot(S_PR_MISC, s.misc);
+    b.abc = (Fr*)ctx->slot(S(S_PR_ABC, S_L1_ABC), s.abc);
+    b.bsc = (Fr*)ctx->slot(S(S_PR_SCALARS, S_L1_SCALARS), s.scalars);
+    b.sorted = (uint32_t*)ctx->slot(S(S_PR_SORTED, S_L1_SORTED), s.sorted);
+    b.counts = (uint32_t*)ctx->slot(S(S_PR_COUNTS, S_L1_COUNTS), s.counts);
+    b.offsets = (uint32_t*)ctx->slot(S(S_PR_OFFSETS, S_L1_OFFSETS), s.offsets);
+    b.cursor = (uint32_t*)ctx->slot(S(S_PR_CURSOR, S_L1_CURSOR), s.cursor);
+    b.heavy = (uint32_t*)ctx->slot(S(S_PR_HEAVY, S_L1_HEAVY), s.heavy);
+    b.bk2 = (G2XYZZ*)ctx->slot(S(S_PR_BUCKETS, S_L1_BUCKETS), s.buckets);
+    b.lvl2 = (G2XYZZ*)ctx->slot(S(S_PR_SEG, S_L1_SEG), s.seg);
+    b.totA = (G1XYZZ*)ctx->slot(S_PR_SUMS, s.sums);
     if (!b.W || !b.rs_m || !b.abc || !b.bsc || !b.sorted || !b.counts || !b.offsets || !b.cursor || !b.heavy || !b.bk2 || !b.lvl2 || !b.totA)
         return OG_E_NOMEM;
     b.aff1 = b.aff2 = nullptr;
     if (affine_mode()) {
-        size_t need = 0;
-        if (affine_mode() & 1) need = msm_aff_scratch_bytes_g1(n_keys);
-        if ((affine_mode() & 2) && msm_aff_scratch_bytes_g2((size_t)B * pk->nb[1]) > need) need = msm_aff_scratch_bytes_g2((size_t)B * pk->nb[1]);
-        void* a = ctx->slot(S(S_PR_AFF, S_L1_AFF), need);
+        void* a = ctx->slot(S(S_PR_AFF, S_L1_AFF), s.aff);
         if (!a) return OG_E_NOMEM;
         if (affine_mode() & 1) b.aff1 = a;
         if (affine_mode() & 2) b.aff2 = a;
     }
     b.ntt_tmp = b.abc + (size_t)B * 3 * m;
     b.csc = b.bsc + (size_t)B * b.bsc_stride;
-    // The sort's staging lives in the bucket array: nothing writes it before the accumulation of the same MSM, and the
-    // previous MSM's reduction, which reads it, runs earlier on the same stream.  Its per-tile counters live in the heavy-bucket
-    // scratch, which msm_buckets uses only after the sort.
-    const uint32_t n_pts[3] = {pk->nA, pk->nB, pk->nC};
-    size_t stage = msm_sort_stage_bytes((size_t)B * max_pts * pk->max_windows), tiles = 0;
-    for (int k = 0; k < 3; k++) { size_t t = msm_sort_tile_bytes(B, pk->nb[k], n_pts[k]); if (t > tiles) tiles = t; }
-    b.sort_stage = stage <= sizeof(G2XYZZ) * n_keys ? (uint32_t*)b.bk2 : (uint32_t*)ctx->slot(S(S_PR_SORT_STAGE, S_L1_SORT_STAGE), stage);
-    b.sort_tiles = tiles <= 4 * (2 * n_keys + 4) ? b.heavy : (uint32_t*)ctx->slot(S(S_PR_SORT_TILES, S_L1_SORT_TILES), tiles);
+    b.sort_stage = !s.stage ? (uint32_t*)b.bk2 : (uint32_t*)ctx->slot(S(S_PR_SORT_STAGE, S_L1_SORT_STAGE), s.stage);
+    b.sort_tiles = !s.tiles ? b.heavy : (uint32_t*)ctx->slot(S(S_PR_SORT_TILES, S_L1_SORT_TILES), s.tiles);
     if (!b.sort_stage || !b.sort_tiles) return OG_E_NOMEM;
     b.bk1 = reinterpret_cast<G1XYZZ*>(b.bk2);       // the G1 and G2 MSMs of a chunk run one after another
     b.lvl1 = reinterpret_cast<G1XYZZ*>(b.lvl2);
@@ -440,11 +471,13 @@ static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
 
 // where a chunk's witness rows come from
 struct WitnessSource {
-    enum Kind { WITHDRAW, DEPOSIT, FULL } kind = FULL;
+    enum Kind { WITHDRAW, DEPOSIT, TRANSFER, FULL } kind = FULL;
     const uint8_t *d_null = nullptr, *d_sec = nullptr;                       // secret inputs (prove_withdraw, prove_deposit)
     const uint8_t *d_rec = nullptr, *d_sib = nullptr;                        // withdraw: recipients, siblings
     const uint32_t* d_bits = nullptr;
     const uint8_t* d_dep = nullptr;                                          // deposit: depositors
+    TransferInputs tin = {};                                                 // transfer: every input array
+    uint32_t transfer_depth = 0;
     const uint8_t* d_wit = nullptr;                                          // or full witnesses (prove)
     uint8_t* d_public = nullptr;
 };
@@ -463,8 +496,11 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
             WithdrawLayout L = WithdrawLayout::make(pk->depth);
             OG_TRY(withdraw_witness_strided_dev(ctx, L, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_rec + 32ull * off,
                                                 src.d_sib + 32ull * off * pk->depth, src.d_bits + off, B, W));
-        } else {
+        } else if (src.kind == WitnessSource::DEPOSIT) {
             OG_TRY(deposit_witness_strided_dev(ctx, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_dep + 32ull * off, B, W));
+        } else {
+            TransferLayout L = TransferLayout::make(src.transfer_depth);
+            OG_TRY(transfer_witness_strided_dev(ctx, L, b.w_stride, src.tin.at(off, src.transfer_depth), B, W));
         }
         if (src.d_public) OG_LAUNCH(ctx, k_public_out, (B * pk->n_pub + 127) / 128, 128, 0, W, b.w_stride, B, pk->n_pub, src.d_public + 32ull * off * pk->n_pub);
     }
@@ -494,19 +530,38 @@ static uint32_t chunk_limit(const og_pk* pk) {
     return (uint32_t)(lim < 1 ? 1 : lim);
 }
 
-// OG_CHUNK proofs per chunk (default 1024 = the whole BASELINE batch, ~28 GB of scratch per lane, which the 80 GB of an H100 holds), OG_LANES chunks in flight (default 2, 1 = serial)
-static uint32_t chunk_size(const og_pk* pk, uint32_t batch) {
-    uint32_t c = env_u32("OG_CHUNK", 1024);
+// Scratch budget of one lane for the default chunk (DESIGN.md section 6).  A fixed constant, not the free memory, so that a
+// key's plan is deterministic: the depth-32 withdraw key (~27.5 GB per 1024 proofs) and the deposit key keep 1024-proof
+// chunks, a larger key gets fewer proofs per chunk, and two lanes plus the key's tables fit in the 80 GB of an H100.
+constexpr uint64_t LANE_SCRATCH_BUDGET = 28ull << 30;
+
+// OG_CHUNK proofs per chunk (default min(1024, budget / the scratch of one proof)), OG_LANES chunks in flight (default 2,
+// 1 = serial); both bounded by the batch
+static void prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes) {
+    const uint64_t by_budget = LANE_SCRATCH_BUDGET / prover_scratch(pk, 1, 1).lane();
+    uint32_t c = env_u32("OG_CHUNK", by_budget < 1 ? 1 : (by_budget < 1024 ? (uint32_t)by_budget : 1024));
     if (c > chunk_limit(pk)) c = chunk_limit(pk);
-    return c < batch ? c : batch;
+    if (c > batch) c = batch;
+    *chunk = c;
+    if (batch == 0) { *lanes = 0; return; }
+    const uint32_t n_chunks = (batch + c - 1) / c;
+    uint32_t l = env_u32("OG_LANES", MAX_LANES);
+    if (l > (uint32_t)MAX_LANES) l = MAX_LANES;
+    *lanes = l < n_chunks ? l : n_chunks;
+}
+
+void pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {
+    uint32_t c, l;
+    prover_plan(pk, batch, &c, &l);
+    if (chunk) *chunk = c;
+    if (lanes) *lanes = l;
+    if (scratch_bytes_per_lane) *scratch_bytes_per_lane = c ? prover_scratch(pk, batch, c).lane() : 0;
 }
 
 static int32_t prove_batch(og_ctx* ctx, const og_pk* pk, const WitnessSource& src, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs) {
-    const uint32_t CB = chunk_size(pk, batch);
+    uint32_t CB, lanes;
+    prover_plan(pk, batch, &CB, &lanes);
     const uint32_t n_chunks = (batch + CB - 1) / CB;
-    uint32_t lanes = env_u32("OG_LANES", MAX_LANES);
-    if (lanes > (uint32_t)MAX_LANES) lanes = MAX_LANES;
-    if (lanes > n_chunks) lanes = n_chunks;
     ChunkBufs bufs[MAX_LANES];
     for (uint32_t l = 0; l < lanes; l++) OG_TRY(alloc_chunk(ctx, pk, batch, CB, (int)l, bufs[l]));
     OG_TRY(ntt_prepare(ctx, pk->log_m));
@@ -560,6 +615,26 @@ int32_t prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, c
     return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
 }
 
+uint32_t pk_transfer_depth(const og_pk* pk) {
+    if (pk->n_pub != TRANSFER_N_PUB) return 0;
+    for (uint32_t d = 1; d <= 32; d++) {
+        TransferLayout L = TransferLayout::make(d);
+        if (pk->n_vars == L.n_vars && pk->n_constraints == L.n_constraints) return d;
+    }
+    return 0;
+}
+
+int32_t prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const TransferInputs& in, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
+                           uint8_t* d_public) {
+    const uint32_t depth = pk_transfer_depth(pk);
+    if (depth == 0) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    WitnessSource src;
+    src.kind = WitnessSource::TRANSFER;
+    src.tin = in; src.transfer_depth = depth; src.d_public = d_public;
+    return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
+}
+
 int32_t prove_witness_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs) {
     if (batch == 0) return OG_OK;
     WitnessSource src;
@@ -599,6 +674,16 @@ int32_t deposit_witness_bytes_dev(og_ctx* ctx, const uint8_t* d_null, const uint
     Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
     if (!W) return OG_E_NOMEM;
     OG_TRY(deposit_witness_strided_dev(ctx, L.n_vars, d_null, d_sec, d_dep, batch, W));
+    uint64_t tot = (uint64_t)batch * L.n_vars;
+    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
+    return OG_OK;
+}
+
+int32_t transfer_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const TransferInputs& in, uint32_t batch, uint8_t* d_out) {
+    TransferLayout L = TransferLayout::make(depth);
+    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
+    if (!W) return OG_E_NOMEM;
+    OG_TRY(transfer_witness_strided_dev(ctx, L, L.n_vars, in, batch, W));
     uint64_t tot = (uint64_t)batch * L.n_vars;
     OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
     return OG_OK;

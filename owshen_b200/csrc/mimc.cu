@@ -1,6 +1,6 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
-// paths (BASELINE config 2), level-by-level tree build, and the witness generators of the withdraw
-// and deposit statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
+// paths (BASELINE config 2), level-by-level tree build, and the witness generators of the withdraw,
+// deposit and transfer statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -173,6 +173,88 @@ __global__ void __launch_bounds__(32) k_deposit_witness(DepositLayout L, uint32_
     w[1] = cm;
 }
 
+// A note's amount (< 2^64), its 64 bits and its commitment MultiMiMC7([nullifier, secret, token, amount], 0), every round
+// value written into the note block v.  Returns the commitment.
+__device__ __forceinline__ Fr transfer_note(const TransferLayout& L, Fr* v, const Fr& nu, const Fr& se, const Fr& token, uint64_t amount,
+                                            uint32_t cm, uint32_t cm_out) {
+    const Fr one = Fr::one(), zero = Fr::zero();
+    uint32_t c[8] = {(uint32_t)amount, (uint32_t)(amount >> 32), 0, 0, 0, 0, 0, 0};
+    Fr am = Fr::from_canonical(c);
+    v[0] = nu; v[1] = se; v[2] = am;
+#pragma unroll 8
+    for (uint32_t k = 0; k < TRANSFER_AMOUNT_BITS; k++) v[3 + k] = ((amount >> k) & 1) ? one : zero;
+    const Fr xs[4] = {nu, se, token, am};
+    Fr r = zero;
+#pragma unroll 1
+    for (int k = 0; k < 4; k++) r = r + xs[k] + mimc7_hash<true>(xs[k], r, v + cm + k * L.perm);
+    v[cm_out] = r;
+    return r;
+}
+
+// Witness of the transfer statement, layout of DESIGN.md section 3 (== oracle/transfer_circuit.py); row p starts at
+// W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with four warps, one per independent hash chain of a proof, so
+// no warp diverges and a proof's critical path is one input's commitment and Merkle path (4 + 2 * depth permutations, about
+// one withdraw path):
+//   warps 0, 1   input i: amount bits, commitment, the depth levels
+//   warps 2, 3   input j - 2's nullifier hash, then output j - 2: amount bits, commitment
+// After the barrier, warp 0 writes the proof's remaining scalars (public amount, recipient, nh_diff_inv).
+__global__ void __launch_bounds__(128) k_transfer_witness(TransferLayout L, uint32_t w_stride, TransferInputs in, uint32_t batch,
+                                                          Fr* __restrict__ W, int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    const bool active = p < batch;
+    Fr* w = W + (uint64_t)p * w_stride;
+    const Fr one = Fr::one();
+    if (active) {
+        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+        if (role < 2) {
+            const uint32_t i = role;
+            Fr* v = w + L.inp(i);
+            Fr nu = load_canonical<Fr>(in.in_null + 64ull * p + 32 * i, flag);
+            Fr se = load_canonical<Fr>(in.in_sec + 64ull * p + 32 * i, flag);
+            Fr cur = transfer_note(L, v, nu, se, token, in.in_amounts[2ull * p + i], L.in_cm, L.in_cm_out);
+            const uint32_t bits = in.in_bits[2ull * p + i];
+            const uint8_t* sp = in.in_sib + 32ull * L.depth * (2ull * p + i);
+#pragma unroll 1
+            for (uint32_t l = 0; l < L.depth; l++) {
+                Fr* lv = v + L.lvl_base + l * L.lvl_size;
+                Fr sib = load_canonical<Fr>(sp + 32 * l, flag);
+                bool right = (bits >> l) & 1;
+                Fr a = right ? sib : cur;
+                Fr b = right ? cur : sib;
+                lv[0] = sib;
+                lv[1] = right ? one : Fr::zero();
+                lv[2] = a;
+                cur = mimc7_hash2<true>(a, b, lv + 3, lv + 3 + L.perm);
+                lv[3 + 2 * L.perm] = cur;
+            }
+        } else {
+            const uint32_t j = role - 2;
+            // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
+            Fr* v = w + L.inp(j);
+            Fr nu = load_canonical<Fr>(in.in_null + 64ull * p + 32 * j, flag);
+            w[5 + j] = one + nu + mimc7_hash<true>(nu, one, v + L.nh_perm);
+            Fr* o = w + L.out(j);
+            Fr onu = load_canonical<Fr>(in.out_null + 64ull * p + 32 * j, flag);
+            Fr ose = load_canonical<Fr>(in.out_sec + 64ull * p + 32 * j, flag);
+            w[7 + j] = transfer_note(L, o, onu, ose, token, in.out_amounts[2ull * p + j], L.out_cm, L.out_cm_out);
+        }
+        if (role == 0) {
+            Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+            w[0] = one;
+            w[1] = load_canonical<Fr>(in.roots + 32ull * p, flag);
+            w[3] = token; w[4] = re;
+            w[9] = re.sqr();
+        }
+    }
+    __syncthreads();   // warps 1..3 wrote the amounts and nullifier hashes read below
+    if (active && role == 0) {
+        Fr a_in = w[L.inp(0) + 2] + w[L.inp(1) + 2], a_out = w[L.out(0) + 2] + w[L.out(1) + 2];
+        w[2] = a_out - a_in;
+        w[10] = (w[5] - w[6]).inv();   // inv(0) = 0: two inputs with one nullifier leave the row unsatisfiable
+    }
+}
+
 // ---- host side ------------------------------------------------------------------------------------
 void mimc_constants_host(Fr* out91) { mimc7_round_constants(out91); }
 
@@ -246,6 +328,14 @@ int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_
     DepositLayout L = DepositLayout::make();
     if (w_stride < L.n_vars) return OG_E_INVALID;
     OG_LAUNCH(ctx, k_deposit_witness, (batch + 31) / 32, 32, 0, L, w_stride, d_null, d_sec, d_dep, batch, d_W, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint32_t w_stride, const TransferInputs& in, uint32_t batch,
+                                     Fr* d_W) {
+    if (batch == 0) return OG_OK;
+    if (w_stride < L.n_vars) return OG_E_INVALID;
+    OG_LAUNCH(ctx, k_transfer_witness, (batch + 31) / 32, 128, 0, L, w_stride, in, batch, d_W, ctx->d_flag);
     return OG_OK;
 }
 

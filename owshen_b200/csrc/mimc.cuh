@@ -1,6 +1,6 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw and deposit statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout
-// and oracle/deposit_circuit.py: Layout).
+// withdraw, deposit and transfer statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
+// oracle/deposit_circuit.py: Layout and oracle/transfer_circuit.py: Layout).
 #pragma once
 #include "common.cuh"
 
@@ -40,6 +40,59 @@ struct DepositLayout {
     }
 };
 
+constexpr uint32_t TRANSFER_N_PUB = 8;
+constexpr uint32_t TRANSFER_AMOUNT_BITS = 64;
+
+// 0 ONE | 1 root | 2 public_amount | 3 token | 4 recipient | 5, 6 nh[2] | 7, 8 out_cm[2] | 9 recipient_sq | 10 nh_diff_inv
+// | input blocks 0, 1 | output blocks 0, 1 (oracle/transfer_circuit.py).  A note block starts with nullifier, secret, amount
+// and the 64 amount bits; offsets below are relative to the block.
+struct TransferLayout {
+    uint32_t depth, perm;
+    uint32_t in_base, in_size, out_base, out_size;
+    uint32_t nh_perm, in_cm, in_cm_out, lvl_base, lvl_size;   // input block
+    uint32_t out_cm, out_cm_out;                              // output block
+    uint32_t n_vars, n_constraints;
+    static TransferLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        TransferLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        const uint32_t P = L.perm;
+        L.lvl_size = 2 * P + 4;
+        L.nh_perm = 67; L.in_cm = 67 + P; L.in_cm_out = 67 + 5 * P; L.lvl_base = 68 + 5 * P;
+        L.out_cm = 67; L.out_cm_out = 67 + 4 * P;
+        L.in_base = 11;
+        L.in_size = 68 + 5 * P + depth * L.lvl_size;
+        L.out_size = 68 + 4 * P;
+        L.out_base = L.in_base + 2 * L.in_size;
+        L.n_vars = L.out_base + 2 * L.out_size;
+        L.n_constraints = 273 + 18 * P + depth * (4 * P + 6);
+        return L;
+    }
+    OG_HD uint32_t inp(uint32_t i) const { return in_base + i * in_size; }
+    OG_HD uint32_t out(uint32_t j) const { return out_base + j * out_size; }
+};
+
+// the caller's inputs of a batch of transfers; per proof, input (output) 0 then 1 in the in_* (out_*) arrays,
+// in_siblings holds 2 * depth elements (input 0's path, then input 1's) and in_path_bits 2 words
+struct TransferInputs {
+    const uint8_t *roots, *tokens, *recipients;
+    const uint8_t *in_null, *in_sec;
+    const uint64_t* in_amounts;
+    const uint8_t* in_sib;
+    const uint32_t* in_bits;
+    const uint8_t *out_null, *out_sec;
+    const uint64_t* out_amounts;
+    // the same inputs from proof `off` on
+    TransferInputs at(uint32_t off, uint32_t depth) const {
+        TransferInputs t = *this;
+        t.roots += 32ull * off; t.tokens += 32ull * off; t.recipients += 32ull * off;
+        t.in_null += 64ull * off; t.in_sec += 64ull * off; t.in_amounts += 2ull * off;
+        t.in_sib += 64ull * depth * off; t.in_bits += 2ull * off;
+        t.out_null += 64ull * off; t.out_sec += 64ull * off; t.out_amounts += 2ull * off;
+        return t;
+    }
+};
+
 int32_t mimc_hash2_dev(og_ctx* ctx, const uint8_t* d_l, const uint8_t* d_r, uint64_t n, uint8_t* d_out);
 int32_t mimc_merkle_paths_dev(og_ctx* ctx, const uint8_t* d_leaves, const uint8_t* d_siblings, const uint32_t* d_bits,
                               uint32_t n_paths, uint32_t depth, uint8_t* d_out);
@@ -52,6 +105,8 @@ int32_t withdraw_witness_strided_dev(og_ctx* ctx, const WithdrawLayout& L, uint3
                                      const uint8_t* d_rec, const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, Fr* d_W);
 int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep,
                                     uint32_t batch, Fr* d_W);
+int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint32_t w_stride, const TransferInputs& in, uint32_t batch,
+                                     Fr* d_W);
 
 // BabyJubJub batch verification (bjj_impl.cuh); out[i] in {0, 1, 2 = public key does not decompress}
 int32_t bjj_verify_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_odd, const uint8_t* d_msgs, const uint8_t* d_sigs,

@@ -1,8 +1,8 @@
-// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw and deposit statements'
+// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit and transfer statements'
 // R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these are the
 // product's own definitions, checked entry for entry against the independently written
-// oracle/withdraw_circuit.py and oracle/deposit_circuit.py through og_withdraw_r1cs_export and
-// og_deposit_r1cs_export.
+// oracle/withdraw_circuit.py, oracle/deposit_circuit.py and oracle/transfer_circuit.py through
+// og_withdraw_r1cs_export, og_deposit_r1cs_export and og_transfer_r1cs_export.
 //
 // withdraw
 //   public : root, nullifier_hash, recipient
@@ -13,6 +13,11 @@
 //   public : commitment, depositor
 //   private: nullifier, secret
 //   commitment = MultiMiMC7([nullifier, secret], 0) (the withdraw statement's leaf); depositor^2 bound.
+// transfer
+//   public : root, public_amount, token, recipient, nullifier_hash[2], out_commitment[2]
+//   private: two input notes (nullifier, secret, amount, siblings[depth], bits[depth]), two output notes
+//   note commitment = MultiMiMC7([nullifier, secret, token, amount], 0), amounts range-checked to 64 bits;
+//   nonzero inputs open under root; in0 + in1 + public_amount = out0 + out1; nh[0] != nh[1]; recipient^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -77,13 +82,19 @@ struct Mimc7Builder {
         }
         return lc_sum({&prev, &k});
     }
+    // MultiMiMC7(xs, key): r = key; r = r + x + hash(x, r) per input, the i-th permutation's rounds at bases[i];
+    // then r * ONE = out
+    void multi_hash(std::initializer_list<const LC*> xs, const LC& key, std::initializer_list<uint32_t> bases, uint32_t out) {
+        LC r = key;
+        const uint32_t* base = bases.begin();
+        for (const LC* x : xs) {
+            LC h = perm(*x, r, *base++);
+            r = lc_sum({&r, x, &h});
+        }
+        cs.add(r, lc_var(0), lc_var(out));
+    }
     void hash2(const LC& left, const LC& right, uint32_t perm1, uint32_t perm2, uint32_t out) {
-        LC zero;
-        LC h1 = perm(left, zero, perm1);
-        LC r1 = lc_sum({&left, &h1});
-        LC h2 = perm(right, r1, perm2);
-        LC r2 = lc_sum({&r1, &right, &h2});
-        cs.add(r2, lc_var(0), lc_var(out));
+        multi_hash({&left, &right}, LC(), {perm1, perm2}, out);
     }
 };
 
@@ -95,11 +106,8 @@ struct WithdrawBuilder {
         b.cs.n_pub = WITHDRAW_N_PUB;
         const uint32_t V_ONE = 0, V_ROOT = 1, V_NHASH = 2, V_RECIP = 3, V_NULL = 4, V_SECRET = 5, V_RSQ = 6, V_NH_PERM = 7;
         b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
-        {
-            LC h = b.perm(lc_var(V_NULL), lc_var(V_ONE), V_NH_PERM);
-            LC one = lc_var(V_ONE), nu = lc_var(V_NULL);
-            b.cs.add(lc_sum({&one, &nu, &h}), lc_var(V_ONE), lc_var(V_NHASH));
-        }
+        LC nu = lc_var(V_NULL);
+        b.multi_hash({&nu}, lc_var(V_ONE), {V_NH_PERM}, V_NHASH);
         b.hash2(lc_var(V_NULL), lc_var(V_SECRET), L.cm_base, L.cm_base + L.perm, L.cm_out);
         uint32_t cur = L.cm_out;
         for (uint32_t l = 0; l < depth; l++) {
@@ -130,6 +138,70 @@ struct DepositBuilder {
         b.hash2(lc_var(V_NULL), lc_var(V_SECRET), L.cm_base, L.cm_base + L.perm, L.cm_out);
         LC vout = lc_var(L.cm_out), ncm = lc_neg_var(V_CM);
         b.cs.add(lc_sum({&vout, &ncm}), lc_var(V_ONE), LC());
+        return b.cs;
+    }
+};
+
+struct TransferBuilder {
+    // the 64 range rows bit_k * (bit_k - ONE) = 0 and (sum 2^k bit_k - amount) * ONE = 0 of the note block at `v`
+    static void range(Mimc7Builder& b, uint32_t v) {
+        LC m1 = lc_neg_var(0), packed = lc_neg_var(v + 2);
+        Fr pow2 = Fr::one();
+        for (uint32_t k = 0; k < TRANSFER_AMOUNT_BITS; k++) {
+            LC vbit = lc_var(v + 3 + k);
+            b.cs.add(vbit, lc_sum({&vbit, &m1}), LC());
+            lc_add_term(packed, v + 3 + k, pow2);
+            pow2 = pow2 + pow2;
+        }
+        b.cs.add(packed, lc_var(0), LC());
+    }
+    // commitment = MultiMiMC7([nullifier, secret, token, amount], 0) of the note block at `v`, rounds from `cm`
+    static void commitment(Mimc7Builder& b, uint32_t v, uint32_t cm, uint32_t cm_out, uint32_t P) {
+        LC nu = lc_var(v), se = lc_var(v + 1), tok = lc_var(3), am = lc_var(v + 2);
+        b.multi_hash({&nu, &se, &tok, &am}, LC(), {cm, cm + P, cm + 2 * P, cm + 3 * P}, cm_out);
+    }
+
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        TransferLayout L = TransferLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = TRANSFER_N_PUB;
+        const uint32_t V_ONE = 0, V_ROOT = 1, V_PUB_AMOUNT = 2, V_RECIP = 4, V_NH = 5, V_OUT_CM = 7, V_RSQ = 9, V_NH_INV = 10;
+        const uint32_t P = L.perm;
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        for (uint32_t i = 0; i < 2; i++) {
+            const uint32_t v = L.inp(i);
+            LC nu = lc_var(v);
+            b.multi_hash({&nu}, lc_var(V_ONE), {v + L.nh_perm}, V_NH + i);
+            range(b, v);
+            commitment(b, v, v + L.in_cm, v + L.in_cm_out, P);
+            uint32_t cur = v + L.in_cm_out;
+            for (uint32_t l = 0; l < depth; l++) {
+                uint32_t base = v + L.lvl_base + l * L.lvl_size;
+                uint32_t sib = base, bit = base + 1, left = base + 2, p1 = base + 3, p2 = base + 3 + P, out = base + 3 + 2 * P;
+                LC vbit = lc_var(bit), m1 = lc_neg_var(V_ONE), vsib = lc_var(sib), ncur = lc_neg_var(cur), vleft = lc_var(left), vcur = lc_var(cur);
+                LC nleft = lc_neg_var(left);
+                b.cs.add(vbit, lc_sum({&vbit, &m1}), LC());
+                b.cs.add(vbit, lc_sum({&vsib, &ncur}), lc_sum({&vleft, &ncur}));
+                LC right = lc_sum({&vsib, &vcur, &nleft});
+                b.hash2(vleft, right, p1, p2, out);
+                cur = out;
+            }
+            LC vroot = lc_var(V_ROOT), ncur = lc_neg_var(cur);
+            b.cs.add(lc_sum({&vroot, &ncur}), lc_var(v + 2), LC());
+        }
+        for (uint32_t j = 0; j < 2; j++) {
+            const uint32_t v = L.out(j);
+            range(b, v);
+            commitment(b, v, v + L.out_cm, v + L.out_cm_out, P);
+            LC vout = lc_var(v + L.out_cm_out), ncm = lc_neg_var(V_OUT_CM + j);
+            b.cs.add(lc_sum({&vout, &ncm}), lc_var(V_ONE), LC());
+        }
+        LC i0 = lc_var(L.inp(0) + 2), i1 = lc_var(L.inp(1) + 2), pa = lc_var(V_PUB_AMOUNT);
+        LC o0 = lc_neg_var(L.out(0) + 2), o1 = lc_neg_var(L.out(1) + 2);
+        b.cs.add(lc_sum({&i0, &i1, &pa, &o0, &o1}), lc_var(V_ONE), LC());
+        LC nh0 = lc_var(V_NH), nh1 = lc_neg_var(V_NH + 1);
+        b.cs.add(lc_sum({&nh0, &nh1}), lc_var(V_NH_INV), lc_var(V_ONE));
         return b.cs;
     }
 };
