@@ -261,6 +261,40 @@ int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness,
 int32_t og_groth16_verify(const uint8_t* vk, uint64_t vk_len, const uint8_t* public_inputs,
                           uint32_t n_pub, const uint8_t* proof256);
 
+/* ---- two-phase setup ceremony (DESIGN.md section 4b) ----------------------------------------------------------------
+ * Phase 1: a powers-of-tau accumulator ("OGPT" v1, log_max in [1, 24], M = 2^log_max): [tau^i]_1 (i < 2M),
+ * [alpha tau^i]_1, [beta tau^i]_1, [tau^i]_2 (i < M), [beta]_2.  og_ptau_new makes the initial one (all generators);
+ * og_ptau_contribute applies secrets (t, a, b) and writes a record ("OGPR" v1) with Schnorr proofs of knowledge made with
+ * the nonces (96 bytes each: three 32-byte scalars); og_ptau_verify checks one update against its record.
+ * og_ptau_prepare / og_ptau_prepare_withdraw derive a circuit's key (gamma = delta = 1) from an accumulator whose
+ * log_max is at least the circuit's log_m.  Phase 2: og_phase2_contribute multiplies delta by d (L and H by 1/d) and
+ * writes a record ("OGDR" v1); og_phase2_verify checks it.  Verification returns OG_OK or OG_E_VERIFY.  Outputs follow
+ * the NULL -> size convention; zero secrets or nonces, malformed blobs and m > M give OG_E_INVALID.  The library zeroes
+ * its copies of the secrets before returning. */
+int32_t og_ptau_new(og_ctx* ctx, uint32_t log_max, uint8_t* out, uint64_t* out_len);
+int32_t og_ptau_contribute(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, const uint8_t* secrets96, const uint8_t* nonces96,
+                           uint8_t* acc_out, uint64_t* acc_out_len, uint8_t* record_out, uint64_t* record_len);
+int32_t og_ptau_verify(og_ctx* ctx, const uint8_t* prev, uint64_t prev_len, const uint8_t* next, uint64_t next_len,
+                       const uint8_t* record, uint64_t record_len);
+int32_t og_ptau_prepare(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
+                        const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
+                        const uint32_t* b_row_ptr, const uint32_t* b_col, const uint8_t* b_coeffs,
+                        const uint32_t* c_row_ptr, const uint32_t* c_col, const uint8_t* c_coeffs,
+                        uint8_t* pk_out, uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len);
+int32_t og_ptau_prepare_withdraw(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, uint32_t depth, uint8_t* pk_out, uint64_t* pk_len,
+                                 uint8_t* vk_out, uint64_t* vk_len);
+int32_t og_phase2_contribute(og_ctx* ctx, const uint8_t* pk, uint64_t pk_len, const uint8_t* vk, uint64_t vk_len, const uint8_t* delta32,
+                             const uint8_t* nonce32, uint8_t* pk_out, uint64_t* pk_out_len, uint8_t* vk_out, uint64_t* vk_out_len,
+                             uint8_t* record_out, uint64_t* record_len);
+int32_t og_phase2_verify(og_ctx* ctx, const uint8_t* pk_prev, uint64_t pk_prev_len, const uint8_t* vk_prev, uint64_t vk_prev_len,
+                         const uint8_t* pk_next, uint64_t pk_next_len, const uint8_t* vk_next, uint64_t vk_next_len,
+                         const uint8_t* record, uint64_t record_len);
+/* the ceremony's point kernels: out_i = s_i P_i (per_point) or s_0 P_i over G1 (g2 = 0) or G2 (g2 = 1), and the in-place
+ * inverse NTT of 2^log_m points (omega = 7^((r-1)/m), as og_ntt) */
+int32_t og_scale_points(og_ctx* ctx, int32_t g2, const uint8_t* points, const uint8_t* scalars, uint64_t n, int32_t per_point,
+                        uint8_t* out);
+int32_t og_intt_points(og_ctx* ctx, int32_t g2, uint8_t* points, uint32_t log_m);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,8 +8,12 @@ anywhere, but creating a Context without a CUDA device raises.
 from .kvstore import KvStore, MirrorKvStore, RamKvStore
 from .api import (Context, ProvingKey, MerkleTree, OwshenB200Error, lib, build_library, prove, verify,
                   setup_withdraw, setup_r1cs, setup_deposit, deposit_r1cs_info, deposit_r1cs_export,
-                  setup_transfer, transfer_r1cs_info, transfer_r1cs_export, FR_MODULUS, PROOF_BYTES)
+                  setup_transfer, transfer_r1cs_info, transfer_r1cs_export, FR_MODULUS, PROOF_BYTES,
+                  ptau_new, ptau_contribute, ptau_verify, ptau_prepare, ptau_prepare_withdraw, ptau_prepare_deposit,
+                  ptau_prepare_transfer, phase2_contribute, phase2_verify)
 
 __all__ = ["Context", "ProvingKey", "MerkleTree", "OwshenB200Error", "lib", "build_library", "prove", "verify",
            "setup_withdraw", "setup_r1cs", "setup_deposit", "deposit_r1cs_info", "deposit_r1cs_export",
-           "setup_transfer", "transfer_r1cs_info", "transfer_r1cs_export", "FR_MODULUS", "PROOF_BYTES", "KvStore", "RamKvStore", "MirrorKvStore"]
+           "setup_transfer", "transfer_r1cs_info", "transfer_r1cs_export", "FR_MODULUS", "PROOF_BYTES", "KvStore", "RamKvStore", "MirrorKvStore",
+           "ptau_new", "ptau_contribute", "ptau_verify", "ptau_prepare", "ptau_prepare_withdraw", "ptau_prepare_deposit",
+           "ptau_prepare_transfer", "phase2_contribute", "phase2_verify"]

@@ -8,6 +8,7 @@ All hashing, witness generation, NTTs and MSMs run in the CUDA library; nothing 
 """
 import ctypes as C
 import os
+import secrets as _rand
 import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -103,6 +104,20 @@ _SIGS = {
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
+    "og_ptau_new": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_ptau_contribute": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_ptau_verify": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]),
+    "og_ptau_prepare": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
+                        + [C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_ptau_prepare_withdraw": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                             C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_phase2_contribute": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64),
+                                         C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_phase2_verify": (C.c_int32, [C.c_void_p] + [C.c_void_p, C.c_uint64] * 5),
+    "og_scale_points": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int32, C.c_void_p]),
+    "og_intt_points": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
 }
 ABI_SYMBOLS = tuple(_SIGS)
 
@@ -500,10 +515,8 @@ def transfer_r1cs_export(depth: int, which: str):
     return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
 
 
-def setup_r1cs(ctx: Context, n_vars: int, n_pub: int, A, B, C_, tau: int, alpha: int, beta: int, gamma: int, delta: int):
-    """Development setup of any R1CS -> (pk_bytes, vk_bytes).  A, B, C_ are (row_ptr, col_idx, coeffs) triples as
-    r1cs_export returns them (coefficients as ints or 32-byte little-endian values); variable 0 is ONE and variables
-    1..n_pub are the public inputs.  The key records depth 0, so it proves through prove_witnesses."""
+def _r1cs_args(A, B, C_):
+    """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
     n_constraints = None
     for name, M in (("A", A), ("B", B), ("C", C_)):
@@ -518,6 +531,14 @@ def setup_r1cs(ctx: Context, n_vars: int, n_pub: int, A, B, C_, tau: int, alpha:
         cb = b"".join(bytes(x) if isinstance(x, (bytes, bytearray)) else int(x).to_bytes(32, "little") for x in val)
         _need(len(cb) == 32 * len(val), f"setup_r1cs: {name} coefficients are 32 bytes each")
         mats += [(C.c_uint32 * len(ptr))(*ptr), (C.c_uint32 * max(1, len(col)))(*col), cb]
+    return n_constraints, mats
+
+
+def setup_r1cs(ctx: Context, n_vars: int, n_pub: int, A, B, C_, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of any R1CS -> (pk_bytes, vk_bytes).  A, B, C_ are (row_ptr, col_idx, coeffs) triples as
+    r1cs_export returns them (coefficients as ints or 32-byte little-endian values); variable 0 is ONE and variables
+    1..n_pub are the public inputs.  The key records depth 0, so it proves through prove_witnesses."""
+    n_constraints, mats = _r1cs_args(A, B, C_)
     toxic = b"".join(fr_bytes(x) for x in (tau, alpha, beta, gamma, delta))
     pl, vl = C.c_uint64(), C.c_uint64()
     _check(lib().og_groth16_setup(ctx._h, n_constraints, n_vars, n_pub, *mats, toxic, None, C.byref(pl), None, C.byref(vl)), ctx)
@@ -550,6 +571,84 @@ def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, ga
     vk = C.create_string_buffer(vl.value)
     _check(lib().og_groth16_setup_withdraw(ctx._h, depth, toxic, pk, C.byref(pl), vk, C.byref(vl)), ctx)
     return pk.raw[:pl.value], vk.raw[:vl.value]
+
+
+# ---- two-phase setup ceremony (DESIGN.md section 4b) -------------------------------------------------------------------
+def _sized(ctx, fn, n_out=1):
+    """Call fn(*out_args) twice (NULL -> sizes, then the buffers) and return its n_out blobs."""
+    lens = [C.c_uint64() for _ in range(n_out)]
+    _check(fn(*[a for x in lens for a in (None, C.byref(x))]), ctx)
+    bufs = [C.create_string_buffer(x.value) for x in lens]
+    _check(fn(*[a for b, x in zip(bufs, lens) for a in (b, C.byref(x))]), ctx)
+    out = [b.raw[:x.value] for b, x in zip(bufs, lens)]
+    return out[0] if n_out == 1 else tuple(out)
+
+
+def _secrets(xs, n, name):
+    if xs is None:
+        return [_rand.randbelow(FR_MODULUS - 1) + 1 for _ in range(n)]
+    xs = list(xs)
+    _need(len(xs) == n, f"{name}: expected {n} values")
+    return xs
+
+
+def ptau_new(ctx: Context, log_max: int) -> bytes:
+    """The initial powers-of-tau accumulator of size M = 2^log_max (every point a generator)."""
+    return _sized(ctx, lambda *io: lib().og_ptau_new(ctx._h, log_max, *io))
+
+
+def ptau_contribute(ctx: Context, acc: bytes, secrets=None, nonces=None):
+    """Apply secrets (t, a, b) to an accumulator -> (new accumulator, record).  Secrets and nonces are drawn with the
+    `secrets` module when not given; given ones make every byte reproducible."""
+    s = _secrets(secrets, 3, "ptau_contribute: secrets")
+    k = _secrets(nonces, 3, "ptau_contribute: nonces")
+    sb, kb = b"".join(fr_bytes(x) for x in s), b"".join(fr_bytes(x) for x in k)
+    return _sized(ctx, lambda *io: lib().og_ptau_contribute(ctx._h, acc, len(acc), sb, kb, *io), n_out=2)
+
+
+def ptau_verify(ctx: Context, prev: bytes, nxt: bytes, record: bytes) -> bool:
+    """True iff `nxt` is `prev` updated by the contribution that `record` proves knowledge of."""
+    rc = lib().og_ptau_verify(ctx._h, prev, len(prev), nxt, len(nxt), record, len(record))
+    if rc in (OG_OK, OG_E_VERIFY):
+        return rc == OG_OK
+    _check(rc, ctx)
+
+
+def ptau_prepare(ctx: Context, acc: bytes, n_vars: int, n_pub: int, A, B, C_):
+    """The phase-2 starting key (pk, vk) of any R1CS from an accumulator: arguments as setup_r1cs; the key records depth 0."""
+    n_constraints, mats = _r1cs_args(A, B, C_)
+    return _sized(ctx, lambda *io: lib().og_ptau_prepare(ctx._h, acc, len(acc), n_constraints, n_vars, n_pub, *mats, *io), n_out=2)
+
+
+def ptau_prepare_withdraw(ctx: Context, acc: bytes, depth: int):
+    """The phase-2 starting key of the depth-`depth` withdraw statement (the depth is recorded, as setup_withdraw)."""
+    return _sized(ctx, lambda *io: lib().og_ptau_prepare_withdraw(ctx._h, acc, len(acc), depth, *io), n_out=2)
+
+
+def ptau_prepare_deposit(ctx: Context, acc: bytes):
+    info = deposit_r1cs_info()
+    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(deposit_r1cs_export(m) for m in "ABC"))
+
+
+def ptau_prepare_transfer(ctx: Context, acc: bytes, depth: int):
+    info = transfer_r1cs_info(depth)
+    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(transfer_r1cs_export(depth, m) for m in "ABC"))
+
+
+def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
+    """Multiply the key's delta by a secret d -> (pk, vk, record); d and the nonce are drawn with `secrets` when not given."""
+    d = _secrets(None if delta is None else [delta], 1, "phase2_contribute: delta")[0]
+    k = _secrets(None if nonce is None else [nonce], 1, "phase2_contribute: nonce")[0]
+    return _sized(ctx, lambda *io: lib().og_phase2_contribute(ctx._h, pk, len(pk), vk, len(vk), fr_bytes(d), fr_bytes(k), *io),
+                  n_out=3)
+
+
+def phase2_verify(ctx: Context, pk_prev: bytes, vk_prev: bytes, pk_next: bytes, vk_next: bytes, record: bytes) -> bool:
+    rc = lib().og_phase2_verify(ctx._h, pk_prev, len(pk_prev), vk_prev, len(vk_prev), pk_next, len(pk_next), vk_next, len(vk_next),
+                                record, len(record))
+    if rc in (OG_OK, OG_E_VERIFY):
+        return rc == OG_OK
+    _check(rc, ctx)
 
 
 class ProvingKey:

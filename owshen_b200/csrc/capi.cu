@@ -1108,4 +1108,81 @@ int32_t og_groth16_verify(const uint8_t* vk, uint64_t vk_len, const uint8_t* pub
     return groth16_verify_host(vk, vk_len, public_inputs, n_pub, proof256);
 }
 
+// ---- setup ceremony (ceremony.cu) -------------------------------------------------------------------------------------
+int32_t og_ptau_new(og_ctx* ctx, uint32_t log_max, uint8_t* out, uint64_t* out_len) {
+    OG_ENTER(ctx);
+    return ptau_new(ctx, log_max, out, out_len);
+}
+int32_t og_ptau_contribute(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, const uint8_t* secrets96, const uint8_t* nonces96,
+                           uint8_t* acc_out, uint64_t* acc_out_len, uint8_t* record_out, uint64_t* record_len) {
+    OG_ENTER(ctx);
+    return ptau_contribute(ctx, acc, acc_len, secrets96, nonces96, acc_out, acc_out_len, record_out, record_len);
+}
+int32_t og_ptau_verify(og_ctx* ctx, const uint8_t* prev, uint64_t prev_len, const uint8_t* next, uint64_t next_len, const uint8_t* record,
+                       uint64_t record_len) {
+    OG_ENTER(ctx);
+    return ptau_verify(ctx, prev, prev_len, next, next_len, record, record_len);
+}
+int32_t og_ptau_prepare(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
+                        const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
+                        const uint32_t* b_row_ptr, const uint32_t* b_col, const uint8_t* b_coeffs,
+                        const uint32_t* c_row_ptr, const uint32_t* c_col, const uint8_t* c_coeffs,
+                        uint8_t* pk_out, uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len) {
+    OG_ENTER(ctx);
+    if (!pk_len || !vk_len) return OG_E_INVALID;
+    const uint32_t* row_ptr[3] = {a_row_ptr, b_row_ptr, c_row_ptr};
+    const uint32_t* col[3] = {a_col, b_col, c_col};
+    const uint8_t* coeffs[3] = {a_coeffs, b_coeffs, c_coeffs};
+    try {
+        R1cs cs;
+        OG_TRY(load_r1cs(n_constraints, n_vars, n_pub, row_ptr, col, coeffs, cs));
+        return ptau_prepare(ctx, acc, acc_len, cs, 0, pk_out, pk_len, vk_out, vk_len);
+    } catch (const std::bad_alloc&) {
+        snprintf(ctx->err, sizeof(ctx->err), "ptau_prepare: host allocation failed");
+        return OG_E_NOMEM;
+    }
+}
+int32_t og_ptau_prepare_withdraw(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, uint32_t depth, uint8_t* pk_out, uint64_t* pk_len,
+                                 uint8_t* vk_out, uint64_t* vk_len) {
+    OG_ENTER(ctx);
+    if (depth == 0 || depth > 32 || !pk_len || !vk_len) return OG_E_INVALID;
+    return ptau_prepare(ctx, acc, acc_len, WithdrawBuilder::build(depth), depth, pk_out, pk_len, vk_out, vk_len);
+}
+int32_t og_phase2_contribute(og_ctx* ctx, const uint8_t* pk, uint64_t pk_len, const uint8_t* vk, uint64_t vk_len, const uint8_t* delta32,
+                             const uint8_t* nonce32, uint8_t* pk_out, uint64_t* pk_out_len, uint8_t* vk_out, uint64_t* vk_out_len,
+                             uint8_t* record_out, uint64_t* record_len) {
+    OG_ENTER(ctx);
+    return phase2_contribute(ctx, pk, pk_len, vk, vk_len, delta32, nonce32, pk_out, pk_out_len, vk_out, vk_out_len, record_out, record_len);
+}
+int32_t og_phase2_verify(og_ctx* ctx, const uint8_t* pk_prev, uint64_t pk_prev_len, const uint8_t* vk_prev, uint64_t vk_prev_len,
+                         const uint8_t* pk_next, uint64_t pk_next_len, const uint8_t* vk_next, uint64_t vk_next_len, const uint8_t* record,
+                         uint64_t record_len) {
+    OG_ENTER(ctx);
+    return phase2_verify(ctx, pk_prev, pk_prev_len, vk_prev, vk_prev_len, pk_next, pk_next_len, vk_next, vk_next_len, record, record_len);
+}
+int32_t og_scale_points(og_ctx* ctx, int32_t g2, const uint8_t* points, const uint8_t* scalars, uint64_t n, int32_t per_point, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (g2 < 0 || g2 > 1 || (n && (!points || !scalars || !out))) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    const uint64_t pb = g2 ? 128 : 64, ns = per_point ? n : 1;
+    OG_SLOT(ctx, dp, uint8_t, S_IO_A, pb * n);
+    OG_SLOT(ctx, ds, uint8_t, S_IO_B, 32 * ns);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dp, points, pb * n); H2D(ctx, ds, scalars, 32 * ns);
+    OG_TRY(scale_points_dev(ctx, g2, dp, ds, n, per_point, dp));
+    D2H(ctx, out, dp, pb * n);
+    return check_flag(ctx);
+}
+int32_t og_intt_points(og_ctx* ctx, int32_t g2, uint8_t* points, uint32_t log_m) {
+    OG_ENTER(ctx);
+    if (g2 < 0 || g2 > 1 || !points || log_m > 25) return OG_E_INVALID;
+    const uint64_t pb = (g2 ? 128ull : 64ull) << log_m;
+    OG_SLOT(ctx, dp, uint8_t, S_IO_A, pb);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dp, points, pb);
+    OG_TRY(intt_points_dev(ctx, g2, dp, log_m));
+    D2H(ctx, points, dp, pb);
+    return check_flag(ctx);
+}
+
 }  // extern "C"

@@ -242,22 +242,34 @@ void pk_free(og_pk* pk) {
     delete pk;
 }
 
-int32_t pk_load(og_ctx* ctx, const uint8_t* bytes, uint64_t len, og_pk** out) {
+bool pk_layout(const uint8_t* bytes, uint64_t len, PkLayout& L) {
     Reader rd{bytes, len};
     const uint8_t* magic = rd.take(4);
-    if (!magic || memcmp(magic, "OGPK", 4) != 0) return OG_E_ENCODING;
-    if (rd.u32() != 1) return OG_E_ENCODING;
+    if (!magic || memcmp(magic, "OGPK", 4) != 0) return false;
+    if (rd.u32() != 1) return false;
+    L.depth = rd.u32(); L.n_constraints = rd.u32(); L.n_vars = rd.u32(); L.n_pub = rd.u32(); L.log_m = rd.u32();
+    if (!rd.ok || L.log_m > 24 || L.n_vars == 0 || L.n_pub > (1u << 16) || L.n_pub + 1 > L.n_vars ||
+        (uint64_t)L.n_constraints + L.n_pub + 1 > (1ull << L.log_m)) return false;
+    const uint32_t nv = L.n_vars, n_priv = nv - L.n_pub - 1, m = 1u << L.log_m;
+    auto at = [&](uint64_t n) { const uint8_t* p = rd.take(n); return p ? (uint64_t)(p - bytes) : 0; };
+    L.alpha1 = at(64); L.beta1 = at(64); L.beta2 = at(128); L.delta1 = at(64); L.delta2 = at(128);
+    L.qa = at(64ull * nv); L.qb1 = at(64ull * nv); L.qb2 = at(128ull * nv); L.ql = at(64ull * n_priv); L.qh = at(64ull * m);
+    L.csr = len - rd.left;
+    return rd.ok;
+}
+
+int32_t pk_load(og_ctx* ctx, const uint8_t* bytes, uint64_t len, og_pk** out) {
+    PkLayout Lk;
+    if (!pk_layout(bytes, len, Lk)) return OG_E_ENCODING;
+    Reader rd{bytes + Lk.csr, len - Lk.csr};
     og_pk* pk = new og_pk();
     pk->device = ctx->device;
-    pk->depth = rd.u32(); pk->n_constraints = rd.u32(); pk->n_vars = rd.u32(); pk->n_pub = rd.u32(); pk->log_m = rd.u32();
-    if (!rd.ok || pk->log_m > 24 || pk->n_vars == 0 || pk->n_pub > (1u << 16) || pk->n_pub + 1 > pk->n_vars ||
-        (uint64_t)pk->n_constraints + pk->n_pub + 1 > (1ull << pk->log_m)) { delete pk; return OG_E_ENCODING; }
+    pk->depth = Lk.depth; pk->n_constraints = Lk.n_constraints; pk->n_vars = Lk.n_vars; pk->n_pub = Lk.n_pub; pk->log_m = Lk.log_m;
     const uint32_t nv = pk->n_vars, n_priv = nv - pk->n_pub - 1, m = 1u << pk->log_m;
-    const uint8_t* alpha1 = rd.take(64); const uint8_t* beta1 = rd.take(64); const uint8_t* beta2 = rd.take(128);
-    const uint8_t* delta1 = rd.take(64); const uint8_t* delta2 = rd.take(128);
-    const uint8_t* qa = rd.take(64ull * nv); const uint8_t* qb1 = rd.take(64ull * nv); const uint8_t* qb2 = rd.take(128ull * nv);
-    const uint8_t* ql = rd.take(64ull * n_priv); const uint8_t* qh = rd.take(64ull * m);
-    if (!rd.ok) { delete pk; return OG_E_ENCODING; }
+    const uint8_t* alpha1 = bytes + Lk.alpha1; const uint8_t* beta1 = bytes + Lk.beta1; const uint8_t* beta2 = bytes + Lk.beta2;
+    const uint8_t* delta1 = bytes + Lk.delta1; const uint8_t* delta2 = bytes + Lk.delta2;
+    const uint8_t* qa = bytes + Lk.qa; const uint8_t* qb1 = bytes + Lk.qb1; const uint8_t* qb2 = bytes + Lk.qb2;
+    const uint8_t* ql = bytes + Lk.ql; const uint8_t* qh = bytes + Lk.qh;
 
     // support of the B queries (v_i(tau) != 0)
     std::vector<uint32_t> supp;

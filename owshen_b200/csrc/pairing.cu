@@ -123,10 +123,18 @@ static bool g2_on_curve(const G2Affine& p) {
 }
 static bool g2_in_subgroup(const G2Affine& p) { return G2XYZZ::mul(p, FR_MODULUS).is_inf(); }
 
-static bool load_g1(G1Affine& p, const uint8_t* b) { return host_load(p.x, b) && host_load(p.y, b + 32) && g1_on_curve(p); }
-static bool load_g2(G2Affine& p, const uint8_t* b) {
+bool load_g1(G1Affine& p, const uint8_t* b) { return host_load(p.x, b) && host_load(p.y, b + 32) && g1_on_curve(p); }
+bool load_g2(G2Affine& p, const uint8_t* b) {
     return host_load(p.x.c0, b) && host_load(p.x.c1, b + 32) && host_load(p.y.c0, b + 64) && host_load(p.y.c1, b + 96) &&
            g2_on_curve(p) && g2_in_subgroup(p);
+}
+
+// prod_k e(P_k, Q_k) == 1: one Miller loop per pair, one final exponentiation
+bool pairing_product_is_one(const G1Affine* P, const G2Affine* Q, int n) {
+    Fq12 f = Fq12::one();
+    for (int k = 0; k < n; k++)
+        if (!miller_loop(f, Q[k], P[k])) return false;
+    return f12_pow(f, FINAL_EXP, 88).is_one();
 }
 
 int32_t groth16_verify_host(const uint8_t* vk, uint64_t vk_len, const uint8_t* pub, uint32_t n_pub, const uint8_t* proof) {
@@ -156,11 +164,9 @@ int32_t groth16_verify_host(const uint8_t* vk, uint64_t vk_len, const uint8_t* p
     }
     G1Affine X = acc.to_affine();
     // e(-A, B) e(alpha, beta) e(X, gamma) e(C, delta) == 1
-    Fq12 f = Fq12::one();
-    if (!miller_loop(f, B, A.neg()) || !miller_loop(f, beta2, alpha1) || !miller_loop(f, gamma2, X) || !miller_loop(f, delta2, C))
-        return OG_E_VERIFY;
-    Fq12 r = f12_pow(f, FINAL_EXP, 88);
-    return r.is_one() ? OG_OK : OG_E_VERIFY;
+    const G1Affine P[4] = {A.neg(), alpha1, X, C};
+    const G2Affine Q[4] = {B, beta2, gamma2, delta2};
+    return pairing_product_is_one(P, Q, 4) ? OG_OK : OG_E_VERIFY;
 }
 
 }  // namespace og

@@ -10,7 +10,7 @@
 
 namespace og {
 
-static Fr host_root_of_unity(uint32_t log_n) {
+Fr host_root_of_unity(uint32_t log_n) {
     uint32_t e[8];
     for (int i = 0; i < 8; i++) e[i] = FrParams::mod(i);
     e[0] -= 1;
@@ -60,6 +60,38 @@ static void put_csr(std::vector<uint8_t>& v, const Csr& M) {
     for (const Fr& c : M.val) { uint8_t b[32]; host_store(b, c); put_bytes(v, b, 32); }
 }
 
+void key_sizes(const R1cs& cs, uint64_t* pk_len, uint64_t* vk_len) {
+    const uint32_t nv = cs.n_vars, n_pub = cs.n_pub, n_priv = nv - n_pub - 1;
+    const uint32_t m = 1u << groth16_domain_log(cs.n_constraints(), n_pub);
+    const uint64_t csr_bound = 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.A.col.size() + 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.B.col.size();
+    *pk_len = 8 + 20 + 64 + 64 + 128 + 64 + 128 + 64ull * nv * 2 + 128ull * nv + 64ull * n_priv + 64ull * m + csr_bound;
+    *vk_len = 8 + 4 + 64 + 128 + 128 + 128 + 64ull * (n_pub + 1);
+}
+
+// The one pk/vk serializer: the development setup and the ceremony's key derivation both write their keys here.
+int32_t write_keys(const R1cs& cs, uint32_t depth, const KeyPoints& P, uint8_t* pk_out, uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len) {
+    const uint32_t nv = cs.n_vars, n_pub = cs.n_pub, n_priv = nv - n_pub - 1;
+    const uint32_t log_m = groth16_domain_log(cs.n_constraints(), n_pub), m = 1u << log_m;
+    uint64_t need_pk, need_vk;
+    key_sizes(cs, &need_pk, &need_vk);
+    std::vector<uint8_t> pk;
+    pk.reserve(need_pk);
+    put_bytes(pk, reinterpret_cast<const uint8_t*>("OGPK"), 4); put_u32(pk, 1);
+    put_u32(pk, depth); put_u32(pk, cs.n_constraints()); put_u32(pk, nv); put_u32(pk, n_pub); put_u32(pk, log_m);
+    put_bytes(pk, P.alpha1, 64); put_bytes(pk, P.beta1, 64); put_bytes(pk, P.beta2, 128); put_bytes(pk, P.delta1, 64); put_bytes(pk, P.delta2, 128);
+    put_bytes(pk, P.qa, 64ull * nv); put_bytes(pk, P.qb1, 64ull * nv); put_bytes(pk, P.qb2, 128ull * nv);
+    put_bytes(pk, P.ql, 64ull * n_priv); put_bytes(pk, P.qh, 64ull * m);
+    put_csr(pk, cs.A); put_csr(pk, cs.B);
+    std::vector<uint8_t> vk;
+    put_bytes(vk, reinterpret_cast<const uint8_t*>("OGVK"), 4); put_u32(vk, 1); put_u32(vk, n_pub);
+    put_bytes(vk, P.alpha1, 64); put_bytes(vk, P.beta2, 128); put_bytes(vk, P.gamma2, 128); put_bytes(vk, P.delta2, 128);
+    put_bytes(vk, P.ic, 64ull * (n_pub + 1));
+    if (pk.size() > *pk_len || vk.size() > *vk_len) return OG_E_INVALID;
+    memcpy(pk_out, pk.data(), pk.size()); *pk_len = pk.size();
+    memcpy(vk_out, vk.data(), vk.size()); *vk_len = vk.size();
+    return OG_OK;
+}
+
 // The setup of any R1CS in the library's conventions (variable 0 = ONE, 1..n_pub public).  `cs` must be well formed:
 // setup_withdraw builds it, setup_generic validates the caller's.  depth is recorded in the key (0 = not a withdraw key).
 static int32_t setup_r1cs(og_ctx* ctx, const R1cs& cs, uint32_t depth, const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len,
@@ -67,9 +99,8 @@ static int32_t setup_r1cs(og_ctx* ctx, const R1cs& cs, uint32_t depth, const uin
     const uint32_t nv = cs.n_vars, n_pub = cs.n_pub, n_priv = nv - n_pub - 1;
     const uint32_t log_m = groth16_domain_log(cs.n_constraints(), n_pub), m = 1u << log_m;
     // sizes first, so callers can allocate
-    const uint64_t csr_bound = 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.A.col.size() + 4 + 4ull * (cs.n_constraints() + 1) + 36ull * cs.B.col.size();
-    const uint64_t need_pk = 8 + 20 + 64 + 64 + 128 + 64 + 128 + 64ull * nv * 2 + 128ull * nv + 64ull * n_priv + 64ull * m + csr_bound;
-    const uint64_t need_vk = 8 + 4 + 64 + 128 + 128 + 128 + 64ull * (n_pub + 1);
+    uint64_t need_pk, need_vk;
+    key_sizes(cs, &need_pk, &need_vk);
     if (!pk_out || !vk_out) { *pk_len = need_pk; *vk_len = need_vk; return OG_OK; }
     if (*pk_len < need_pk || *vk_len < need_vk) return OG_E_INVALID;
 
@@ -125,28 +156,13 @@ static int32_t setup_r1cs(og_ctx* ctx, const R1cs& cs, uint32_t depth, const uin
     OG_CUDA(ctx, cudaMemcpyAsync(p2.data(), d_bytes, 128 * n2, cudaMemcpyDeviceToHost, ctx->stream));
     OG_TRY(check_flag(ctx));
 
-    const uint8_t* alpha1 = p1.data(); const uint8_t* beta1 = p1.data() + 64; const uint8_t* delta1 = p1.data() + 128;
-    const uint8_t* qa = p1.data() + 64 * 3; const uint8_t* qb1 = qa + 64ull * nv; const uint8_t* ql = qb1 + 64ull * nv;
-    const uint8_t* ic = ql + 64ull * n_priv; const uint8_t* qh = ic + 64ull * (n_pub + 1);
-    const uint8_t* beta2 = p2.data(); const uint8_t* delta2 = p2.data() + 128; const uint8_t* gamma2 = p2.data() + 256;
-    const uint8_t* qb2 = p2.data() + 384;
-
-    std::vector<uint8_t> pk;
-    pk.reserve(need_pk);
-    put_bytes(pk, reinterpret_cast<const uint8_t*>("OGPK"), 4); put_u32(pk, 1);
-    put_u32(pk, depth); put_u32(pk, cs.n_constraints()); put_u32(pk, nv); put_u32(pk, n_pub); put_u32(pk, log_m);
-    put_bytes(pk, alpha1, 64); put_bytes(pk, beta1, 64); put_bytes(pk, beta2, 128); put_bytes(pk, delta1, 64); put_bytes(pk, delta2, 128);
-    put_bytes(pk, qa, 64ull * nv); put_bytes(pk, qb1, 64ull * nv); put_bytes(pk, qb2, 128ull * nv);
-    put_bytes(pk, ql, 64ull * n_priv); put_bytes(pk, qh, 64ull * m);
-    put_csr(pk, cs.A); put_csr(pk, cs.B);
-    std::vector<uint8_t> vk;
-    put_bytes(vk, reinterpret_cast<const uint8_t*>("OGVK"), 4); put_u32(vk, 1); put_u32(vk, n_pub);
-    put_bytes(vk, alpha1, 64); put_bytes(vk, beta2, 128); put_bytes(vk, gamma2, 128); put_bytes(vk, delta2, 128);
-    put_bytes(vk, ic, 64ull * (n_pub + 1));
-    if (pk.size() > *pk_len || vk.size() > *vk_len) return OG_E_INVALID;
-    memcpy(pk_out, pk.data(), pk.size()); *pk_len = pk.size();
-    memcpy(vk_out, vk.data(), vk.size()); *vk_len = vk.size();
-    return OG_OK;
+    KeyPoints P;
+    P.alpha1 = p1.data(); P.beta1 = p1.data() + 64; P.delta1 = p1.data() + 128;
+    P.qa = p1.data() + 64 * 3; P.qb1 = P.qa + 64ull * nv; P.ql = P.qb1 + 64ull * nv;
+    P.ic = P.ql + 64ull * n_priv; P.qh = P.ic + 64ull * (n_pub + 1);
+    P.beta2 = p2.data(); P.delta2 = p2.data() + 128; P.gamma2 = p2.data() + 256;
+    P.qb2 = p2.data() + 384;
+    return write_keys(cs, depth, P, pk_out, pk_len, vk_out, vk_len);
 }
 
 int32_t setup_withdraw(og_ctx* ctx, uint32_t depth, const uint8_t* toxic160, uint8_t* pk_out, uint64_t* pk_len,
@@ -171,17 +187,24 @@ static int32_t load_csr(uint32_t n_rows, uint32_t n_vars, const uint32_t* row_pt
     return OG_OK;
 }
 
-int32_t setup_generic(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub, const uint32_t* const row_ptr[3],
-                      const uint32_t* const col[3], const uint8_t* const coeffs[3], const uint8_t* toxic160, uint8_t* pk_out,
-                      uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len) {
+int32_t load_r1cs(uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub, const uint32_t* const row_ptr[3], const uint32_t* const col[3],
+                  const uint8_t* const coeffs[3], R1cs& cs) {
     // the limits og_load_pk enforces: n_pub <= 2^16, n_pub + 1 <= n_vars, a domain of at most 2^24
-    if (!pk_len || !vk_len || n_constraints == 0 || n_pub > (1u << 16) || (uint64_t)n_pub + 1 > n_vars ||
+    if (n_constraints == 0 || n_pub > (1u << 16) || (uint64_t)n_pub + 1 > n_vars ||
         (uint64_t)n_constraints + n_pub + 1 > (1ull << 24)) return OG_E_INVALID;
-    R1cs cs;
     cs.n_vars = n_vars;
     cs.n_pub = n_pub;
     Csr* M[3] = {&cs.A, &cs.B, &cs.C};
     for (int k = 0; k < 3; k++) OG_TRY(load_csr(n_constraints, n_vars, row_ptr[k], col[k], coeffs[k], *M[k]));
+    return OG_OK;
+}
+
+int32_t setup_generic(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub, const uint32_t* const row_ptr[3],
+                      const uint32_t* const col[3], const uint8_t* const coeffs[3], const uint8_t* toxic160, uint8_t* pk_out,
+                      uint64_t* pk_len, uint8_t* vk_out, uint64_t* vk_len) {
+    if (!pk_len || !vk_len) return OG_E_INVALID;
+    R1cs cs;
+    OG_TRY(load_r1cs(n_constraints, n_vars, n_pub, row_ptr, col, coeffs, cs));
     return setup_r1cs(ctx, cs, 0, toxic160, pk_out, pk_len, vk_out, vk_len);
 }
 
