@@ -123,6 +123,34 @@ struct XYZZ {
     }
 };
 
+// ---- G2 mixed addition over lazily reduced Fq2 (bounds at fp.cuh: Fq2::add_lazy) ---------------------------------------
+// acc += q for a finite accumulator held by A (A.ld(c) / A.st(c, v), c = 0..3 for x, y, zz, zzz, every coordinate in
+// [0, 2p), each loaded where the formula uses it) and a finite affine q with canonical coordinates.  Returns false when the
+// sum is the point at infinity (A is then left as it was).  The formula is XYZZ::madd's; its exceptional tests ask
+// "== 0 mod p", since a lazy zero is 0 or p.  Callers make the coordinates canonical (Fq2::canonical) when a point leaves.
+template <class Acc>
+OG_HD bool g2_madd_lazy(const Acc& A, const Affine<Fq2>& q) {
+    Fq2 p = Fq2::sub_lazy(fq2_mul_lazy(q.x, A.ld(2)), A.ld(0));
+    Fq2 r = Fq2::sub_lazy(fq2_mul_lazy(q.y, A.ld(3)), A.ld(1));
+    if (p.is_zero_lazy()) {
+        if (!r.is_zero_lazy()) return false;                  // acc == -q
+        XYZZ<Fq2> d = XYZZ<Fq2>::dbl_affine(q);               // acc == q (rare): canonical values are lazy values too
+        A.st(0, d.x); A.st(1, d.y); A.st(2, d.zz); A.st(3, d.zzz);
+        return true;
+    }
+    // ordered so that few temporaries are live at a time: zz and zzz are updated as soon as pp / ppp exist
+    Fq2 pp = fq2_sqr_lazy(p);
+    A.st(2, fq2_mul_lazy(A.ld(2), pp));
+    Fq2 ppp = fq2_mul_lazy(p, pp);
+    A.st(3, fq2_mul_lazy(A.ld(3), ppp));
+    Fq2 q1 = fq2_mul_lazy(A.ld(0), pp);
+    Fq2 x3 = Fq2::sub_lazy(Fq2::sub_lazy(fq2_sqr_lazy(r), ppp), Fq2::add_lazy(q1, q1));
+    A.st(0, x3);
+    Fq2 t = fq2_mul_lazy(A.ld(1), ppp);
+    A.st(1, Fq2::sub_lazy(fq2_mul_lazy(r, Fq2::sub_lazy(q1, x3)), t));
+    return true;
+}
+
 // Out-of-line copies for kernels where a group operation is not the inner loop (reductions, table
 // builds, finalisation): one body per field instead of one per call site keeps ptxas time sane.
 #if defined(__CUDACC__)

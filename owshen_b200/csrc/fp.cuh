@@ -549,6 +549,118 @@ struct Fq2 {
     }
     OG_HD Fq2 conj() const { return Fq2{c0, c1.neg()}; }
     OG_HD Fq2 mul_fq(const Fq& s) const { return Fq2{c0 * s, c1 * s}; }
+
+    // ---- lazily reduced forms for the G2 group law (bucket accumulation, reductions) ------------------------------------
+    // Every coordinate of a lazy value lies in [0, 2p) instead of [0, p).  With p < 0.19 * 2^256 (so 4p < 2^256 and
+    // 16p^2 < 0.58 * 2^512) the bounds are:
+    //   add_lazy    a + b < 4p, one conditional subtraction of 2p                       -> [0, 2p)
+    //   sub_lazy    a - b in (-2p, 2p), 2p added on borrow                               -> [0, 2p)
+    //   sub_raw     a + 2p - b in (0, 4p), no correction (only as an operand of a wide product whose bound allows it)
+    //   mul_lazy    Karatsuba over three wide products, two reductions r < T / 2^256 + p (mont_reduce_wide_lazy):
+    //                 c0: T0 - T1 + p 2^256 with T0, T1 = a0 b0, a1 b1 < 4p^2:  T in (0, p 2^256 + 4p^2), r < 2p + 0.76p
+    //                 c1: (a0 + a1)(b0 + b1) - T0 - T1 = a0 b1 + a1 b0 < 8p^2, where the middle term itself is < 16p^2
+    //                     (sums < 4p, no correction) and fits the 512-bit product:  r < 1.52p + p
+    //               each followed by one conditional subtraction of 2p                  -> [0, 2p)
+    //   sqr_lazy    c1 = 2 red(a0 a1): red(a0 a1) < 4p^2 / 2^256 + p < 1.76p, doubled by add_lazy      -> [0, 2p)
+    //               c0 = red(u v), u = a0 + a1 reduced to [0, 2p), v = a0 + 2p - a1 in (0, 4p):
+    //                    u v < 8p^2, r < 2.52p, one conditional subtraction of 2p                  -> [0, 2p)
+    // Zero has two lazy forms per coordinate (0 and p): is_zero_lazy tests "== 0 mod p", canonical() maps to [0, p).
+    // Values in [0, p) are valid lazy values, so canonical inputs (table points, one()) enter without conversion.
+    OG_HD static void add_lazy_fq(uint32_t* r, const uint32_t* a, const uint32_t* b) {
+        CC cc;
+        r[0] = add_cc(a[0], b[0], cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) r[j] = addc_cc(a[j], b[j], cc);
+        r[7] = addc(a[7], b[7], cc);
+        cond_sub_2p<FqParams>(r);
+    }
+    OG_HD static void sub_lazy_fq(uint32_t* r, const uint32_t* a, const uint32_t* b) {
+        CC cc;
+        r[0] = sub_cc(a[0], b[0], cc);
+#pragma unroll
+        for (int j = 1; j < 8; j++) r[j] = subc_cc(a[j], b[j], cc);
+        uint32_t borrow = subc(0u, 0u, cc);
+        r[0] = add_cc(r[0], mod2<FqParams>(0) & borrow, cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) r[j] = addc_cc(r[j], mod2<FqParams>(j) & borrow, cc);
+        r[7] = addc(r[7], mod2<FqParams>(7) & borrow, cc);
+    }
+    OG_HD static void sub_raw_fq(uint32_t* r, const uint32_t* a, const uint32_t* b) {     // a + 2p - b, a, b < 2p
+        CC cc;
+        r[0] = add_cc(a[0], mod2<FqParams>(0), cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) r[j] = addc_cc(a[j], mod2<FqParams>(j), cc);
+        r[7] = addc(a[7], mod2<FqParams>(7), cc);
+        r[0] = sub_cc(r[0], b[0], cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) r[j] = subc_cc(r[j], b[j], cc);
+        r[7] = subc(r[7], b[7], cc);
+    }
+    OG_HD static bool is_zero_lazy_fq(const uint32_t* a) {
+        uint32_t z = 0, q = 0;
+#pragma unroll
+        for (int j = 0; j < 8; j++) { z |= a[j]; q |= a[j] ^ FqParams::mod(j); }
+        return z == 0 || q == 0;
+    }
+    OG_HD static Fq2 add_lazy(const Fq2& a, const Fq2& b) { Fq2 r; add_lazy_fq(r.c0.l, a.c0.l, b.c0.l); add_lazy_fq(r.c1.l, a.c1.l, b.c1.l); return r; }
+    OG_HD static Fq2 sub_lazy(const Fq2& a, const Fq2& b) { Fq2 r; sub_lazy_fq(r.c0.l, a.c0.l, b.c0.l); sub_lazy_fq(r.c1.l, a.c1.l, b.c1.l); return r; }
+    OG_HD bool is_zero_lazy() const { return is_zero_lazy_fq(c0.l) && is_zero_lazy_fq(c1.l); }
+    OG_HD Fq2 canonical() const { Fq2 r = *this; final_sub<FqParams>(r.c0.l); final_sub<FqParams>(r.c1.l); return r; }
+
+    // Operands in [0, 2p), result in [0, 2p).  Ordered so that at most two 16-limb products are live at a time: c0 is reduced
+    // before the middle product is formed.
+    OG_HD static Fq2 mul_lazy_inl(const Fq2& a, const Fq2& b) {
+        uint32_t T0[16], T1[16], S[16];
+        CC cc;
+        mul_wide(T0, a.c0.l, b.c0.l);
+        mul_wide(T1, a.c1.l, b.c1.l);
+        // S = T0 + T1 (< 8p^2);  T0 = T0 - T1 + p 2^256  (mod 2^512; the true value lies in (0, p 2^256 + 4p^2))
+        S[0] = add_cc(T0[0], T1[0], cc);
+#pragma unroll
+        for (int j = 1; j < 15; j++) S[j] = addc_cc(T0[j], T1[j], cc);
+        S[15] = addc(T0[15], T1[15], cc);
+        T0[0] = sub_cc(T0[0], T1[0], cc);
+#pragma unroll
+        for (int j = 1; j < 15; j++) T0[j] = subc_cc(T0[j], T1[j], cc);
+        T0[15] = subc(T0[15], T1[15], cc);
+        T0[8] = add_cc(T0[8], FqParams::mod(0), cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) T0[8 + j] = addc_cc(T0[8 + j], FqParams::mod(j), cc);
+        T0[15] = addc(T0[15], FqParams::mod(7), cc);
+        Fq2 r;
+        mont_reduce_wide_lazy<FqParams>(r.c0.l, T0);
+        cond_sub_2p<FqParams>(r.c0.l);
+        uint32_t sa[8], sb[8];
+        sa[0] = add_cc(a.c0.l[0], a.c1.l[0], cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) sa[j] = addc_cc(a.c0.l[j], a.c1.l[j], cc);
+        sa[7] = addc(a.c0.l[7], a.c1.l[7], cc);                    // < 4p < 2^256
+        sb[0] = add_cc(b.c0.l[0], b.c1.l[0], cc);
+#pragma unroll
+        for (int j = 1; j < 7; j++) sb[j] = addc_cc(b.c0.l[j], b.c1.l[j], cc);
+        sb[7] = addc(b.c0.l[7], b.c1.l[7], cc);
+        mul_wide(T1, sa, sb);                                       // < 16p^2 < 2^512
+        T1[0] = sub_cc(T1[0], S[0], cc);
+#pragma unroll
+        for (int j = 1; j < 15; j++) T1[j] = subc_cc(T1[j], S[j], cc);
+        T1[15] = subc(T1[15], S[15], cc);                           // a0 b1 + a1 b0 >= 0 exactly
+        mont_reduce_wide_lazy<FqParams>(r.c1.l, T1);
+        cond_sub_2p<FqParams>(r.c1.l);
+        return r;
+    }
+    OG_HD static Fq2 sqr_lazy_inl(const Fq2& a) {
+        uint32_t T[16], u[8], v[8];
+        Fq2 r;
+        mul_wide(T, a.c0.l, a.c1.l);
+        mont_reduce_wide_lazy<FqParams>(r.c1.l, T);
+        add_lazy_fq(r.c1.l, r.c1.l, r.c1.l);
+        add_lazy_fq(u, a.c0.l, a.c1.l);
+        sub_raw_fq(v, a.c0.l, a.c1.l);
+        mul_wide(T, u, v);
+        mont_reduce_wide_lazy<FqParams>(r.c0.l, T);
+        cond_sub_2p<FqParams>(r.c0.l);
+        return r;
+    }
 };
 
 // Fq2 products are inlined.  Kernels keep ptxas time sane by calling the out-of-line group operations of
@@ -565,6 +677,18 @@ OG_HD Fq2 Fq2::sqr() const { return fq2_sqr_call(*this); }
 #else
 OG_HD Fq2 operator*(const Fq2& a, const Fq2& b) { return Fq2::mul_inl(a, b); }
 OG_HD Fq2 Fq2::sqr() const { return Fq2::sqr_inl(*this); }
+#endif
+
+// The lazy Fq2 product and squaring of the G2 group law (bounds at Fq2::add_lazy), with the same one-copy rule as above: the
+// G2 bucket kernel with both inlined (about 7.5k instructions in its loop) was 9 % slower than with one out-of-line copy of each
+#if defined(__CUDA_ARCH__) && defined(OG_FP_MUL_CALL)
+static __device__ __noinline__ Fq2 fq2_mul_lazy_call(Fq2 a, Fq2 b) { return Fq2::mul_lazy_inl(a, b); }
+static __device__ __noinline__ Fq2 fq2_sqr_lazy_call(Fq2 a) { return Fq2::sqr_lazy_inl(a); }
+OG_HD Fq2 fq2_mul_lazy(const Fq2& a, const Fq2& b) { return fq2_mul_lazy_call(a, b); }
+OG_HD Fq2 fq2_sqr_lazy(const Fq2& a) { return fq2_sqr_lazy_call(a); }
+#else
+OG_HD Fq2 fq2_mul_lazy(const Fq2& a, const Fq2& b) { return Fq2::mul_lazy_inl(a, b); }
+OG_HD Fq2 fq2_sqr_lazy(const Fq2& a) { return Fq2::sqr_lazy_inl(a); }
 #endif
 
 }  // namespace og

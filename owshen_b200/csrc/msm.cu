@@ -573,8 +573,9 @@ __global__ void __launch_bounds__(128, OG_ACC1_MINB) k_bucket_acc_sm1(const Affi
 
 #ifdef OG_MSM_G2
 // G2 variant with the 256-byte accumulator in shared memory (16-byte chunks interleaved over the CTA's threads, so
-// every access is conflict-free): registers hold only the temporaries of one mixed addition, which buys resident
-// warps in a kernel whose top stall is the fixed-latency wait of the carry chains (of 4, 5 and 6 resident CTAs, 6 was fastest).
+// every access is conflict-free).  The mixed addition is g2_madd_lazy (ec.cuh): lazily reduced Fq2 through one out-of-line copy
+// of the lazy product and squaring; the accumulator stays in [0, 2p) and is made canonical when the bucket is stored.  4 resident
+// CTAs (128 registers) beat 6 (80 registers, whose multiplier spilled around every call): 116.7 vs 139.6 ms per prover step.
 struct SmAcc {
     uint4* base;    // [16 chunks][128 threads]
     __device__ __forceinline__ Fq2 ld(int coord) const {
@@ -592,7 +593,10 @@ struct SmAcc {
     }
 };
 
-__global__ void __launch_bounds__(128, 6) k_bucket_acc_sm(const Affine<Fq2>* __restrict__ table, const uint32_t* __restrict__ sorted,
+#ifndef OG_ACC2_MINB
+#define OG_ACC2_MINB 4
+#endif
+__global__ void __launch_bounds__(128, OG_ACC2_MINB) k_bucket_acc_sm(const Affine<Fq2>* __restrict__ table, const uint32_t* __restrict__ sorted,
                                                        const uint32_t* __restrict__ offsets, const uint32_t* __restrict__ counts,
                                                        uint32_t n_keys, uint32_t cap, XYZZ<Fq2>* __restrict__ buckets,
                                                        uint32_t* __restrict__ heavy, const uint32_t* __restrict__ perm) {
@@ -616,26 +620,9 @@ __global__ void __launch_bounds__(128, 6) k_bucket_acc_sm(const Affine<Fq2>* __r
         e = en;
         if (q.is_inf()) continue;
         if (inf) { A.st(0, q.x); A.st(1, q.y); A.st(2, Fq2::one()); A.st(3, Fq2::one()); inf = false; continue; }
-        Fq2 p = q.x * A.ld(2) - A.ld(0);
-        Fq2 r = q.y * A.ld(3) - A.ld(1);
-        if (p.is_zero()) {
-            if (r.is_zero()) { XYZZ<Fq2> d = XYZZ<Fq2>::dbl_affine(q); A.st(0, d.x); A.st(1, d.y); A.st(2, d.zz); A.st(3, d.zzz); }
-            else inf = true;
-            continue;
-        }
-        // ordered so that few Fq2 temporaries are live across the out-of-line multiplier calls (each one is 16 registers
-        // that would otherwise be spilled around every call): zz and zzz are updated as soon as pp / ppp exist
-        Fq2 pp = p.sqr();
-        A.st(2, A.ld(2) * pp);
-        Fq2 ppp = p * pp;
-        A.st(3, A.ld(3) * ppp);
-        Fq2 q1 = A.ld(0) * pp;
-        Fq2 x3 = r.sqr() - ppp - q1.dbl();
-        A.st(0, x3);
-        Fq2 t = A.ld(1) * ppp;
-        A.st(1, r * (q1 - x3) - t);
+        if (!g2_madd_lazy(A, q)) inf = true;          // the accumulator stays lazy ([0, 2p)) until the bucket is stored
     }
-    buckets[key] = inf ? XYZZ<Fq2>::inf() : XYZZ<Fq2>{A.ld(0), A.ld(1), A.ld(2), A.ld(3)};
+    buckets[key] = inf ? XYZZ<Fq2>::inf() : XYZZ<Fq2>{A.ld(0).canonical(), A.ld(1).canonical(), A.ld(2).canonical(), A.ld(3).canonical()};
 }
 #endif
 
