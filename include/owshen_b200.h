@@ -130,6 +130,33 @@ int32_t og_bjj_sign_batch_dev(og_ctx* ctx, const uint8_t* d_secret_keys, const u
                               uint32_t n, int32_t hash_kind, uint8_t* d_out_pk_x, uint8_t* d_out_pk_is_odd,
                               uint8_t* d_out_signatures, uint8_t* d_out_status);
 
+/* ---- Encrypted note delivery (DESIGN.md section 3, "Encrypted notes"; spec oracle/notes.py) ---------------------------
+ * A view key v is a canonical Fr element with v mod l != 0 (l = the order of BASE); its public key (the address) is the
+ * compressed point v BASE: x (32 B) and the parity of y (1 byte), exactly PrivateKey::to_pub.  A non-canonical view key
+ * fails the call with OG_E_ENCODING, a key that is zero mod l with OG_E_INVALID.
+ * A record is 160 B: E.x with the parity of E.y in bit 255, then c_0..c_3 (32 B little-endian words). */
+int32_t og_note_public_keys(og_ctx* ctx, const uint8_t* view_keys, uint32_t n, uint8_t* out_pk_x, uint8_t* out_pk_is_odd);
+/* One note per recipient key: nullifier, secret, token (32 B each), amount (u64), ephemeral scalar e (32 B) -> record,
+ * commitment MultiMiMC7([nullifier, secret, token, amount], 0) (the transfer statement's output commitment) and
+ * out_status[i]: 1 = written; 2 = the key does not decompress or 8 V = O; 3 = e = 0 mod l.  Refused notes get an all-zero
+ * record and commitment.  Records and commitments must be 4-byte aligned in the _dev variant. */
+int32_t og_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* nullifiers, const uint8_t* secrets,
+                        const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
+                        uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status);
+int32_t og_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                            const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals, uint64_t n,
+                            uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status);
+/* Trial-decrypt n records (with their commitments, 32 B each: the transfer proofs' out_commitment inputs) under n_keys
+ * view keys (at most 65535).  out_owner[i]: the lowest index of a key that owns record i, 0xFFFFFFFF if none does,
+ * 0xFFFFFFFE if the record is malformed (E.x >= r or bit 254 set, a c_i or the commitment >= r, E does not decompress,
+ * 8 E = O).  out_plaintexts: 128 B per record, nullifier || secret || token || amount as field elements, zero unless owned.
+ * view_keys is host memory in both variants (checked, then staged); the _dev variant's other buffers are device memory,
+ * 4-byte aligned. */
+int32_t og_note_scan(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* records, const uint8_t* commitments,
+                     uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts);
+int32_t og_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments,
+                         uint64_t n, uint32_t* d_out_owner, uint8_t* d_out_plaintexts);
+
 /* ---- MSM (BASELINE configs 3 and 5) ----------------------------------------------------------- */
 int32_t og_msm_g1(og_ctx* ctx, const uint8_t* points, const uint8_t* scalars, uint64_t n, uint8_t* out64);
 int32_t og_msm_g2(og_ctx* ctx, const uint8_t* points, const uint8_t* scalars, uint64_t n, uint8_t* out128);

@@ -21,6 +21,12 @@ PROOF_BYTES = 256
 
 OG_OK, OG_E_INVALID, OG_E_VERIFY = 0, -1, -6
 
+# encrypted notes: l, the prime order of the BabyJubJub BASE (view keys and ephemerals must be nonzero mod l), and the two
+# owner sentinels of note_scan
+NOTE_SUBGROUP_ORDER = 2736030358979909402780800718157159386076813972158567259200215660948447373041
+NOTE_NOT_OWNED, NOTE_MALFORMED = 0xFFFFFFFF, 0xFFFFFFFE
+NOTE_RECORD_BYTES, NOTE_PLAINTEXT_BYTES = 160, 128
+
 
 class OwshenB200Error(RuntimeError):
     def __init__(self, code, detail=""):
@@ -64,6 +70,11 @@ _SIGS = {
     "og_bjj_verify_batch_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p]),
     "og_bjj_sign_batch_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_bjj_sign_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_note_public_keys": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "og_note_encrypt": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint64] + [C.c_void_p] * 3),
+    "og_note_encrypt_dev": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint64] + [C.c_void_p] * 3),
+    "og_note_scan": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "og_note_scan_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "og_msm_g1": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "og_msm_g2": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "og_msm_g1_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -365,6 +376,56 @@ class Context:
         sg, st = C.create_string_buffer(96 * n), C.create_string_buffer(n)
         _check(lib().og_bjj_sign_batch(self._h, secret_keys, randomness, messages, n, hash_kind, px, odd, sg, st), self)
         return px.raw, odd.raw[:n], sg.raw, st.raw[:n]
+
+    # ---- encrypted notes (DESIGN.md section 3, "Encrypted notes") ----------------------------------------------------
+    def note_public_keys(self, view_keys: bytes):
+        """View keys (32 bytes each, canonical, nonzero mod l) -> (pk_x, pk_is_odd): the compressed addresses v BASE."""
+        _need(len(view_keys) % 32 == 0, "note_public_keys: view keys must be a multiple of 32 bytes")
+        n = len(view_keys) // 32
+        px, odd = C.create_string_buffer(32 * n), C.create_string_buffer(n)
+        _check(lib().og_note_public_keys(self._h, view_keys, n, px, odd), self)
+        return px.raw, odd.raw[:n]
+
+    def note_encrypt(self, pk_x: bytes, pk_is_odd: bytes, nullifiers: bytes, secrets: bytes, tokens: bytes, amounts, ephemerals=None):
+        """Encrypt note i to the address (pk_x[i], pk_is_odd[i]) -> (records (160 B each), commitments (32 B each), status)
+        with status 1 = written, 2 = the address does not decompress or has 8 V = O, 3 = the ephemeral is 0 mod l.
+        Amounts: a sequence of ints < 2^64 or little-endian u64 bytes.  Ephemerals (32 B each) are drawn with the `secrets`
+        module in [1, l) when not given; given ones make every byte reproducible."""
+        n = len(pk_is_odd)
+        if ephemerals is None:
+            ephemerals = b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n))
+        am = _u64_array(amounts)
+        for name, buf in (("pk_x", pk_x), ("nullifiers", nullifiers), ("secrets", secrets), ("tokens", tokens), ("ephemerals", ephemerals)):
+            _need(len(buf) == 32 * n, f"note_encrypt: {name}: expected {32 * n} bytes, got {len(buf)}")
+        _need((C.sizeof(am) if isinstance(am, C.Array) else _blen(am)) == 8 * n, "note_encrypt: expected one amount per note")
+        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
+        _check(lib().og_note_encrypt(self._h, pk_x, pk_is_odd, nullifiers, secrets, tokens, _ptr(am), ephemerals, n, rec, cm, st), self)
+        return rec.raw, cm.raw, st.raw[:n]
+
+    def note_encrypt_dev(self, d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts, d_ephemerals, n: int,
+                         d_out_records, d_out_commitments, d_out_status):
+        """og_note_encrypt_dev: device buffers (addresses or tensors), enqueued on the context's stream."""
+        _check(lib().og_note_encrypt_dev(self._h, *[_ptr(x) for x in (d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts,
+                                                                     d_ephemerals)], n,
+                                         *[_ptr(x) for x in (d_out_records, d_out_commitments, d_out_status)]), self)
+
+    def note_scan(self, view_keys: bytes, records: bytes, commitments: bytes):
+        """Trial-decrypt every record under every view key -> (owners, plaintexts): owners[i] is the lowest index of a key
+        that owns record i, NOTE_NOT_OWNED or NOTE_MALFORMED; plaintexts holds 128 bytes per record (nullifier, secret, token,
+        amount), zero unless owned."""
+        _need(len(view_keys) % 32 == 0, "note_scan: view keys must be a multiple of 32 bytes")
+        _need(len(records) % 160 == 0, "note_scan: records must be a multiple of 160 bytes")
+        n = len(records) // 160
+        _need(len(commitments) == 32 * n, "note_scan: expected one 32-byte commitment per record")
+        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
+        _check(lib().og_note_scan(self._h, view_keys, len(view_keys) // 32, records, commitments, n, owner, plain), self)
+        return list(owner), plain.raw
+
+    def note_scan_dev(self, view_keys: bytes, d_records, d_commitments, n: int, d_out_owner, d_out_plaintexts):
+        """og_note_scan_dev: view keys on the host, every other buffer on the device, enqueued on the context's stream."""
+        _need(len(view_keys) % 32 == 0, "note_scan_dev: view keys must be a multiple of 32 bytes")
+        _check(lib().og_note_scan_dev(self._h, view_keys, len(view_keys) // 32, _ptr(d_records), _ptr(d_commitments), n,
+                                      _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
 
     def msm_g1(self, points: bytes, scalars: bytes) -> bytes:
         _need(len(scalars) % 32 == 0, "msm_g1: scalars must be a multiple of 32 bytes")

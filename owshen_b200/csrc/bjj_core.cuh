@@ -89,6 +89,19 @@ OG_BJJ_FN bool fr_sqrt(Fr* out, const Fr* a) {
 OG_HD bool fr_is_odd(const Fr& v) { uint32_t c[8]; v.to_canonical(c); return c[0] & 1; }
 
 
+// PointCompressed::decompress (mod.rs:88-98): y of the point (x, y) whose parity is `odd`; false where the reference
+// returns Err (1 - D x^2 is zero, or (1 - A x^2) / (1 - D x^2) is not a square)
+OG_BJJ_FN bool bjj_decompress(Fr* y, const Fr* x, bool odd) {
+    const Fr A = bjj_a(), D = bjj_d(), one = Fr::one();
+    Fr xx = x->sqr();
+    Fr den = one - D * xx;
+    if (den.is_zero()) return false;
+    Fr y2 = den.inv() * (one - A * xx);
+    if (!fr_sqrt(y, &y2)) return false;
+    if (fr_is_odd(*y) != odd) *y = y->neg();
+    return true;
+}
+
 // status: 1 verifies, 0 does not, 2 = Err in the reference (public key does not decompress).  `h_mimc` is only
 // read when hash_kind == 1 (the caller computes MultiMiMC7([R.x, R.y, pk.x, pk.y, msg]) after decompression via cb).
 // fixed-base multiplication k * BASE from a table of window multiples: tab[w * 15 + d - 1] = d * 16^w * BASE (affine x, y),
@@ -119,13 +132,8 @@ template <class HashFn>
 OG_HD uint8_t bjj_verify_one(const Fr& x, bool pk_odd, const Fr& msg, const Fr& rx, const Fr& ry, const Fr& s, const BjjBase& base,
                              HashFn hash5) {
     const Fr A = bjj_a(), D = bjj_d(), one = Fr::one();
-    // decompress (mod.rs:88-98)
-    Fr xx = x.sqr();
-    Fr den = one - D * xx;
-    if (den.is_zero()) return 2;
-    Fr y2 = den.inv() * (one - A * xx), y;
-    if (!fr_sqrt(&y, &y2)) return 2;
-    if (fr_is_odd(y) != pk_odd) y = y.neg();
+    Fr y;
+    if (!bjj_decompress(&y, &x, pk_odd)) return 2;
     // verify (mod.rs:99-115)
     if (!bjj_on_curve(x, y, A, D) || !bjj_on_curve(rx, ry, A, D)) return 0;
     Fr in[5] = {rx, ry, x, y, msg};
@@ -184,6 +192,15 @@ OG_BJJ_FN void bjj_to_affine(Fr* x, Fr* y, const BjjPoint* p) {
     *x = p->x * zi; *y = p->y * zi;
 }
 
+// PrivateKey::to_pub (mod.rs:207-209): the affine point sk BASE; the public key is its compression (x, parity of y), and
+// decompressing that gives y back
+OG_BJJ_FN void bjj_to_pub(Fr* x, Fr* y, const BjjBase* base, const Fr* sk) {
+    const Fr A = bjj_a(), D = bjj_d();
+    BjjPoint acc;
+    bjj_mul_base(&acc, base, sk, &A, &D);
+    bjj_to_affine(x, y, &acc);
+}
+
 // PrivateKey::to_pub + sign (mod.rs:207-237).  status 1: pk and signature written; 2: the reference returns
 // Err("Invalid repr") because s >= r cannot be represented as an Fp (ORDER > r: the wart SURVEY.md 8a notes).
 template <class HashFn2, class HashFn5>
@@ -192,8 +209,7 @@ OG_HD uint8_t bjj_sign_one(const Fr& sk, const Fr& randomness, const Fr& msg, co
     const Fr A = bjj_a(), D = bjj_d();
     BjjPoint acc;
     Fr px, py, rx, ry;
-    bjj_mul_base(&acc, &base, &sk, &A, &D);                    // to_pub: BASE * sk, compressed (x, parity of y); decompressing gives y back
-    bjj_to_affine(&px, &py, &acc);
+    bjj_to_pub(&px, &py, &base, &sk);
     *pk_x = px; *pk_odd = fr_is_odd(py);
     Fr in2[2] = {randomness, msg};
     Fr r = hash2(in2);                                 // r = H(b, M)

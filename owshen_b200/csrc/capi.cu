@@ -639,6 +639,87 @@ int32_t og_bjj_sign_batch(og_ctx* ctx, const uint8_t* secret_keys, const uint8_t
     return check_flag(ctx);
 }
 
+// ---- encrypted notes (note_impl.cuh; spec oracle/notes.py) ------------------------------------------------------
+int32_t og_note_public_keys(og_ctx* ctx, const uint8_t* view_keys, uint32_t n, uint8_t* out_pk_x, uint8_t* out_pk_is_odd) {
+    OG_ENTER(ctx);
+    if (n && (!view_keys || !out_pk_x || !out_pk_is_odd)) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_TRY(note_check_view_keys(ctx, view_keys, n));
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 65ull * n);
+    uint8_t *dk = io, *dx = io + 32ull * n, *dodd = io + 64ull * n;
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dk, view_keys, 32ull * n);
+    OG_TRY(note_public_keys_dev(ctx, dk, n, dx, dodd));
+    D2H(ctx, out_pk_x, dx, 32ull * n); D2H(ctx, out_pk_is_odd, dodd, n);
+    return check_flag(ctx);
+}
+
+int32_t og_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                            const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals, uint64_t n,
+                            uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
+    OG_ENTER(ctx);
+    if (n && (!d_pk_x || !d_pk_is_odd || !d_nullifiers || !d_secrets || !d_tokens || !d_amounts || !d_ephemerals || !d_out_records ||
+              !d_out_commitments || !d_out_status)) return OG_E_INVALID;
+    return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts, d_ephemerals}, n,
+                            d_out_records, d_out_commitments, d_out_status);
+}
+
+int32_t og_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* nullifiers, const uint8_t* secrets,
+                        const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
+                        uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
+    OG_ENTER(ctx);
+    if (n && (!pk_x || !pk_is_odd || !nullifiers || !secrets || !tokens || !amounts || !ephemerals || !out_records || !out_commitments ||
+              !out_status)) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    // per note: 5 x 32 B inputs, 8 B amount, 1 B parity in; 160 B record, 32 B commitment, 1 B status out (u64s first: aligned)
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 362ull * n);
+    uint64_t* da = reinterpret_cast<uint64_t*>(io);
+    uint8_t *dx = io + 8 * n, *dnu = dx + 32 * n, *dse = dnu + 32 * n, *dto = dse + 32 * n, *de = dto + 32 * n;
+    uint8_t *drec = de + 32 * n, *dcm = drec + 160 * n, *dodd = dcm + 32 * n, *dst = dodd + n;
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dnu, nullifiers, 32 * n); H2D(ctx, dse, secrets, 32 * n);
+    H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n);
+    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dnu, dse, dto, da, de}, n, drec, dcm, dst));
+    D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
+    return check_flag(ctx);
+}
+
+// view keys are host memory in both variants: they are checked here, then staged to the device
+static int32_t note_stage_keys(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint32_t** d_keys) {
+    if (n_keys > 65535) { snprintf(ctx->err, sizeof(ctx->err), "at most 65535 view keys per scan"); return OG_E_INVALID; }
+    OG_TRY(note_check_view_keys(ctx, view_keys, n_keys));
+    OG_SLOT(ctx, dk, uint32_t, S_NOTE_KEYS, 32ull * n_keys);
+    if (n_keys) H2D(ctx, dk, view_keys, 32ull * n_keys);
+    *d_keys = dk;
+    return OG_OK;
+}
+
+int32_t og_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments,
+                         uint64_t n, uint32_t* d_out_owner, uint8_t* d_out_plaintexts) {
+    OG_ENTER(ctx);
+    if ((n_keys && !view_keys) || (n && (!d_records || !d_commitments || !d_out_owner || !d_out_plaintexts))) return OG_E_INVALID;
+    const uint32_t* dk;
+    OG_TRY(note_stage_keys(ctx, view_keys, n_keys, &dk));
+    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts);
+}
+
+int32_t og_note_scan(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* records, const uint8_t* commitments, uint64_t n,
+                     uint32_t* out_owner, uint8_t* out_plaintexts) {
+    OG_ENTER(ctx);
+    if ((n_keys && !view_keys) || (n && (!records || !commitments || !out_owner || !out_plaintexts))) return OG_E_INVALID;
+    const uint32_t* dk;
+    OG_TRY(note_stage_keys(ctx, view_keys, n_keys, &dk));
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // 160 B record, 32 B commitment in; 4 B owner, 128 B plaintext out
+    uint32_t* downer = reinterpret_cast<uint32_t*>(io);
+    uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
+    H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
+    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl));
+    D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
+    OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return OG_OK;
+}
+
 // ---- MSM --------------------------------------------------------------------------------------------------
 int32_t og_msm_g1_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_scalars, uint64_t n, uint8_t* d_out64) {
     OG_ENTER(ctx);

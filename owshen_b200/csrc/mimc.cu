@@ -342,3 +342,4 @@ int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint3
 }  // namespace og
 
 #include "bjj_impl.cuh"
+#include "note_impl.cuh"

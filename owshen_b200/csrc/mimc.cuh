@@ -116,4 +116,17 @@ int32_t bjj_verify_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_o
 int32_t bjj_sign_dev(og_ctx* ctx, const uint8_t* d_sk, const uint8_t* d_rnd, const uint8_t* d_msgs, uint32_t n, int hash_kind,
                      uint8_t* d_pk_x, uint8_t* d_pk_odd, uint8_t* d_sigs, uint8_t* d_status);
 
+// encrypted notes (note_impl.cuh; spec oracle/notes.py).  Per note: the recipient's compressed key (pk_x 32 B, pk_odd 1 B),
+// nullifier, secret, token (32 B each), amount (u64) and the ephemeral scalar (32 B)
+struct NoteEncryptInputs {
+    const uint8_t *pk_x, *pk_odd, *nullifiers, *secrets, *tokens;
+    const uint64_t* amounts;
+    const uint8_t* ephemerals;
+};
+int32_t note_check_view_keys(og_ctx* ctx, const uint8_t* h_keys, uint32_t n);
+int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uint8_t* d_pk_x, uint8_t* d_pk_odd);
+int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status);
+int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
+                      uint32_t* d_owner, uint8_t* d_plaintexts);
+
 }  // namespace og

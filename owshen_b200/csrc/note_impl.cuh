@@ -1,0 +1,151 @@
+// owshen_b200/csrc/note_impl.cuh -- (included at the end of mimc.cu, after bjj_impl.cuh: it shares the MiMC7 round constants
+// and the BabyJubJub fixed-base table) encrypted note delivery on sm_90a (DESIGN.md sections 3 and 5.6; spec: oracle/notes.py).
+//
+//   k_note_public_keys   one thread per view key: v BASE through the fixed-base table
+//   k_note_encrypt       one thread per note
+//   k_note_prepare       one thread per record: parse, decompress E, E' = 8 E and the malformed checks, once for all keys;
+//                        writes E' (the only scratch) and seeds the owner word with NOT_OWNED or MALFORMED
+//   k_note_scan          one thread per (record, key); blockIdx.y is the key, so a warp shares one scalar and the
+//                        double-and-add (or the window digits) never diverge.  An owner is recorded with atomicMin, so the
+//                        lowest owning key index wins whatever the scheduling
+//   k_note_finish        one thread per record: zero plaintext, or the note decrypted again under the winning key
+#include "note_core.cuh"
+
+namespace og {
+
+struct NoteC {                                        // the round constants, as the `c(i)` of note_core.cuh
+    __device__ __forceinline__ Fr operator()(int i) const { return mimc_c(i); }
+};
+
+__global__ void __launch_bounds__(64) k_note_public_keys(const Fr* __restrict__ base_tab, const uint8_t* __restrict__ keys, uint32_t n,
+                                                         uint8_t* __restrict__ pk_x, uint8_t* __restrict__ pk_odd, int* flag) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fr v = load_canonical<Fr>(keys + 32ull * i, flag), x, y;
+    const BjjBase base{Fr::zero(), Fr::zero(), base_tab};
+    bjj_to_pub(&x, &y, &base, &v);
+    store_canonical(pk_x + 32ull * i, x);
+    pk_odd[i] = fr_is_odd(y) ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(64) k_note_encrypt(const Fr* __restrict__ base_tab, NoteEncryptInputs in, uint64_t n,
+                                                     uint8_t* __restrict__ records, uint8_t* __restrict__ commitments,
+                                                     uint8_t* __restrict__ status, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t amount = in.amounts[i];
+    uint32_t a[8] = {(uint32_t)amount, (uint32_t)(amount >> 32), 0, 0, 0, 0, 0, 0};
+    Fr m[4] = {load_canonical<Fr>(in.nullifiers + 32 * i, flag), load_canonical<Fr>(in.secrets + 32 * i, flag),
+               load_canonical<Fr>(in.tokens + 32 * i, flag), Fr::from_canonical(a)};
+    Fr pk_x = load_canonical<Fr>(in.pk_x + 32 * i, flag), e = load_canonical<Fr>(in.ephemerals + 32 * i, flag), cm;
+    uint32_t w[NOTE_RECORD_WORDS];
+    status[i] = note_encrypt_one(pk_x, in.pk_odd[i] != 0, m, e, BjjBase{Fr::zero(), Fr::zero(), base_tab}, NoteC{}, w, &cm);
+    uint32_t* out = reinterpret_cast<uint32_t*>(records + 160 * i);
+#pragma unroll
+    for (uint32_t k = 0; k < NOTE_RECORD_WORDS; k++) out[k] = w[k];
+    store_canonical(commitments + 32 * i, cm);
+}
+
+__global__ void __launch_bounds__(128) k_note_prepare(const uint8_t* __restrict__ records, const uint8_t* __restrict__ commitments,
+                                                      uint64_t n, Fr* __restrict__ prepared, uint32_t* __restrict__ owner) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fr x, y;
+    bool ok = note_prepare_one(reinterpret_cast<const uint32_t*>(records + 160 * i), reinterpret_cast<const uint32_t*>(commitments + 32 * i),
+                               &x, &y);
+    prepared[2 * i] = ok ? x : Fr::zero();
+    prepared[2 * i + 1] = ok ? y : Fr::one();
+    owner[i] = ok ? NOTE_NOT_OWNED : NOTE_MALFORMED;
+}
+
+template <bool WINDOW>
+__global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ keys, const uint8_t* __restrict__ records,
+                                                  const uint8_t* __restrict__ commitments, const Fr* __restrict__ prepared, uint64_t n,
+                                                  uint32_t* owner) {
+    const uint32_t key = blockIdx.y;
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || owner[i] == NOTE_MALFORMED) return;     // MALFORMED is written by k_note_prepare only, never by atomicMin
+    uint32_t v[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) v[k] = keys[8 * key + k];
+    Fr m[4];
+    if (note_decrypt_one<WINDOW>(prepared[2 * i], prepared[2 * i + 1], v, reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                 reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m))
+        atomicMin(owner + i, key);
+}
+
+__global__ void __launch_bounds__(64) k_note_finish(const uint32_t* __restrict__ keys, uint32_t n_keys, const uint8_t* __restrict__ records,
+                                                    const uint8_t* __restrict__ commitments, const Fr* __restrict__ prepared, uint64_t n,
+                                                    const uint32_t* __restrict__ owner, uint8_t* __restrict__ plaintexts) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t o = owner[i];
+    Fr m[4] = {Fr::zero(), Fr::zero(), Fr::zero(), Fr::zero()};
+    if (o < n_keys)
+        note_decrypt_one<false>(prepared[2 * i], prepared[2 * i + 1], keys + 8ull * o, reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m);
+    for (int k = 0; k < 4; k++) store_canonical(plaintexts + 128 * i + 32 * k, m[k]);
+}
+
+// ---- host side ------------------------------------------------------------------------------------
+// a view key must be canonical (OG_E_ENCODING) and nonzero mod l (OG_E_INVALID); v < r < 8 l, so the multiples to refuse are
+// 0, l, ..., 7 l, with l = ORDER / 8
+int32_t note_check_view_keys(og_ctx* ctx, const uint8_t* keys, uint32_t n) {
+    uint32_t l[8];
+    for (int i = 0; i < 8; i++) l[i] = (bjj_order_limb(i) >> 3) | (i < 7 ? bjj_order_limb(i + 1) << 29 : 0);
+    for (uint32_t j = 0; j < n; j++) {
+        uint32_t v[8];
+        memcpy(v, keys + 32ull * j, 32);
+        if (!Fr::canonical_lt_mod(v)) {
+            snprintf(ctx->err, sizeof(ctx->err), "view key %u is not a canonical field element", j);
+            return OG_E_ENCODING;
+        }
+        uint32_t kl[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        for (int k = 0; k < 8; k++) {
+            if (memcmp(kl, v, 32) == 0) {
+                snprintf(ctx->err, sizeof(ctx->err), "view key %u is zero mod the subgroup order l", j);
+                return OG_E_INVALID;
+            }
+            uint64_t c = 0;
+            for (int t = 0; t < 8; t++) { c += (uint64_t)kl[t] + l[t]; kl[t] = (uint32_t)c; c >>= 32; }
+        }
+    }
+    return OG_OK;
+}
+
+int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uint8_t* d_pk_x, uint8_t* d_pk_odd) {
+    if (n == 0) return OG_OK;
+    const Fr* tab;
+    OG_TRY(bjj_table(ctx, &tab));
+    OG_LAUNCH(ctx, k_note_public_keys, (n + 63) / 64, 64, 0, tab, d_keys, n, d_pk_x, d_pk_odd, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status) {
+    if (n == 0) return OG_OK;
+    const Fr* tab;
+    OG_TRY(bjj_table(ctx, &tab));
+    OG_LAUNCH(ctx, k_note_encrypt, (unsigned)((n + 63) / 64), 64, 0, tab, in, n, d_records, d_commitments, d_status, ctx->d_flag);
+    return OG_OK;
+}
+
+// d_keys: n_keys checked view keys (canonical limbs) in device memory; the prepared points go to a context slot
+int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
+                      uint32_t* d_owner, uint8_t* d_plaintexts) {
+    if (n == 0) return OG_OK;
+    if (n_keys > 65535) { snprintf(ctx->err, sizeof(ctx->err), "at most 65535 view keys per scan"); return OG_E_INVALID; }
+    OG_SLOT(ctx, prep, Fr, S_NOTE_PREP, sizeof(Fr) * 2 * n);
+    const unsigned blocks = (unsigned)((n + 63) / 64);
+    OG_LAUNCH(ctx, k_note_prepare, (unsigned)((n + 127) / 128), 128, 0, d_records, d_commitments, n, prep, d_owner);
+    if (n_keys) {
+        // the variable-base multiplier: the 4-bit window, or plain double-and-add with OG_NOTE_WINDOW=0 (DESIGN.md section 8:
+        // the window is 15 % faster at 2^20 records x 8 keys on an H100)
+        const char* w = getenv("OG_NOTE_WINDOW");
+        if (!w || atoi(w) != 0) OG_LAUNCH(ctx, k_note_scan<true>, dim3(blocks, n_keys), 64, 0, d_keys, d_records, d_commitments, prep, n, d_owner);
+        else OG_LAUNCH(ctx, k_note_scan<false>, dim3(blocks, n_keys), 64, 0, d_keys, d_records, d_commitments, prep, n, d_owner);
+    }
+    OG_LAUNCH(ctx, k_note_finish, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n, d_owner, d_plaintexts);
+    return OG_OK;
+}
+
+}  // namespace og

@@ -81,6 +81,10 @@ def to_json(obj: dict) -> str:
 # RLP itself is the Ethereum yellow-paper appendix B encoding (crate `rlp` 0.5.2 in the reference's Cargo.toml:13).
 
 SHIELDED_WITHDRAW_KIND = "shielded-withdraw"
+# A shielded transfer carries its proof, the statement's 8 public inputs and the two 160-byte encrypted note records of its
+# outputs (out 0, then out 1; DESIGN.md section 3, "Encrypted notes"):
+#     ["shielded-transfer", proof (256 B), 8 public inputs (32 B LE each), record 0, record 1 (160 B each)]
+SHIELDED_TRANSFER_KIND = "shielded-transfer"
 
 
 def rlp_encode(item) -> bytes:
@@ -164,3 +168,24 @@ def shielded_withdraw_from_rlp(msg: bytes):
     if kind != SHIELDED_WITHDRAW_KIND.encode() or len(proof) != 256 or any(len(x) != 32 for x in (root, nh, rcpt)):
         raise ValueError("Invalid tx!")
     return proof, root + nh + rcpt
+
+
+def shielded_transfer_to_rlp(proof: bytes, public_inputs: bytes, records: bytes) -> bytes:
+    """CustomTxMsg-shaped message for one transfer proof: public_inputs = the 8 inputs of og_groth16_prove_transfer's
+    `public_out` row (256 B), records = the encrypted notes of output 0 and output 1 (2 x 160 B, og_note_encrypt)."""
+    if len(proof) != 256 or len(public_inputs) != 256 or len(records) != 320:
+        raise ValueError("shielded_transfer_to_rlp: proof must be 256 bytes, public inputs 256, records 320")
+    return rlp_encode([SHIELDED_TRANSFER_KIND, proof] + [public_inputs[32 * i:32 * i + 32] for i in range(8)]
+                      + [records[0:160], records[160:320]])
+
+
+def shielded_transfer_from_rlp(msg: bytes):
+    """-> (proof, public_inputs, records); raises ValueError("Invalid tx!") on anything that is not a well-formed
+    shielded-transfer message."""
+    item = rlp_decode(msg)
+    if not isinstance(item, list) or len(item) != 12 or any(isinstance(x, list) for x in item):
+        raise ValueError("Invalid tx!")
+    kind, proof, pub, recs = item[0], item[1], item[2:10], item[10:12]
+    if kind != SHIELDED_TRANSFER_KIND.encode() or len(proof) != 256 or any(len(x) != 32 for x in pub) or any(len(r) != 160 for r in recs):
+        raise ValueError("Invalid tx!")
+    return proof, b"".join(pub), b"".join(recs)
