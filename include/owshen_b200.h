@@ -322,6 +322,24 @@ int32_t og_scale_points(og_ctx* ctx, int32_t g2, const uint8_t* points, const ui
                         uint8_t* out);
 int32_t og_intt_points(og_ctx* ctx, int32_t g2, uint8_t* points, uint32_t log_m);
 
+/* ---- test/debug probes of the MSM engine (not for integrators) ----------------------------------------------------------
+ * og_msm_bucket_sums runs the bucket stage of the G1 (g2 = 0) or G2 (g2 = 1) MSM -- bucket order, accumulation, heavy buckets,
+ * reduction -- on bucket lists the caller gives.  counts: n_groups * nb list lengths (key = g * nb + b); entries: sum(counts)
+ * words in key order, (point index << 1) | negate.  out_totals: n_groups affine points sum_b (b + 1) B_b; out_buckets (NULL
+ * to skip): the n_groups * nb buckets after accumulation and heavy combine.  few_groups selects the one-shot MSM's reduction
+ * (the tree-sum tail).  OG_E_INVALID, before anything is launched, unless nb is a power of two in [2, 2^15], n_groups is in
+ * [1, 65535], n_groups * nb <= 2^26, every point index is below n_points, sum(counts) < 2^32,
+ * sum(counts) <= n_entries_max < 2^30, and the heavy buckets' segments fit the engine's level scratch (the heavy-bucket cap and
+ * segment length follow n_entries_max / (n_groups * nb); a plan over that scratch needs an average of 512 or more entries per key). */
+int32_t og_msm_bucket_sums(og_ctx* ctx, int32_t g2, const uint8_t* points, uint32_t n_points, const uint32_t* counts,
+                           const uint32_t* entries, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, int32_t few_groups,
+                           uint8_t* out_totals, uint8_t* out_buckets);
+/* Element-wise arithmetic of the MSM units on raw Montgomery limbs (no conversion, no range check), through the functions the bucket
+ * kernels call (the same source and PTX; the compiler gives each kernel its own machine-code copy of them).  unit 0 (G1 unit, Fq, 32 B per operand): op 0 a * b, 1 a^2 (the out-of-line squarer), 2 a - b, 3 a + a.
+ * unit 1 (G2 unit, Fq2, 64 B): op 0 lazy a * b, 1 lazy a^2, 2 lazy a + b, 3 lazy a - b, 4 a reduced to [0, p), 5 a * b,
+ * 6 a^2, 7 "a == 0 mod p" (1 or 0 in the first byte, the rest zero).  b is read for every op. */
+int32_t og_field_probe_raw(og_ctx* ctx, int32_t unit, int32_t op, const uint8_t* a, const uint8_t* b, uint64_t n, uint8_t* out);
+
 #ifdef __cplusplus
 }
 #endif

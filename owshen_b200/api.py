@@ -6,6 +6,7 @@ little-endian (/root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.r
 
 All hashing, witness generation, NTTs and MSMs run in the CUDA library; nothing here computes.
 """
+import array
 import ctypes as C
 import os
 import secrets as _rand
@@ -129,6 +130,9 @@ _SIGS = {
     "og_phase2_verify": (C.c_int32, [C.c_void_p] + [C.c_void_p, C.c_uint64] * 5),
     "og_scale_points": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int32, C.c_void_p]),
     "og_intt_points": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
+    "og_msm_bucket_sums": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
+                                       C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p]),
+    "og_field_probe_raw": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
 }
 ABI_SYMBOLS = tuple(_SIGS)
 
@@ -321,6 +325,47 @@ class Context:
         out = C.create_string_buffer(32 * n)
         _check(lib().og_field_op(self._h, {"fq": 0, "fr": 1}[field], {"mul": 0, "add": 1, "sub": 2}[op], a, b, n, out), self)
         return out.raw
+
+    # ops of field_probe_raw per unit (include/owshen_b200.h: og_field_probe_raw)
+    FIELD_PROBE_OPS = {"g1": ("mul", "sqr", "sub", "dbl"),
+                       "g2": ("mul_lazy", "sqr_lazy", "add_lazy", "sub_lazy", "canonical", "mul", "sqr", "is_zero_lazy")}
+
+    def field_probe_raw(self, unit: str, op: str, a: bytes, b: bytes = None) -> bytes:
+        """Test/debug probe: element-wise arithmetic of the G1 ("g1": Fq, 32 B per operand) or G2 ("g2": Fq2, 64 B) MSM unit on
+        raw Montgomery limbs, through the functions its bucket kernels call (the probe kernel's own compiled copies); raw limbs out."""
+        _need(unit in self.FIELD_PROBE_OPS and op in self.FIELD_PROBE_OPS[unit], "field_probe_raw: unknown unit or op")
+        eb = 32 if unit == "g1" else 64
+        b = a if b is None else b
+        _need(len(a) % eb == 0 and len(b) == len(a), f"field_probe_raw: a and b must be equally long multiples of {eb} bytes")
+        n = len(a) // eb
+        out = C.create_string_buffer(eb * n)
+        _check(lib().og_field_probe_raw(self._h, unit == "g2", self.FIELD_PROBE_OPS[unit].index(op), a, b, n, out), self)
+        return out.raw
+
+    def msm_bucket_sums(self, curve: str, points: bytes, counts, entries, n_groups: int, nb: int, n_entries_max=None,
+                        few_groups=False, buckets=False):
+        """Test/debug probe (og_msm_bucket_sums): the MSM engine's bucket stage on the given bucket lists.  counts: n_groups * nb
+        list lengths (key = g * nb + b); entries: sum(counts) words (point index << 1) | negate in key order; n_entries_max
+        (default sum(counts)) sets the heavy-bucket cap as in the MSM.  Returns (n_groups affine totals sum_b (b + 1) B_b, the
+        n_groups * nb affine buckets or None)."""
+        _need(curve in ("g1", "g2"), "msm_bucket_sums: curve must be 'g1' or 'g2'")
+        pb = 64 if curve == "g1" else 128
+        _need(len(points) % pb == 0, f"msm_bucket_sums: points must be a multiple of {pb} bytes")
+        def u32(xs):                       # a sequence of ints or a numpy array -> a buffer of uint32
+            if not hasattr(xs, "astype"):
+                return array.array("I", xs)
+            a = array.array("I")
+            a.frombytes(xs.astype("<u4").tobytes())
+            return a
+        cnt, ent = u32(counts), u32(entries)
+        total = sum(cnt)
+        _need(len(cnt) == n_groups * nb and len(ent) == total, "msm_bucket_sums: need n_groups * nb counts and sum(counts) entries")
+        out = C.create_string_buffer(pb * n_groups)
+        bk = C.create_string_buffer(pb * n_groups * nb) if buckets else None
+        _check(lib().og_msm_bucket_sums(self._h, curve == "g2", points, len(points) // pb, C.c_void_p(cnt.buffer_info()[0]),
+                                        C.c_void_p(ent.buffer_info()[0]) if total else None, n_groups, nb,
+                                        total if n_entries_max is None else n_entries_max, int(few_groups), out, bk), self)
+        return out.raw, (bk.raw if buckets else None)
 
     def mimc7_hash2(self, left: bytes, right: bytes) -> bytes:
         _need(len(left) % 32 == 0 and len(right) == len(left), "mimc7_hash2: left and right must be equally long multiples of 32 bytes")

@@ -1266,4 +1266,81 @@ int32_t og_intt_points(og_ctx* ctx, int32_t g2, uint8_t* points, uint32_t log_m)
     return check_flag(ctx);
 }
 
+// ---- test/debug probes of the MSM units (msm.cu) ----------------------------------------------------------------------
+// Every argument is checked before anything is staged or launched: msm_buckets trusts its lists and its heavy plan.  The cap and the
+// segment length follow n_entries_max / n_keys (msm.cuh: msm_heavy_cap / msm_heavy_seg); n_entries_max < 2^30 keeps them and the
+// segment arithmetic of k_heavy_plan / k_bucket_heavy within 32 bits, and the segment count is checked against the d_lvl scratch the
+// segment sums are written into (which an n_entries_max below sum(counts), or avg >= 512, can exceed).
+int32_t og_msm_bucket_sums(og_ctx* ctx, int32_t g2, const uint8_t* points, uint32_t n_points, const uint32_t* counts,
+                           const uint32_t* entries, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, int32_t few_groups,
+                           uint8_t* out_totals, uint8_t* out_buckets) {
+    OG_ENTER(ctx);
+    if (g2 < 0 || g2 > 1 || !counts || !out_totals || (n_points && !points)) return OG_E_INVALID;
+    if (nb < 2 || nb > 32768 || (nb & (nb - 1)) || n_groups == 0 || n_groups > 65535 || (uint64_t)n_groups * nb > (1u << 26)) {
+        snprintf(ctx->err, sizeof(ctx->err), "nb must be a power of two in [2, 2^15], n_groups in [1, 65535], n_groups * nb <= 2^26");
+        return OG_E_INVALID;
+    }
+    const uint32_t n_keys = n_groups * nb;
+    std::vector<uint32_t> offsets;
+    try { offsets.resize((size_t)n_keys + 1); } catch (const std::bad_alloc&) { return OG_E_NOMEM; }
+    uint64_t total = 0;
+    for (uint32_t k = 0; k < n_keys; k++) {
+        offsets[k] = (uint32_t)total;
+        total += counts[k];
+        if (total > 0xFFFFFFFFull) { snprintf(ctx->err, sizeof(ctx->err), "sum(counts) does not fit 32 bits"); return OG_E_INVALID; }
+    }
+    offsets[n_keys] = (uint32_t)total;
+    if (n_entries_max < total || n_entries_max >= (1ull << 30)) {
+        snprintf(ctx->err, sizeof(ctx->err), "n_entries_max must lie in [sum(counts), 2^30)");
+        return OG_E_INVALID;
+    }
+    const uint64_t avg = n_entries_max / n_keys;
+    const uint32_t cap = msm_heavy_cap(avg), seg = msm_heavy_seg(avg);
+    uint64_t n_seg = 0;
+    for (uint32_t k = 0; k < n_keys; k++)
+        if (counts[k] > cap) n_seg += (counts[k] + (uint64_t)seg - 1) / seg;
+    if (n_seg > msm_lvl_elems(n_groups, nb)) {
+        snprintf(ctx->err, sizeof(ctx->err), "%llu heavy segments exceed the %llu segment sums of the level scratch", (unsigned long long)n_seg,
+                 (unsigned long long)msm_lvl_elems(n_groups, nb));
+        return OG_E_INVALID;
+    }
+    if (total && !entries) return OG_E_INVALID;
+    for (uint64_t i = 0; i < total; i++)
+        if ((entries[i] >> 1) >= n_points) { snprintf(ctx->err, sizeof(ctx->err), "entry %llu: point index out of range", (unsigned long long)i); return OG_E_INVALID; }
+    const uint64_t pb = g2 ? 128 : 64;
+    OG_SLOT(ctx, dp, uint8_t, S_IO_A, pb * n_points);
+    OG_SLOT(ctx, de, uint32_t, S_IO_B, 4 * total);
+    OG_SLOT(ctx, dc, uint32_t, S_IO_C, 4ull * n_keys);
+    OG_SLOT(ctx, doff, uint32_t, S_IO_D, 4ull * (n_keys + 1ull));
+    OG_SLOT(ctx, dtot, uint8_t, S_IO_E, pb * n_groups);
+    uint8_t* dbk = nullptr;
+    if (out_buckets) { dbk = (uint8_t*)ctx->slot(S_IO_F, pb * n_keys); if (!dbk) return OG_E_NOMEM; }
+    OG_TRY(clear_flag(ctx));
+    if (n_points) H2D(ctx, dp, points, pb * n_points);
+    if (total) H2D(ctx, de, entries, 4 * total);
+    H2D(ctx, dc, counts, 4ull * n_keys);
+    H2D(ctx, doff, offsets.data(), 4ull * (n_keys + 1ull));
+    if (g2) OG_TRY(msm_bucket_sums_g2(ctx, dp, n_points, de, doff, dc, n_groups, nb, n_entries_max, few_groups != 0, dtot, dbk));
+    else OG_TRY(msm_bucket_sums_g1(ctx, dp, n_points, de, doff, dc, n_groups, nb, n_entries_max, few_groups != 0, dtot, dbk));
+    D2H(ctx, out_totals, dtot, pb * n_groups);
+    if (out_buckets) D2H(ctx, out_buckets, dbk, pb * n_keys);
+    return check_flag(ctx);
+}
+
+int32_t og_field_probe_raw(og_ctx* ctx, int32_t unit, int32_t op, const uint8_t* a, const uint8_t* b, uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (unit < 0 || unit > 1 || op < 0 || op > (unit ? 7 : 3) || (n && (!a || !b || !out))) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    const uint64_t eb = unit ? 64 : 32;
+    OG_SLOT(ctx, da, uint8_t, S_IO_A, eb * n);
+    OG_SLOT(ctx, db, uint8_t, S_IO_B, eb * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_C, eb * n);
+    H2D(ctx, da, a, eb * n); H2D(ctx, db, b, eb * n);
+    if (unit) OG_TRY(field_probe_raw_g2(ctx, op, da, db, n, dout));
+    else OG_TRY(field_probe_raw_g1(ctx, op, da, db, n, dout));
+    D2H(ctx, out, dout, eb * n);
+    OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return OG_OK;
+}
+
 }  // extern "C"

@@ -569,6 +569,23 @@ __global__ void __launch_bounds__(128, OG_ACC1_MINB) k_bucket_acc_sm1(const Affi
     }
     buckets[key] = inf ? XYZZ<Fq>::inf() : XYZZ<Fq>{A.ld(0), A.ld(1), A.ld(2), A.ld(3)};
 }
+
+// Test/debug probe (og_field_probe_raw, unit 0): raw Montgomery limbs in and out, no conversion and no range check, through the
+// product and the squarer (fq_sqr_call) of k_bucket_acc_sm1, with its launch bounds.  In this whole-program build ptxas compiles a
+// copy of every __noinline__ callee into each kernel that calls it, so the probe runs its own copy of fq_sqr_call: the same PTX, but
+// not necessarily the bucket kernel's register allocation.  op 0: a * b, 1: sqr(a), 2: a - b, 3: a.dbl()
+__global__ void __launch_bounds__(128, OG_ACC1_MINB) k_field_probe_g1(int32_t op, const Fq* __restrict__ a, const Fq* __restrict__ b, uint64_t n,
+                                                        Fq* __restrict__ out) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fq x = a[i], y = b[i];
+    out[i] = op == 0 ? OG_ACC_MUL(x, y) : op == 1 ? OG_ACC_SQR(x) : op == 2 ? x - y : x.dbl();
+}
+int32_t field_probe_raw_g1(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out) {
+    if (n) OG_LAUNCH(ctx, k_field_probe_g1, (unsigned)((n + 127) / 128), 128, 0, op, reinterpret_cast<const Fq*>(d_a),
+                     reinterpret_cast<const Fq*>(d_b), n, reinterpret_cast<Fq*>(d_out));
+    return OG_OK;
+}
 #endif
 
 #ifdef OG_MSM_G2
@@ -623,6 +640,35 @@ __global__ void __launch_bounds__(128, OG_ACC2_MINB) k_bucket_acc_sm(const Affin
         if (!g2_madd_lazy(A, q)) inf = true;          // the accumulator stays lazy ([0, 2p)) until the bucket is stored
     }
     buckets[key] = inf ? XYZZ<Fq2>::inf() : XYZZ<Fq2>{A.ld(0).canonical(), A.ld(1).canonical(), A.ld(2).canonical(), A.ld(3).canonical()};
+}
+
+// Test/debug probe (og_field_probe_raw, unit 1): raw Montgomery limbs in and out, no conversion and no range check, through the
+// lazy and canonical Fq2 products of this unit (fq2_mul_lazy_call, fq2_sqr_lazy_call, fq2_mul_call, fq2_sqr_call), with
+// k_bucket_acc_sm's launch bounds.  Like every kernel of this build, the probe gets its own ptxas copy of those callees: the same PTX
+// as the bucket kernel's, not necessarily the same register allocation.  op 0: fq2_mul_lazy, 1: fq2_sqr_lazy, 2: add_lazy, 3: sub_lazy,
+// 4: canonical(a), 5: a * b, 6: a.sqr(), 7: is_zero_lazy(a) (1 or 0 in limb 0 of c0, every other limb 0)
+__global__ void __launch_bounds__(128, OG_ACC2_MINB) k_field_probe_g2(int32_t op, const Fq2* __restrict__ a, const Fq2* __restrict__ b, uint64_t n,
+                                                        Fq2* __restrict__ out) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fq2 x = a[i], y = b[i];
+    Fq2 z;
+    switch (op) {
+        case 0: z = fq2_mul_lazy(x, y); break;
+        case 1: z = fq2_sqr_lazy(x); break;
+        case 2: z = Fq2::add_lazy(x, y); break;
+        case 3: z = Fq2::sub_lazy(x, y); break;
+        case 4: z = x.canonical(); break;
+        case 5: z = x * y; break;
+        case 6: z = x.sqr(); break;
+        default: z = Fq2::zero(); z.c0.l[0] = x.is_zero_lazy() ? 1u : 0u; break;
+    }
+    out[i] = z;
+}
+int32_t field_probe_raw_g2(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out) {
+    if (n) OG_LAUNCH(ctx, k_field_probe_g2, (unsigned)((n + 127) / 128), 128, 0, op, reinterpret_cast<const Fq2*>(d_a),
+                     reinterpret_cast<const Fq2*>(d_b), n, reinterpret_cast<Fq2*>(d_out));
+    return OG_OK;
 }
 #endif
 
@@ -944,7 +990,7 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
     // cap: a bucket that would keep one thread busy far longer than the average goes to a whole CTA
     // (skewed scalars: witness 0/1 values, short scalars whose top window has few distinct digits)
     uint64_t avg = n_entries_max / (n_keys ? n_keys : 1);
-    uint32_t cap = (uint32_t)(4 * avg < 128 ? 128 : 4 * avg);
+    uint32_t cap = msm_heavy_cap(avg);
 #ifdef OG_EXPERIMENT_AFFINE
     if (aff_scratch) {
         OG_TRY((bucket_acc_affine<F>(ctx, d_table, d_sorted, d_offsets, d_counts, n_keys, cap, avg, d_buckets, d_heavy, d_perm, aff_scratch)));
@@ -969,9 +1015,8 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
         if (ctx->acc_stream) OG_CUDA(ctx, stream_handoff(ctx->acc_ev, ctx->acc_stream, hi));
     }
     {
-        // segment length: long enough that the segment sums of ALL heavy buckets fit in the (still unused) reduction scratch
-        // (at most n_keys / 4 heavy buckets, since each holds more than 4 x the average load)
-        uint32_t seg = (uint32_t)(4 * avg < 2048 ? 2048 : 4 * avg);
+        // segment sums go to the (still unused) reduction scratch; they fit it while avg < 512 (msm.cuh: msm_heavy_seg)
+        uint32_t seg = msm_heavy_seg(avg);
         auto k_heavy = k_bucket_heavy<F, HT>;
         OG_LAUNCHN(ctx, "k_heavy_plan", k_heavy_plan<F>, 1, 256, 0, d_heavy, d_counts, n_keys, seg);
         OG_LAUNCHN(ctx, sizeof(F) == 32 ? "k_bucket_heavy_g1" : "k_bucket_heavy_g2", k_heavy, 4 * ctx->sm_count, HT, HT * sizeof(XYZZ<F>), d_table, d_sorted,
@@ -1053,6 +1098,56 @@ size_t msm_aff_scratch_bytes_g2(uint64_t n_keys) { return aff_scratch_bytes_t<Fq
 #else
 size_t msm_aff_scratch_bytes_g2(uint64_t) { return 0; }
 #endif
+#endif  // OG_MSM_G2
+
+// ---- test/debug probe (og_msm_bucket_sums): msm_buckets on bucket lists the caller gives -------------------------------------
+template <class F>
+__global__ void __launch_bounds__(128) k_xyzz_to_bytes(const XYZZ<F>* __restrict__ in, uint64_t n, uint8_t* __restrict__ out) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    constexpr int B = FieldIO<F>::BYTES;
+    Affine<F> a;
+    xyzz_to_affine_ni(&a, &in[i]);
+    FieldIO<F>::store(out + 2 * B * i, a.x);
+    FieldIO<F>::store(out + 2 * B * i + B, a.y);
+}
+
+template <class F>
+static int32_t msm_bucket_sums_t(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted,
+                                 const uint32_t* d_offsets, const uint32_t* d_counts, uint32_t n_groups, uint32_t nb,
+                                 uint64_t n_entries_max, bool few_groups, uint8_t* d_out_totals, uint8_t* d_out_buckets) {
+    const uint32_t n_keys = n_groups * nb;
+    OG_SLOT(ctx, pts, Affine<F>, S_MSM_POINTS, sizeof(Affine<F>) * (size_t)n_points);
+    OG_SLOT(ctx, buckets, XYZZ<F>, S_MSM_BUCKETS, sizeof(XYZZ<F>) * (size_t)n_keys);
+    OG_SLOT(ctx, lvl, XYZZ<F>, S_MSM_SEG, sizeof(XYZZ<F>) * msm_lvl_elems(n_groups, nb));
+    OG_SLOT(ctx, heavy, uint32_t, S_MSM_HEAVY, 4 * (2 * (size_t)n_keys + 4));
+    OG_SLOT(ctx, perm, uint32_t, S_MSM_CURSOR, 4 * (size_t)n_keys);
+    OG_SLOT(ctx, totals, XYZZ<F>, S_MSM_OUT, sizeof(XYZZ<F>) * (size_t)n_groups);
+    if (n_points) OG_LAUNCH(ctx, k_points_to_mont<F>, (n_points + 127) / 128, 128, 0, d_points, (uint64_t)n_points, pts, ctx->d_flag);
+    OG_TRY((msm_buckets<F>(ctx, pts, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, buckets, lvl, heavy, perm, totals,
+                           nullptr, few_groups)));
+    OG_LAUNCH(ctx, k_xyzz_to_bytes<F>, (n_groups + 127) / 128, 128, 0, totals, (uint64_t)n_groups, d_out_totals);
+    // the buckets as the reduction read them: accumulated, heavy ones combined
+    if (d_out_buckets) OG_LAUNCH(ctx, k_xyzz_to_bytes<F>, (n_keys + 127) / 128, 128, 0, buckets, (uint64_t)n_keys, d_out_buckets);
+    return OG_OK;
+}
+
+#ifdef OG_MSM_G1
+int32_t msm_bucket_sums_g1(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
+                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
+                           uint8_t* d_out_totals, uint8_t* d_out_buckets) {
+    return msm_bucket_sums_t<Fq>(ctx, d_points, n_points, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, few_groups,
+                                 d_out_totals, d_out_buckets);
+}
+#endif  // OG_MSM_G1
+
+#ifdef OG_MSM_G2
+int32_t msm_bucket_sums_g2(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
+                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
+                           uint8_t* d_out_totals, uint8_t* d_out_buckets) {
+    return msm_bucket_sums_t<Fq2>(ctx, d_points, n_points, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, few_groups,
+                                  d_out_totals, d_out_buckets);
+}
 #endif  // OG_MSM_G2
 
 

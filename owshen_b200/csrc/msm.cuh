@@ -51,6 +51,31 @@ int32_t msm_buckets_g2(og_ctx* ctx, const G2Affine* d_table, const uint32_t* d_s
 size_t msm_aff_scratch_bytes_g1(uint64_t n_keys);
 size_t msm_aff_scratch_bytes_g2(uint64_t n_keys);
 static inline size_t msm_lvl_elems(uint32_t n_groups, uint32_t nb) { return 4 * ((size_t)n_groups * ((nb + 7) / 8) + 16); }   // RED_FAN = 8
+// Heavy buckets of msm_buckets, with avg = n_entries_max / n_keys: a list of more than cap = max(128, 4 avg) entries goes to
+// k_bucket_heavy, cut into segments of seg = max(2048, 4 avg) entries whose sums are written into d_lvl.  Both values must fit 32 bits
+// (avg < 2^30).  While avg < 512 the segment sums always fit d_lvl: a heavy list takes at most one segment per min(cap + 1, 1024) of
+// its entries, so fewer than (avg + 1) n_keys / min(cap + 1, 1024) <= n_keys / 2 segments exist.  From avg = 512 on, cap == seg, so a
+// list of cap + 1 entries takes two segments and the count can exceed msm_lvl_elems by up to about 3 n_keys / (8 avg) elements.  The
+// MSM and prover callers stay far below avg = 512 (one-shot MSMs 16 to 32, the prover's A, B and C' MSMs about 25, 13 and 34).
+static inline uint32_t msm_heavy_cap(uint64_t avg) { return (uint32_t)(4 * avg < 128 ? 128 : 4 * avg); }
+static inline uint32_t msm_heavy_seg(uint64_t avg) { return (uint32_t)(4 * avg < 2048 ? 2048 : 4 * avg); }
+
+// Test/debug probes behind og_msm_bucket_sums and og_field_probe_raw (not used by the product).
+// msm_bucket_sums_*: msm_buckets (few_groups as given) on caller-given lists -- d_points: n_points affine boundary points;
+// d_sorted / d_offsets / d_counts as msm_buckets reads them, with n_entries_max >= offsets[n_keys] and a heavy plan whose segment
+// sums fit d_lvl (msm_heavy_cap / msm_heavy_seg above; og_msm_bucket_sums checks both); out: n_groups totals and, when
+// d_out_buckets is not null, the n_keys accumulated buckets, as affine boundary points.
+int32_t msm_bucket_sums_g1(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
+                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
+                           uint8_t* d_out_totals, uint8_t* d_out_buckets);
+int32_t msm_bucket_sums_g2(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
+                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
+                           uint8_t* d_out_totals, uint8_t* d_out_buckets);
+// field_probe_raw_*: raw Montgomery limbs in and out, no range check, through the functions the bucket kernels of each unit call
+// (the probe kernels' own ptxas copies of them):
+// G1 (Fq, 32 B) ops 0..3, G2 (Fq2, 64 B) ops 0..7 (msm.cu: k_field_probe_g1 / k_field_probe_g2)
+int32_t field_probe_raw_g1(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out);
+int32_t field_probe_raw_g2(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out);
 
 // one-shot MSMs on device buffers holding boundary bytes (affine points, canonical scalars)
 int32_t msm_g1_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_scalars, uint64_t n, uint8_t* d_out64);

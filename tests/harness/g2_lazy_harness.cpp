@@ -21,7 +21,8 @@ struct HostAcc {                         // the accumulator's four coordinates, 
 
 extern "C" {
 // raw Montgomery limbs in, raw limbs out (no conversion, no reduction): op 0 mul_lazy, 1 sqr_lazy (of a), 2 add_lazy,
-// 3 sub_lazy, 4 canonical (of a); 64 bytes per operand
+// 3 sub_lazy, 4 canonical (of a), 5 the canonical product a * b, 6 the canonical squaring (of a); 64 bytes per operand.
+// The numbering is og_field_probe_raw's for the G2 unit, so tests compare the device's raw limbs with these byte for byte.
 void hl_fq2_op(int op, const uint8_t* a, const uint8_t* b, uint8_t* out, uint64_t n) {
     for (uint64_t i = 0; i < n; i++) {
         Fq2 x = raw2(a + 64 * i), y = raw2(b + 64 * i), z;
@@ -30,6 +31,8 @@ void hl_fq2_op(int op, const uint8_t* a, const uint8_t* b, uint8_t* out, uint64_
             case 1: z = fq2_sqr_lazy(x); break;
             case 2: z = Fq2::add_lazy(x, y); break;
             case 3: z = Fq2::sub_lazy(x, y); break;
+            case 5: z = x * y; break;
+            case 6: z = x.sqr(); break;
             default: z = x.canonical(); break;
         }
         put2(out + 64 * i, z);

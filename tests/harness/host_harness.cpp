@@ -148,6 +148,16 @@ extern "C" void ht_fr_lazy_raw(int op, const uint8_t* a, const uint8_t* b, uint8
     }
 }
 
+// the same for Fq, numbered as og_field_probe_raw's G1 unit: op 0 a * b, 1 a.sqr() (the bucket kernel's squarer), 2 a - b, 3 a.dbl()
+extern "C" void ht_fq_raw(int op, const uint8_t* a, const uint8_t* b, uint8_t* out, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) {
+        Fq x, y, z;
+        memcpy(x.l, a + 32 * i, 32); memcpy(y.l, b + 32 * i, 32);
+        z = op == 0 ? x * y : op == 1 ? x.sqr() : op == 2 ? x - y : x.dbl();
+        memcpy(out + 32 * i, z.l, 32);
+    }
+}
+
 // ---- GLV decomposition (glv.cuh): out = |k1| (32 B) | |k2| (32 B) | sign bits (1 B: bit 0 = k1 < 0, bit 1 = k2 < 0) per scalar
 #include "glv.cuh"
 extern "C" void ht_glv_decompose(const uint8_t* ks, uint8_t* out, uint64_t n) {
