@@ -218,6 +218,23 @@ int32_t og_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, c
                             const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
                             uint32_t batch, uint8_t* witnesses);
 
+/* ---- the association-set withdraw statement (DESIGN.md section 3): a note in the pool and in an approved subset ---- */
+/* Public inputs (root, nullifier_hash, recipient, association_root); the first three are the withdraw statement's.  The
+ * note's commitment MultiMiMC7([nullifier, secret], 0) reaches root along the pool path and association_root along the
+ * path in an association set provider's tree over a subset of the deposits; both trees have the same depth, 1..32.  At
+ * depth 32: 47 949 variables, 47 881 constraints, domain 2^16. */
+int32_t og_association_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_association_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                   uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: nullifier, secret, recipient 32 B each; siblings
+ * and assoc_siblings depth * 32 B each (leaf level first); path_bits and assoc_path_bits one word each (bit l set when the
+ * level-l node is a right child).  Both roots are derived from the paths: a note that is not a leaf of a tree gives a root
+ * that no one published. */
+int32_t og_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifiers, const uint8_t* secrets,
+                               const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
+                               const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -281,6 +298,18 @@ int32_t og_groth16_prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_
                                       const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
                                       const uint8_t* d_out_nullifiers, const uint8_t* d_out_secrets, const uint64_t* d_out_amounts,
                                       uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of association-set withdraw proofs, witness generation on the GPU; inputs as in og_association_witness.
+ * OG_E_INVALID unless the key has an association statement's shape (the depth is recognised from it).  public_out
+ * (optional): batch * 4 * 32 B = root, nullifier_hash, recipient, association_root. */
+int32_t og_groth16_prove_association(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets,
+                                     const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
+                                     const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch,
+                                     const uint8_t* rs, uint8_t* proofs, uint8_t* public_out);
+/* same with every buffer already in HBM; no synchronisation */
+int32_t og_groth16_prove_association_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                         const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits,
+                                         const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
+                                         const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

@@ -99,6 +99,9 @@ _SIGS = {
     "og_transfer_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_transfer_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_transfer_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p]),
+    "og_association_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_association_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_association_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -113,6 +116,8 @@ _SIGS = {
     "og_groth16_prove_deposit_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_transfer": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_association": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_association_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -231,6 +236,19 @@ def _transfer_args(fn, batch, depth, roots, tokens, recipients, in_nullifiers, i
             _need_len(buf, size * batch, f"{fn}: {name}")
     return [_ptr(x) for x in (roots, tokens, recipients, in_nullifiers, in_secrets, amounts[0], in_siblings, bits,
                               out_nullifiers, out_secrets, amounts[1])]
+
+
+def _association_args(fn, batch, depth, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits):
+    """Length checks of an association batch's seven input arrays -> their pointers in C ABI order."""
+    bits, abits = _u32_array(path_bits), _u32_array(assoc_path_bits)
+    for name, buf, size in (("nullifiers", nullifiers, 32), ("secrets", secrets, 32), ("recipients", recipients, 32),
+                            ("siblings", siblings, 32 * depth), ("path_bits", bits, 4),
+                            ("assoc_siblings", assoc_siblings, 32 * depth), ("assoc_path_bits", abits, 4)):
+        if isinstance(buf, C.Array):        # converted from a sequence above
+            _need(C.sizeof(buf) == size * batch, f"{fn}: {name}: expected {batch} values, got {len(buf)}")
+        else:
+            _need_len(buf, size * batch, f"{fn}: {name}")
+    return [_ptr(x) for x in (nullifiers, secrets, recipients, siblings, bits, assoc_siblings, abits)]
 
 
 def fr_bytes(x: int) -> bytes:
@@ -556,6 +574,20 @@ class Context:
         _check(lib().og_transfer_witness(self._h, depth, *args, n, out), self)
         return out.raw
 
+    def association_witness(self, depth, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits) -> bytes:
+        """Full assignments of the depth-`depth` association-set withdraw statement, n_vars * 32 bytes per proof, computed on
+        the GPU.  Per proof: nullifier, secret, recipient 32 bytes each; siblings and assoc_siblings depth elements each (the
+        pool path and the association path, leaf level first); path_bits and assoc_path_bits one word each."""
+        _need(1 <= depth <= 32 and _blen(nullifiers) is not None and _blen(nullifiers) % 32 == 0,
+              "association_witness: depth must be 1..32 and nullifiers a multiple of 32 bytes")
+        n = _blen(nullifiers) // 32
+        args = _association_args("association_witness", n, depth, nullifiers, secrets, recipients, siblings, path_bits,
+                                 assoc_siblings, assoc_path_bits)
+        nv = association_r1cs_info(depth)["n_vars"]
+        out = C.create_string_buffer(32 * n * nv)
+        _check(lib().og_association_witness(self._h, depth, *args, n, out), self)
+        return out.raw
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -621,6 +653,25 @@ def transfer_r1cs_export(depth: int, which: str):
     return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
 
 
+def association_r1cs_info(depth: int) -> dict:
+    v = [C.c_uint32() for _ in range(4)]
+    _check(lib().og_association_r1cs_info(depth, *[C.byref(x) for x in v]))
+    return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+
+
+def association_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` association R1CS."""
+    w = "ABC".index(which)
+    nnz = C.c_uint64()
+    _check(lib().og_association_r1cs_export(depth, w, None, None, None, C.byref(nnz)))
+    nc = association_r1cs_info(depth)["n_constraints"]
+    ptr = (C.c_uint32 * (nc + 1))()
+    col = (C.c_uint32 * nnz.value)()
+    val = C.create_string_buffer(32 * nnz.value)
+    _check(lib().og_association_r1cs_export(depth, w, ptr, col, val, C.byref(nnz)))
+    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -665,6 +716,14 @@ def setup_transfer(ctx: Context, depth: int, tau: int, alpha: int, beta: int, ga
     setup_r1cs.  The key records depth 0; the prover recognises it as a transfer key by its shape."""
     info = transfer_r1cs_info(depth)
     return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(transfer_r1cs_export(depth, m) for m in "ABC"),
+                      tau, alpha, beta, gamma, delta)
+
+
+def setup_association(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` association-set withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS
+    through setup_r1cs.  The key records depth 0; the prover recognises it as an association key by its shape."""
+    info = association_r1cs_info(depth)
+    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(association_r1cs_export(depth, m) for m in "ABC"),
                       tau, alpha, beta, gamma, delta)
 
 
@@ -739,6 +798,11 @@ def ptau_prepare_deposit(ctx: Context, acc: bytes):
 def ptau_prepare_transfer(ctx: Context, acc: bytes, depth: int):
     info = transfer_r1cs_info(depth)
     return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(transfer_r1cs_export(depth, m) for m in "ABC"))
+
+
+def ptau_prepare_association(ctx: Context, acc: bytes, depth: int):
+    info = association_r1cs_info(depth)
+    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(association_r1cs_export(depth, m) for m in "ABC"))
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -853,6 +917,32 @@ class ProvingKey:
         proofs = C.create_string_buffer(PROOF_BYTES * batch)
         pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
         _check(lib().og_groth16_prove_transfer(self.ctx._h, self._h, *args, batch, _ptr(rs), proofs, pub), self.ctx)
+        return proofs.raw, (pub.raw if want_public else None)
+
+    @property
+    def association_depth(self):
+        """The depth d whose association statement has this key's shape (association_r1cs_info), or None."""
+        for d in range(1, 33):
+            info = association_r1cs_info(d)
+            if (info["n_vars"], info["n_pub"]) == (self.n_vars, self.n_pub):
+                return d
+        return None
+
+    def prove_association(self, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits, rs,
+                          want_public=True):
+        """Batch of association-set withdraw proofs from the secret inputs (witness generation on the GPU).  Inputs as in
+        Context.association_witness; returns (proofs, public_inputs) with public inputs (root, nullifier_hash, recipient,
+        association_root) per proof."""
+        depth = self.association_depth
+        if depth is None:
+            raise OwshenB200Error(OG_E_INVALID, "prove_association: this key was not made for an association statement")
+        _need(_blen(rs) is not None and _blen(rs) % 64 == 0, "prove_association: rs must be a buffer of 64 bytes (r, s) per proof")
+        batch = _blen(rs) // 64
+        args = _association_args("prove_association", batch, depth, nullifiers, secrets, recipients, siblings, path_bits,
+                                 assoc_siblings, assoc_path_bits)
+        proofs = C.create_string_buffer(PROOF_BYTES * batch)
+        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
+        _check(lib().og_groth16_prove_association(self.ctx._h, self._h, *args, batch, _ptr(rs), proofs, pub), self.ctx)
         return proofs.raw, (pub.raw if want_public else None)
 
     def prover_plan(self, batch: int) -> dict:

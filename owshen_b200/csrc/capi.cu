@@ -1000,6 +1000,63 @@ int32_t og_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, c
     return check_flag(ctx);
 }
 
+// ---- association-set withdraw statement ---------------------------------------------------------------------------
+int32_t og_association_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    if (depth == 0 || depth > 32) return OG_E_INVALID;
+    AssociationLayout L = AssociationLayout::make(depth);
+    if (n_constraints) *n_constraints = L.n_constraints;
+    if (n_vars) *n_vars = L.n_vars;
+    if (n_pub) *n_pub = ASSOCIATION_N_PUB;
+    if (log_m) *log_m = groth16_domain_log(L.n_constraints, ASSOCIATION_N_PUB);
+    return OG_OK;
+}
+int32_t og_association_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    if (depth == 0 || depth > 32 || which < 0 || which > 2 || !nnz) return OG_E_INVALID;
+    R1cs cs = AssociationBuilder::build(depth);
+    const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
+    *nnz = M.col.size();
+    if (!row_ptr || !col_idx || !coeffs) return OG_OK;
+    memcpy(row_ptr, M.row_ptr.data(), 4 * M.row_ptr.size());
+    memcpy(col_idx, M.col.data(), 4 * M.col.size());
+    for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
+    return OG_OK;
+}
+
+// the seven host input arrays of an association batch, copied into one device slot (each array 256-byte aligned)
+static int32_t stage_association_inputs(og_ctx* ctx, uint32_t depth, uint32_t batch, const uint8_t* nullifiers, const uint8_t* secrets,
+                                        const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
+                                        const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, AssociationInputs& d) {
+    const uint64_t b = batch;
+    const void* src[7] = {nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits};
+    const uint64_t bytes[7] = {32 * b, 32 * b, 32 * b, 32ull * depth * b, 4 * b, 32ull * depth * b, 4 * b};
+    uint64_t off[7], tot = 0;
+    for (int k = 0; k < 7; k++) { off[k] = tot; tot += (bytes[k] + 255) & ~255ull; }
+    OG_SLOT(ctx, base, uint8_t, S_IO_ASSOCIATION, tot);
+    for (int k = 0; k < 7; k++) H2D(ctx, base + off[k], src[k], bytes[k]);
+    d.nullifiers = base + off[0]; d.secrets = base + off[1]; d.recipients = base + off[2];
+    d.siblings = base + off[3]; d.path_bits = (const uint32_t*)(base + off[4]);
+    d.assoc_siblings = base + off[5]; d.assoc_path_bits = (const uint32_t*)(base + off[6]);
+    return OG_OK;
+}
+
+int32_t og_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* recipients,
+                               const uint8_t* siblings, const uint32_t* path_bits, const uint8_t* assoc_siblings,
+                               const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses) {
+    OG_ENTER(ctx);
+    if (!ctx || depth == 0 || depth > 32 || !nullifiers || !secrets || !recipients || !siblings || !path_bits || !assoc_siblings ||
+        !assoc_path_bits || !witnesses) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    AssociationLayout L = AssociationLayout::make(depth);
+    AssociationInputs d;
+    OG_TRY(stage_association_inputs(ctx, depth, batch, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
+                                    assoc_path_bits, d));
+    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
+    OG_TRY(clear_flag(ctx));
+    OG_TRY(association_witness_bytes_dev(ctx, depth, d, batch, dout));
+    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
+    return check_flag(ctx);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1161,6 +1218,43 @@ int32_t og_groth16_prove_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* r
     OG_TRY(prove_transfer_dev(ctx, pk, d, batch, drs, dpr, public_out ? dpub : nullptr));
     D2H(ctx, proofs, dpr, 256ull * batch);
     if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * TRANSFER_N_PUB);
+    return check_flag(ctx);
+}
+
+int32_t og_groth16_prove_association_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                         const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits,
+                                         const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
+                                         const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    OG_ENTER(ctx);
+    if (!ctx || !pk || !d_nullifiers || !d_secrets || !d_recipients || !d_siblings || !d_path_bits || !d_assoc_siblings ||
+        !d_assoc_path_bits || !d_rs || !d_proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    AssociationInputs d{d_nullifiers, d_secrets, d_recipients, d_siblings, d_path_bits, d_assoc_siblings, d_assoc_path_bits};
+    return prove_association_dev(ctx, pk, d, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_association(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets,
+                                     const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
+                                     const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch, const uint8_t* rs,
+                                     uint8_t* proofs, uint8_t* public_out) {
+    OG_ENTER(ctx);
+    if (!ctx || !pk || !nullifiers || !secrets || !recipients || !siblings || !path_bits || !assoc_siblings || !assoc_path_bits || !rs ||
+        !proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    const uint32_t depth = pk_association_depth(pk);
+    if (depth == 0) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    AssociationInputs d;
+    OG_TRY(stage_association_inputs(ctx, depth, batch, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
+                                    assoc_path_bits, d));
+    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
+    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
+    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * ASSOCIATION_N_PUB);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, drs, rs, 64ull * batch);
+    OG_TRY(prove_association_dev(ctx, pk, d, batch, drs, dpr, public_out ? dpub : nullptr));
+    D2H(ctx, proofs, dpr, 256ull * batch);
+    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * ASSOCIATION_N_PUB);
     return check_flag(ctx);
 }
 

@@ -105,6 +105,7 @@ enum Slot {
     S_PR_SORT_STAGE, S_L1_SORT_STAGE, S_PR_SORT_TILES, S_L1_SORT_TILES,   // only for keys whose sort scratch outgrows bk2 / heavy
     S_IO_TRANSFER,                                                          // the staged input arrays of a transfer batch
     S_IO_NOTE, S_NOTE_KEYS, S_NOTE_PREP,                                    // note encryption / scanning (note_impl.cuh)
+    S_IO_ASSOCIATION,                                                       // the staged input arrays of an association batch
     S_COUNT
 };
 static_assert(S_COUNT <= N_SLOTS, "grow N_SLOTS");

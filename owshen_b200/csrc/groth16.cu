@@ -2,7 +2,7 @@
 // development setup.  The reference has no prover (SURVEY.md section 0); conventions are frozen in
 // DESIGN.md section 4 and checked bit-for-bit against oracle/groth16.py and oracle/cpu.
 //
-// Once per batch:  witness  k_withdraw_witness / k_deposit_witness / k_transfer_witness (mimc.cu): every MiMC7 round value
+// Once per batch:  witness  k_withdraw_witness / k_deposit_witness / k_transfer_witness / k_association_witness (mimc.cu): every MiMC7 round value
 //                  -> W[batch][n_vars+2] (or full witnesses from the caller)
 // Per chunk of B proofs (default min(1024, the lane budget / one proof's scratch); everything stays in HBM, nothing returns to the host until the proofs):
 //   a, b, c      k_abc: sparse A.w, B.w over the CSR kept in L2, c = a*b
@@ -483,13 +483,15 @@ static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
 
 // where a chunk's witness rows come from
 struct WitnessSource {
-    enum Kind { WITHDRAW, DEPOSIT, TRANSFER, FULL } kind = FULL;
+    enum Kind { WITHDRAW, DEPOSIT, TRANSFER, ASSOCIATION, FULL } kind = FULL;
     const uint8_t *d_null = nullptr, *d_sec = nullptr;                       // secret inputs (prove_withdraw, prove_deposit)
     const uint8_t *d_rec = nullptr, *d_sib = nullptr;                        // withdraw: recipients, siblings
     const uint32_t* d_bits = nullptr;
     const uint8_t* d_dep = nullptr;                                          // deposit: depositors
     TransferInputs tin = {};                                                 // transfer: every input array
     uint32_t transfer_depth = 0;
+    AssociationInputs ain = {};                                              // association: every input array
+    uint32_t association_depth = 0;
     const uint8_t* d_wit = nullptr;                                          // or full witnesses (prove)
     uint8_t* d_public = nullptr;
 };
@@ -510,9 +512,12 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
                                                 src.d_sib + 32ull * off * pk->depth, src.d_bits + off, B, W));
         } else if (src.kind == WitnessSource::DEPOSIT) {
             OG_TRY(deposit_witness_strided_dev(ctx, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_dep + 32ull * off, B, W));
-        } else {
+        } else if (src.kind == WitnessSource::TRANSFER) {
             TransferLayout L = TransferLayout::make(src.transfer_depth);
             OG_TRY(transfer_witness_strided_dev(ctx, L, b.w_stride, src.tin.at(off, src.transfer_depth), B, W));
+        } else {
+            AssociationLayout L = AssociationLayout::make(src.association_depth);
+            OG_TRY(association_witness_strided_dev(ctx, L, b.w_stride, src.ain.at(off, src.association_depth), B, W));
         }
         if (src.d_public) OG_LAUNCH(ctx, k_public_out, (B * pk->n_pub + 127) / 128, 128, 0, W, b.w_stride, B, pk->n_pub, src.d_public + 32ull * off * pk->n_pub);
     }
@@ -647,6 +652,26 @@ int32_t prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const TransferInputs& i
     return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
 }
 
+uint32_t pk_association_depth(const og_pk* pk) {
+    if (pk->n_pub != ASSOCIATION_N_PUB) return 0;
+    for (uint32_t d = 1; d <= 32; d++) {
+        AssociationLayout L = AssociationLayout::make(d);
+        if (pk->n_vars == L.n_vars && pk->n_constraints == L.n_constraints) return d;
+    }
+    return 0;
+}
+
+int32_t prove_association_dev(og_ctx* ctx, const og_pk* pk, const AssociationInputs& in, uint32_t batch, const uint8_t* d_rs,
+                              uint8_t* d_proofs, uint8_t* d_public) {
+    const uint32_t depth = pk_association_depth(pk);
+    if (depth == 0) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    WitnessSource src;
+    src.kind = WitnessSource::ASSOCIATION;
+    src.ain = in; src.association_depth = depth; src.d_public = d_public;
+    return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
+}
+
 int32_t prove_witness_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs) {
     if (batch == 0) return OG_OK;
     WitnessSource src;
@@ -696,6 +721,16 @@ int32_t transfer_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const TransferIn
     Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
     if (!W) return OG_E_NOMEM;
     OG_TRY(transfer_witness_strided_dev(ctx, L, L.n_vars, in, batch, W));
+    uint64_t tot = (uint64_t)batch * L.n_vars;
+    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
+    return OG_OK;
+}
+
+int32_t association_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const AssociationInputs& in, uint32_t batch, uint8_t* d_out) {
+    AssociationLayout L = AssociationLayout::make(depth);
+    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
+    if (!W) return OG_E_NOMEM;
+    OG_TRY(association_witness_strided_dev(ctx, L, L.n_vars, in, batch, W));
     uint64_t tot = (uint64_t)batch * L.n_vars;
     OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
     return OG_OK;

@@ -24,6 +24,10 @@ int32_t prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, c
 uint32_t pk_transfer_depth(const og_pk* pk);
 int32_t prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const TransferInputs& in, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
                            uint8_t* d_public);
+// the depth d in 1..32 whose association layout matches the key's n_vars, n_constraints and n_pub = 4; 0 = not an association key
+uint32_t pk_association_depth(const og_pk* pk);
+int32_t prove_association_dev(og_ctx* ctx, const og_pk* pk, const AssociationInputs& in, uint32_t batch, const uint8_t* d_rs,
+                              uint8_t* d_proofs, uint8_t* d_public);
 // the chunk size and lanes prove_batch uses for `batch` proofs with this key, and the scratch bytes of one lane
 void pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane);
 int32_t prove_witness_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs);
@@ -33,6 +37,7 @@ int32_t withdraw_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const uint8_t* d
 int32_t deposit_witness_bytes_dev(og_ctx* ctx, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
                                   uint8_t* d_out);
 int32_t transfer_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const TransferInputs& in, uint32_t batch, uint8_t* d_out);
+int32_t association_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const AssociationInputs& in, uint32_t batch, uint8_t* d_out);
 // byte offsets of a serialized pk's sections (og_load_pk's layout); false if the header or a section is malformed
 struct PkLayout {
     uint32_t depth, n_constraints, n_vars, n_pub, log_m;

@@ -1,6 +1,6 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
 // paths (BASELINE config 2), level-by-level tree build, and the witness generators of the withdraw,
-// deposit and transfer statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
+// deposit, transfer and association statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -118,6 +118,28 @@ __global__ void __launch_bounds__(32) k_merkle_paths(const uint8_t* __restrict__
     }
 }
 
+// The witness of a Merkle path from the leaf `cur`: `depth` level blocks (sibling, bit, left, perm1[perm], perm2[perm], out)
+// written from v on, lvl_size elements apart, with the siblings from sp (32 B canonical each) and bit l of `bits` set when
+// the node is a right child.  Returns the root.  Shared by the withdraw, transfer and association witness kernels.
+__device__ __forceinline__ Fr witness_path(Fr cur, Fr* v, uint32_t depth, uint32_t lvl_size, uint32_t perm, const uint8_t* sp,
+                                           uint32_t bits, int* flag) {
+    const Fr one = Fr::one();
+#pragma unroll 1
+    for (uint32_t l = 0; l < depth; l++) {
+        Fr* lv = v + l * lvl_size;
+        Fr sib = load_canonical<Fr>(sp + 32 * l, flag);
+        bool right = (bits >> l) & 1;
+        Fr a = right ? sib : cur;
+        Fr b = right ? cur : sib;
+        lv[0] = sib;
+        lv[1] = right ? one : Fr::zero();
+        lv[2] = a;
+        cur = mimc7_hash2<true>(a, b, lv + 3, lv + 3 + perm);
+        lv[3 + 2 * perm] = cur;
+    }
+    return cur;
+}
+
 // Witness of the withdraw statement, layout of DESIGN.md section 3 (== oracle/withdraw_circuit.py).
 // One thread per proof; W is [batch][n_vars] in Montgomery form.
 __global__ void __launch_bounds__(32) k_withdraw_witness(WithdrawLayout L, uint32_t w_stride, const uint8_t* __restrict__ nullifiers,
@@ -137,22 +159,7 @@ __global__ void __launch_bounds__(32) k_withdraw_witness(WithdrawLayout L, uint3
     w[2] = one + nu + mimc7_hash<true>(nu, one, w + 7);
     Fr cur = mimc7_hash2<true>(nu, se, w + L.cm_base, w + L.cm_base + L.perm);
     w[L.cm_out] = cur;
-    uint32_t bits = path_bits[p];
-    const uint8_t* sp = siblings + (uint64_t)p * L.depth * 32;
-#pragma unroll 1
-    for (uint32_t l = 0; l < L.depth; l++) {
-        Fr* v = w + L.lvl_base + l * L.lvl_size;
-        Fr sib = load_canonical<Fr>(sp + 32 * l, flag);
-        bool right = (bits >> l) & 1;
-        Fr a = right ? sib : cur;
-        Fr b = right ? cur : sib;
-        v[0] = sib;
-        v[1] = right ? one : Fr::zero();
-        v[2] = a;
-        cur = mimc7_hash2<true>(a, b, v + 3, v + 3 + L.perm);
-        v[3 + 2 * L.perm] = cur;
-    }
-    w[1] = cur;
+    w[1] = witness_path(cur, w + L.lvl_base, L.depth, L.lvl_size, L.perm, siblings + (uint64_t)p * L.depth * 32, path_bits[p], flag);
 }
 
 // Witness of the deposit statement, layout of DESIGN.md section 3 (== oracle/deposit_circuit.py).
@@ -213,21 +220,8 @@ __global__ void __launch_bounds__(128) k_transfer_witness(TransferLayout L, uint
             Fr nu = load_canonical<Fr>(in.in_null + 64ull * p + 32 * i, flag);
             Fr se = load_canonical<Fr>(in.in_sec + 64ull * p + 32 * i, flag);
             Fr cur = transfer_note(L, v, nu, se, token, in.in_amounts[2ull * p + i], L.in_cm, L.in_cm_out);
-            const uint32_t bits = in.in_bits[2ull * p + i];
-            const uint8_t* sp = in.in_sib + 32ull * L.depth * (2ull * p + i);
-#pragma unroll 1
-            for (uint32_t l = 0; l < L.depth; l++) {
-                Fr* lv = v + L.lvl_base + l * L.lvl_size;
-                Fr sib = load_canonical<Fr>(sp + 32 * l, flag);
-                bool right = (bits >> l) & 1;
-                Fr a = right ? sib : cur;
-                Fr b = right ? cur : sib;
-                lv[0] = sib;
-                lv[1] = right ? one : Fr::zero();
-                lv[2] = a;
-                cur = mimc7_hash2<true>(a, b, lv + 3, lv + 3 + L.perm);
-                lv[3 + 2 * L.perm] = cur;
-            }
+            witness_path(cur, v + L.lvl_base, L.depth, L.lvl_size, L.perm, in.in_sib + 32ull * L.depth * (2ull * p + i),
+                         in.in_bits[2ull * p + i], flag);
         } else {
             const uint32_t j = role - 2;
             // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
@@ -252,6 +246,37 @@ __global__ void __launch_bounds__(128) k_transfer_witness(TransferLayout L, uint
         Fr a_in = w[L.inp(0) + 2] + w[L.inp(1) + 2], a_out = w[L.out(0) + 2] + w[L.out(1) + 2];
         w[2] = a_out - a_in;
         w[10] = (w[5] - w[6]).inv();   // inv(0) = 0: two inputs with one nullifier leave the row unsatisfiable
+    }
+}
+
+// Witness of the association-set withdraw statement, layout of DESIGN.md section 3 (== oracle/association_circuit.py); row p
+// starts at W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with two warps, one per independent chain of a proof,
+// so no warp diverges and a proof's critical path stays at about one withdraw path:
+//   warp 0   ONE, recipient, recipient_sq, the nullifier hash, the commitment with its round values, the pool path, root
+//   warp 1   the commitment again in registers (no stores), the association path, association_root
+// The warps write disjoint variables, so no barrier is needed.
+__global__ void __launch_bounds__(64) k_association_witness(AssociationLayout L, uint32_t w_stride, AssociationInputs in, uint32_t batch,
+                                                            Fr* __restrict__ W, int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    if (p >= batch) return;
+    Fr* w = W + (uint64_t)p * w_stride;
+    Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
+    Fr se = load_canonical<Fr>(in.secrets + 32ull * p, flag);
+    if (role == 0) {
+        Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+        Fr one = Fr::one();
+        w[0] = one; w[3] = re; w[5] = nu; w[6] = se;
+        w[7] = re.sqr();
+        // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
+        w[2] = one + nu + mimc7_hash<true>(nu, one, w + 8);
+        Fr cm = mimc7_hash2<true>(nu, se, w + L.cm_base, w + L.cm_base + L.perm);
+        w[L.cm_out] = cm;
+        w[1] = witness_path(cm, w + L.pool_base, L.depth, L.lvl_size, L.perm, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
+    } else {
+        Fr cm = mimc7_hash2<false>(nu, se, nullptr, nullptr);
+        w[4] = witness_path(cm, w + L.assoc_base, L.depth, L.lvl_size, L.perm, in.assoc_siblings + 32ull * L.depth * p,
+                            in.assoc_path_bits[p], flag);
     }
 }
 
@@ -336,6 +361,14 @@ int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint3
     if (batch == 0) return OG_OK;
     if (w_stride < L.n_vars) return OG_E_INVALID;
     OG_LAUNCH(ctx, k_transfer_witness, (batch + 31) / 32, 128, 0, L, w_stride, in, batch, d_W, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t association_witness_strided_dev(og_ctx* ctx, const AssociationLayout& L, uint32_t w_stride, const AssociationInputs& in,
+                                        uint32_t batch, Fr* d_W) {
+    if (batch == 0) return OG_OK;
+    if (w_stride < L.n_vars) return OG_E_INVALID;
+    OG_LAUNCH(ctx, k_association_witness, (batch + 31) / 32, 64, 0, L, w_stride, in, batch, d_W, ctx->d_flag);
     return OG_OK;
 }
 

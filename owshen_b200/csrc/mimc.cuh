@@ -1,6 +1,6 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit and transfer statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
-// oracle/deposit_circuit.py: Layout and oracle/transfer_circuit.py: Layout).
+// withdraw, deposit, transfer and association statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
+// oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout and oracle/association_circuit.py: Layout).
 #pragma once
 #include "common.cuh"
 
@@ -93,6 +93,45 @@ struct TransferInputs {
     }
 };
 
+constexpr uint32_t ASSOCIATION_N_PUB = 4;
+
+// 0 ONE | 1 root | 2 nullifier_hash | 3 recipient | 4 association_root | 5 nullifier | 6 secret | 7 recipient_sq
+// | 8.. nullifier-hash permutation | commitment perm1, perm2, out | depth pool levels | depth association levels
+// (oracle/association_circuit.py); a level block is the withdraw statement's.
+struct AssociationLayout {
+    uint32_t depth, perm, cm_base, cm_out, pool_base, assoc_base, lvl_size, n_vars, n_constraints;
+    static AssociationLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        AssociationLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        L.cm_base = 8 + L.perm;
+        L.cm_out = L.cm_base + 2 * L.perm;
+        L.lvl_size = 2 * L.perm + 4;
+        L.pool_base = L.cm_out + 1;
+        L.assoc_base = L.pool_base + depth * L.lvl_size;
+        L.n_vars = L.assoc_base + depth * L.lvl_size;
+        L.n_constraints = 5 + 3 * L.perm + depth * (4 * L.perm + 6);
+        return L;
+    }
+};
+
+// the caller's inputs of a batch of association-set withdrawals: per proof 32 B each of nullifier, secret, recipient,
+// depth siblings per tree and one path-bits word per tree
+struct AssociationInputs {
+    const uint8_t *nullifiers, *secrets, *recipients, *siblings;
+    const uint32_t* path_bits;
+    const uint8_t* assoc_siblings;
+    const uint32_t* assoc_path_bits;
+    // the same inputs from proof `off` on
+    AssociationInputs at(uint32_t off, uint32_t depth) const {
+        AssociationInputs a = *this;
+        a.nullifiers += 32ull * off; a.secrets += 32ull * off; a.recipients += 32ull * off;
+        a.siblings += 32ull * depth * off; a.path_bits += off;
+        a.assoc_siblings += 32ull * depth * off; a.assoc_path_bits += off;
+        return a;
+    }
+};
+
 int32_t mimc_hash2_dev(og_ctx* ctx, const uint8_t* d_l, const uint8_t* d_r, uint64_t n, uint8_t* d_out);
 int32_t mimc_merkle_paths_dev(og_ctx* ctx, const uint8_t* d_leaves, const uint8_t* d_siblings, const uint32_t* d_bits,
                               uint32_t n_paths, uint32_t depth, uint8_t* d_out);
@@ -107,6 +146,8 @@ int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_
                                     uint32_t batch, Fr* d_W);
 int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint32_t w_stride, const TransferInputs& in, uint32_t batch,
                                      Fr* d_W);
+int32_t association_witness_strided_dev(og_ctx* ctx, const AssociationLayout& L, uint32_t w_stride, const AssociationInputs& in,
+                                        uint32_t batch, Fr* d_W);
 
 // BabyJubJub batch verification (bjj_impl.cuh); out[i] in {0, 1, 2 = public key does not decompress}
 int32_t bjj_verify_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_odd, const uint8_t* d_msgs, const uint8_t* d_sigs,

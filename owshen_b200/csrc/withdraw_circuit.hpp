@@ -1,8 +1,8 @@
-// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit and transfer statements'
+// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit, transfer and association statements'
 // R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these are the
 // product's own definitions, checked entry for entry against the independently written
-// oracle/withdraw_circuit.py, oracle/deposit_circuit.py and oracle/transfer_circuit.py through
-// og_withdraw_r1cs_export, og_deposit_r1cs_export and og_transfer_r1cs_export.
+// oracle/withdraw_circuit.py, oracle/deposit_circuit.py, oracle/transfer_circuit.py and oracle/association_circuit.py
+// through og_withdraw_r1cs_export, og_deposit_r1cs_export, og_transfer_r1cs_export and og_association_r1cs_export.
 //
 // withdraw
 //   public : root, nullifier_hash, recipient
@@ -18,6 +18,11 @@
 //   private: two input notes (nullifier, secret, amount, siblings[depth], bits[depth]), two output notes
 //   note commitment = MultiMiMC7([nullifier, secret, token, amount], 0), amounts range-checked to 64 bits;
 //   nonzero inputs open under root; in0 + in1 + public_amount = out0 + out1; nh[0] != nh[1]; recipient^2 bound.
+// association
+//   public : root, nullifier_hash, recipient, association_root
+//   private: nullifier, secret, siblings[depth], bits[depth], assoc_siblings[depth], assoc_bits[depth]
+//   withdraw's nullifier hash and commitment; the commitment reaches root along the pool path and association_root along
+//   the association path (one depth for both trees); recipient^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -96,6 +101,24 @@ struct Mimc7Builder {
     void hash2(const LC& left, const LC& right, uint32_t perm1, uint32_t perm2, uint32_t out) {
         multi_hash({&left, &right}, LC(), {perm1, perm2}, out);
     }
+    // The `depth` levels of a Merkle path from the leaf variable `cur`, level l's block (sibling, bit, left, perm1, perm2, out)
+    // at base + l * lvl_size: bit * (bit - ONE) = 0, bit * (sib - cur) = left - cur, then left, right = sib + cur - left
+    // hashed into out.  Returns the variable of the root it reaches.
+    uint32_t merkle_path(uint32_t cur, uint32_t base, uint32_t lvl_size, uint32_t depth) {
+        const uint32_t P = 4 * n_rounds;
+        for (uint32_t l = 0; l < depth; l++) {
+            uint32_t lb = base + l * lvl_size;
+            uint32_t sib = lb, bit = lb + 1, left = lb + 2, p1 = lb + 3, p2 = lb + 3 + P, out = lb + 3 + 2 * P;
+            LC vbit = lc_var(bit), m1 = lc_neg_var(0), vsib = lc_var(sib), ncur = lc_neg_var(cur), vleft = lc_var(left), vcur = lc_var(cur);
+            LC nleft = lc_neg_var(left);
+            cs.add(vbit, lc_sum({&vbit, &m1}), LC());
+            cs.add(vbit, lc_sum({&vsib, &ncur}), lc_sum({&vleft, &ncur}));
+            LC right = lc_sum({&vsib, &vcur, &nleft});
+            hash2(vleft, right, p1, p2, out);
+            cur = out;
+        }
+        return cur;
+    }
 };
 
 struct WithdrawBuilder {
@@ -109,18 +132,7 @@ struct WithdrawBuilder {
         LC nu = lc_var(V_NULL);
         b.multi_hash({&nu}, lc_var(V_ONE), {V_NH_PERM}, V_NHASH);
         b.hash2(lc_var(V_NULL), lc_var(V_SECRET), L.cm_base, L.cm_base + L.perm, L.cm_out);
-        uint32_t cur = L.cm_out;
-        for (uint32_t l = 0; l < depth; l++) {
-            uint32_t base = L.lvl_base + l * L.lvl_size;
-            uint32_t sib = base, bit = base + 1, left = base + 2, p1 = base + 3, p2 = base + 3 + L.perm, out = base + 3 + 2 * L.perm;
-            LC vbit = lc_var(bit), m1 = lc_neg_var(V_ONE), vsib = lc_var(sib), ncur = lc_neg_var(cur), vleft = lc_var(left), vcur = lc_var(cur);
-            LC nleft = lc_neg_var(left);
-            b.cs.add(vbit, lc_sum({&vbit, &m1}), LC());
-            b.cs.add(vbit, lc_sum({&vsib, &ncur}), lc_sum({&vleft, &ncur}));
-            LC right = lc_sum({&vsib, &vcur, &nleft});
-            b.hash2(vleft, right, p1, p2, out);
-            cur = out;
-        }
+        const uint32_t cur = b.merkle_path(L.cm_out, L.lvl_base, L.lvl_size, depth);
         LC vcur = lc_var(cur), nroot = lc_neg_var(V_ROOT);
         b.cs.add(lc_sum({&vcur, &nroot}), lc_var(V_ONE), LC());
         return b.cs;
@@ -175,18 +187,7 @@ struct TransferBuilder {
             b.multi_hash({&nu}, lc_var(V_ONE), {v + L.nh_perm}, V_NH + i);
             range(b, v);
             commitment(b, v, v + L.in_cm, v + L.in_cm_out, P);
-            uint32_t cur = v + L.in_cm_out;
-            for (uint32_t l = 0; l < depth; l++) {
-                uint32_t base = v + L.lvl_base + l * L.lvl_size;
-                uint32_t sib = base, bit = base + 1, left = base + 2, p1 = base + 3, p2 = base + 3 + P, out = base + 3 + 2 * P;
-                LC vbit = lc_var(bit), m1 = lc_neg_var(V_ONE), vsib = lc_var(sib), ncur = lc_neg_var(cur), vleft = lc_var(left), vcur = lc_var(cur);
-                LC nleft = lc_neg_var(left);
-                b.cs.add(vbit, lc_sum({&vbit, &m1}), LC());
-                b.cs.add(vbit, lc_sum({&vsib, &ncur}), lc_sum({&vleft, &ncur}));
-                LC right = lc_sum({&vsib, &vcur, &nleft});
-                b.hash2(vleft, right, p1, p2, out);
-                cur = out;
-            }
+            const uint32_t cur = b.merkle_path(v + L.in_cm_out, v + L.lvl_base, L.lvl_size, depth);
             LC vroot = lc_var(V_ROOT), ncur = lc_neg_var(cur);
             b.cs.add(lc_sum({&vroot, &ncur}), lc_var(v + 2), LC());
         }
@@ -202,6 +203,27 @@ struct TransferBuilder {
         b.cs.add(lc_sum({&i0, &i1, &pa, &o0, &o1}), lc_var(V_ONE), LC());
         LC nh0 = lc_var(V_NH), nh1 = lc_neg_var(V_NH + 1);
         b.cs.add(lc_sum({&nh0, &nh1}), lc_var(V_NH_INV), lc_var(V_ONE));
+        return b.cs;
+    }
+};
+
+struct AssociationBuilder {
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        AssociationLayout L = AssociationLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = ASSOCIATION_N_PUB;
+        const uint32_t V_ONE = 0, V_ROOT = 1, V_NHASH = 2, V_RECIP = 3, V_AROOT = 4, V_NULL = 5, V_SECRET = 6, V_RSQ = 7, V_NH_PERM = 8;
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        LC nu = lc_var(V_NULL);
+        b.multi_hash({&nu}, lc_var(V_ONE), {V_NH_PERM}, V_NHASH);
+        b.hash2(lc_var(V_NULL), lc_var(V_SECRET), L.cm_base, L.cm_base + L.perm, L.cm_out);
+        const uint32_t bases[2] = {L.pool_base, L.assoc_base}, roots[2] = {V_ROOT, V_AROOT};
+        for (int t = 0; t < 2; t++) {
+            const uint32_t cur = b.merkle_path(L.cm_out, bases[t], L.lvl_size, depth);
+            LC vcur = lc_var(cur), nroot = lc_neg_var(roots[t]);
+            b.cs.add(lc_sum({&vcur, &nroot}), lc_var(V_ONE), LC());
+        }
         return b.cs;
     }
 };
