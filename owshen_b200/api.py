@@ -221,34 +221,39 @@ def _u32_array(xs):
     return xs if _blen(xs) is not None or isinstance(xs, int) else _bits_array(xs)
 
 
-def _transfer_args(fn, batch, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
-                   out_nullifiers, out_secrets, out_amounts):
-    """Length checks of a transfer batch's eleven input arrays -> their pointers in C ABI order."""
-    amounts = [_u64_array(in_amounts), _u64_array(out_amounts)]
-    bits = _u32_array(in_path_bits)
-    for name, buf, size in (("roots", roots, 32), ("tokens", tokens, 32), ("recipients", recipients, 32),
-                            ("in_nullifiers", in_nullifiers, 64), ("in_secrets", in_secrets, 64), ("in_amounts", amounts[0], 16),
-                            ("in_siblings", in_siblings, 64 * depth), ("in_path_bits", bits, 8),
-                            ("out_nullifiers", out_nullifiers, 64), ("out_secrets", out_secrets, 64), ("out_amounts", amounts[1], 16)):
-        if isinstance(buf, C.Array):        # converted from a sequence above
-            _need(C.sizeof(buf) == size * batch, f"{fn}: {name}: expected {size * batch // C.sizeof(buf._type_)} values, got {len(buf)}")
-        else:
-            _need_len(buf, size * batch, f"{fn}: {name}")
-    return [_ptr(x) for x in (roots, tokens, recipients, in_nullifiers, in_secrets, amounts[0], in_siblings, bits,
-                              out_nullifiers, out_secrets, amounts[1])]
+# The statements' boundary, mirroring the statement table of csrc/mimc.cuh: statement -> (takes a depth, input arrays in C ABI
+# order as (name, bytes per proof, bytes per proof and tree level, conversion of a sequence of ints)).  The C entry points are
+# og_<statement>_r1cs_info / _r1cs_export / _witness and og_groth16_prove_<statement>(_dev).
+_STATEMENTS = {
+    "withdraw": (True, (("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("recipients", 32, 0, None), ("siblings", 0, 32, None),
+                        ("path_bits", 4, 0, _u32_array))),
+    "deposit": (False, (("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("depositors", 32, 0, None))),
+    "transfer": (True, (("roots", 32, 0, None), ("tokens", 32, 0, None), ("recipients", 32, 0, None), ("in_nullifiers", 64, 0, None),
+                        ("in_secrets", 64, 0, None), ("in_amounts", 16, 0, _u64_array), ("in_siblings", 0, 64, None),
+                        ("in_path_bits", 8, 0, _u32_array), ("out_nullifiers", 64, 0, None), ("out_secrets", 64, 0, None),
+                        ("out_amounts", 16, 0, _u64_array))),
+    "association": (True, (("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("recipients", 32, 0, None), ("siblings", 0, 32, None),
+                           ("path_bits", 4, 0, _u32_array), ("assoc_siblings", 0, 32, None), ("assoc_path_bits", 4, 0, _u32_array))),
+}
 
 
-def _association_args(fn, batch, depth, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits):
-    """Length checks of an association batch's seven input arrays -> their pointers in C ABI order."""
-    bits, abits = _u32_array(path_bits), _u32_array(assoc_path_bits)
-    for name, buf, size in (("nullifiers", nullifiers, 32), ("secrets", secrets, 32), ("recipients", recipients, 32),
-                            ("siblings", siblings, 32 * depth), ("path_bits", bits, 4),
-                            ("assoc_siblings", assoc_siblings, 32 * depth), ("assoc_path_bits", abits, 4)):
-        if isinstance(buf, C.Array):        # converted from a sequence above
-            _need(C.sizeof(buf) == size * batch, f"{fn}: {name}: expected {batch} values, got {len(buf)}")
+def _depth_arg(stmt, depth):
+    """The depth argument of statement `stmt`'s C entry points: [depth], or [] for a statement of one fixed shape."""
+    return [depth] if _STATEMENTS[stmt][0] else []
+
+
+def _statement_args(stmt, fn, batch, depth, arrays):
+    """Length checks of a batch's input arrays (sequences of ints converted first) -> their pointers in C ABI order."""
+    out = []
+    for (name, per_proof, per_level, conv), buf in zip(_STATEMENTS[stmt][1], arrays):
+        buf = conv(buf) if conv else buf
+        size = (per_proof + per_level * depth) * batch
+        if isinstance(buf, C.Array):        # converted from a sequence
+            _need(C.sizeof(buf) == size, f"{fn}: {name}: expected {size // C.sizeof(buf._type_)} values, got {len(buf)}")
         else:
-            _need_len(buf, size * batch, f"{fn}: {name}")
-    return [_ptr(x) for x in (nullifiers, secrets, recipients, siblings, bits, assoc_siblings, abits)]
+            _need_len(buf, size, f"{fn}: {name}")
+        out.append(_ptr(buf))
+    return out
 
 
 def fr_bytes(x: int) -> bytes:
@@ -538,25 +543,24 @@ class Context:
         _check(lib().og_ntt(self._h, buf, log_n, batch, int(inverse), int(coset)), self)
         return buf.raw
 
-    def withdraw_witness(self, depth, nullifiers: bytes, secrets: bytes, recipients: bytes, siblings: bytes, path_bits) -> bytes:
-        _need(len(nullifiers) % 32 == 0 and 1 <= depth <= 32, "withdraw_witness: bad nullifiers length or depth")
-        n = len(nullifiers) // 32
-        _need(len(secrets) == 32 * n and len(recipients) == 32 * n and len(siblings) == 32 * n * depth and len(path_bits) == n,
-              "withdraw_witness: secrets / recipients / siblings / path_bits do not match the batch")
-        nv = r1cs_info(depth)["n_vars"]
-        out = C.create_string_buffer(32 * n * nv)
-        _check(lib().og_withdraw_witness(self._h, depth, nullifiers, secrets, recipients, siblings, _bits_array(path_bits), n, out), self)
+    def _statement_witness(self, stmt, depth, arrays) -> bytes:
+        """Full assignments of statement `stmt` at `depth`, n_vars * 32 bytes per proof; the batch is the first array's
+        32-byte elements."""
+        fn, first = f"{stmt}_witness", _STATEMENTS[stmt][1][0][0]
+        _need(not _STATEMENTS[stmt][0] or 1 <= depth <= 32, f"{fn}: depth must be 1..32")
+        _need(_blen(arrays[0]) is not None and _blen(arrays[0]) % 32 == 0, f"{fn}: {first} must be a multiple of 32 bytes")
+        n = _blen(arrays[0]) // 32
+        args = _statement_args(stmt, fn, n, depth, arrays)
+        out = C.create_string_buffer(32 * n * _statement_r1cs_info(stmt, depth)["n_vars"])
+        _check(getattr(lib(), f"og_{stmt}_witness")(self._h, *_depth_arg(stmt, depth), *args, n, out), self)
         return out.raw
+
+    def withdraw_witness(self, depth, nullifiers: bytes, secrets: bytes, recipients: bytes, siblings: bytes, path_bits) -> bytes:
+        return self._statement_witness("withdraw", depth, (nullifiers, secrets, recipients, siblings, path_bits))
 
     def deposit_witness(self, nullifiers: bytes, secrets: bytes, depositors: bytes) -> bytes:
         """Full assignments of the deposit statement, n_vars * 32 bytes per deposit, computed on the GPU."""
-        _need(len(nullifiers) % 32 == 0, "deposit_witness: nullifiers must be a multiple of 32 bytes")
-        n = len(nullifiers) // 32
-        _need(len(secrets) == 32 * n and len(depositors) == 32 * n, "deposit_witness: secrets / depositors do not match the batch")
-        nv = deposit_r1cs_info()["n_vars"]
-        out = C.create_string_buffer(32 * n * nv)
-        _check(lib().og_deposit_witness(self._h, nullifiers, secrets, depositors, n, out), self)
-        return out.raw
+        return self._statement_witness("deposit", 0, (nullifiers, secrets, depositors))
 
     def transfer_witness(self, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
                          out_nullifiers, out_secrets, out_amounts) -> bytes:
@@ -564,29 +568,15 @@ class Context:
         Per transfer: roots / tokens / recipients 32 bytes each; in_* / out_* note 0 then note 1 (nullifiers and secrets
         2 x 32 bytes, amounts 2 x uint64 as 8-byte little-endian buffers, uint64 arrays or ints); in_siblings 2 * depth
         elements (input 0's path, then input 1's); in_path_bits 2 words."""
-        _need(1 <= depth <= 32 and _blen(roots) is not None and _blen(roots) % 32 == 0,
-              "transfer_witness: depth must be 1..32 and roots a multiple of 32 bytes")
-        n = _blen(roots) // 32
-        args = _transfer_args("transfer_witness", n, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts,
-                              in_siblings, in_path_bits, out_nullifiers, out_secrets, out_amounts)
-        nv = transfer_r1cs_info(depth)["n_vars"]
-        out = C.create_string_buffer(32 * n * nv)
-        _check(lib().og_transfer_witness(self._h, depth, *args, n, out), self)
-        return out.raw
+        return self._statement_witness("transfer", depth, (roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
+                                                           in_path_bits, out_nullifiers, out_secrets, out_amounts))
 
     def association_witness(self, depth, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits) -> bytes:
         """Full assignments of the depth-`depth` association-set withdraw statement, n_vars * 32 bytes per proof, computed on
         the GPU.  Per proof: nullifier, secret, recipient 32 bytes each; siblings and assoc_siblings depth elements each (the
         pool path and the association path, leaf level first); path_bits and assoc_path_bits one word each."""
-        _need(1 <= depth <= 32 and _blen(nullifiers) is not None and _blen(nullifiers) % 32 == 0,
-              "association_witness: depth must be 1..32 and nullifiers a multiple of 32 bytes")
-        n = _blen(nullifiers) // 32
-        args = _association_args("association_witness", n, depth, nullifiers, secrets, recipients, siblings, path_bits,
-                                 assoc_siblings, assoc_path_bits)
-        nv = association_r1cs_info(depth)["n_vars"]
-        out = C.create_string_buffer(32 * n * nv)
-        _check(lib().og_association_witness(self._h, depth, *args, n, out), self)
-        return out.raw
+        return self._statement_witness("association", depth, (nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
+                                                              assoc_path_bits))
 
 
 def mimc7_constants():
@@ -596,80 +586,59 @@ def mimc7_constants():
     return [int.from_bytes(out.raw[32 * i:32 * i + 32], "little") for i in range(n.value)]
 
 
-def r1cs_info(depth: int) -> dict:
+def _statement_r1cs_info(stmt, depth) -> dict:
     v = [C.c_uint32() for _ in range(4)]
-    _check(lib().og_withdraw_r1cs_info(depth, *[C.byref(x) for x in v]))
+    _check(getattr(lib(), f"og_{stmt}_r1cs_info")(*_depth_arg(stmt, depth), *[C.byref(x) for x in v]))
     return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+
+
+def _statement_r1cs_export(stmt, depth, which):
+    w = "ABC".index(which)
+    export = getattr(lib(), f"og_{stmt}_r1cs_export")
+    nnz = C.c_uint64()
+    _check(export(*_depth_arg(stmt, depth), w, None, None, None, C.byref(nnz)))
+    nc = _statement_r1cs_info(stmt, depth)["n_constraints"]
+    ptr = (C.c_uint32 * (nc + 1))()
+    col = (C.c_uint32 * nnz.value)()
+    val = C.create_string_buffer(32 * nnz.value)
+    _check(export(*_depth_arg(stmt, depth), w, ptr, col, val, C.byref(nnz)))
+    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+
+
+def r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("withdraw", depth)
 
 
 def r1cs_export(depth: int, which: str):
     """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's withdraw R1CS."""
-    w = "ABC".index(which)
-    nnz = C.c_uint64()
-    _check(lib().og_withdraw_r1cs_export(depth, w, None, None, None, C.byref(nnz)))
-    nc = r1cs_info(depth)["n_constraints"]
-    ptr = (C.c_uint32 * (nc + 1))()
-    col = (C.c_uint32 * nnz.value)()
-    val = C.create_string_buffer(32 * nnz.value)
-    _check(lib().og_withdraw_r1cs_export(depth, w, ptr, col, val, C.byref(nnz)))
-    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+    return _statement_r1cs_export("withdraw", depth, which)
 
 
 def deposit_r1cs_info() -> dict:
-    v = [C.c_uint32() for _ in range(4)]
-    _check(lib().og_deposit_r1cs_info(*[C.byref(x) for x in v]))
-    return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+    return _statement_r1cs_info("deposit", 0)
 
 
 def deposit_r1cs_export(which: str):
     """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's deposit R1CS."""
-    w = "ABC".index(which)
-    nnz = C.c_uint64()
-    _check(lib().og_deposit_r1cs_export(w, None, None, None, C.byref(nnz)))
-    nc = deposit_r1cs_info()["n_constraints"]
-    ptr = (C.c_uint32 * (nc + 1))()
-    col = (C.c_uint32 * nnz.value)()
-    val = C.create_string_buffer(32 * nnz.value)
-    _check(lib().og_deposit_r1cs_export(w, ptr, col, val, C.byref(nnz)))
-    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+    return _statement_r1cs_export("deposit", 0, which)
 
 
 def transfer_r1cs_info(depth: int) -> dict:
-    v = [C.c_uint32() for _ in range(4)]
-    _check(lib().og_transfer_r1cs_info(depth, *[C.byref(x) for x in v]))
-    return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+    return _statement_r1cs_info("transfer", depth)
 
 
 def transfer_r1cs_export(depth: int, which: str):
     """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` transfer R1CS."""
-    w = "ABC".index(which)
-    nnz = C.c_uint64()
-    _check(lib().og_transfer_r1cs_export(depth, w, None, None, None, C.byref(nnz)))
-    nc = transfer_r1cs_info(depth)["n_constraints"]
-    ptr = (C.c_uint32 * (nc + 1))()
-    col = (C.c_uint32 * nnz.value)()
-    val = C.create_string_buffer(32 * nnz.value)
-    _check(lib().og_transfer_r1cs_export(depth, w, ptr, col, val, C.byref(nnz)))
-    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+    return _statement_r1cs_export("transfer", depth, which)
 
 
 def association_r1cs_info(depth: int) -> dict:
-    v = [C.c_uint32() for _ in range(4)]
-    _check(lib().og_association_r1cs_info(depth, *[C.byref(x) for x in v]))
-    return dict(n_constraints=v[0].value, n_vars=v[1].value, n_pub=v[2].value, log_m=v[3].value)
+    return _statement_r1cs_info("association", depth)
 
 
 def association_r1cs_export(depth: int, which: str):
     """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` association R1CS."""
-    w = "ABC".index(which)
-    nnz = C.c_uint64()
-    _check(lib().og_association_r1cs_export(depth, w, None, None, None, C.byref(nnz)))
-    nc = association_r1cs_info(depth)["n_constraints"]
-    ptr = (C.c_uint32 * (nc + 1))()
-    col = (C.c_uint32 * nnz.value)()
-    val = C.create_string_buffer(32 * nnz.value)
-    _check(lib().og_association_r1cs_export(depth, w, ptr, col, val, C.byref(nnz)))
-    return list(ptr), list(col), [int.from_bytes(val.raw[32 * i:32 * i + 32], "little") for i in range(nnz.value)]
+    return _statement_r1cs_export("association", depth, which)
 
 
 def _r1cs_args(A, B, C_):
@@ -705,26 +674,26 @@ def setup_r1cs(ctx: Context, n_vars: int, n_pub: int, A, B, C_, tau: int, alpha:
     return pk.raw[:pl.value], vk.raw[:vl.value]
 
 
+def _setup_statement(ctx, stmt, depth, toxic):
+    info = _statement_r1cs_info(stmt, depth)
+    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(_statement_r1cs_export(stmt, depth, m) for m in "ABC"), *toxic)
+
+
 def setup_deposit(ctx: Context, tau: int, alpha: int, beta: int, gamma: int, delta: int):
     """Development setup of the deposit statement -> (pk_bytes, vk_bytes): its exported R1CS through setup_r1cs."""
-    info = deposit_r1cs_info()
-    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(deposit_r1cs_export(m) for m in "ABC"), tau, alpha, beta, gamma, delta)
+    return _setup_statement(ctx, "deposit", 0, (tau, alpha, beta, gamma, delta))
 
 
 def setup_transfer(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
     """Development setup of the depth-`depth` transfer statement -> (pk_bytes, vk_bytes): its exported R1CS through
     setup_r1cs.  The key records depth 0; the prover recognises it as a transfer key by its shape."""
-    info = transfer_r1cs_info(depth)
-    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(transfer_r1cs_export(depth, m) for m in "ABC"),
-                      tau, alpha, beta, gamma, delta)
+    return _setup_statement(ctx, "transfer", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_association(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
     """Development setup of the depth-`depth` association-set withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS
     through setup_r1cs.  The key records depth 0; the prover recognises it as an association key by its shape."""
-    info = association_r1cs_info(depth)
-    return setup_r1cs(ctx, info["n_vars"], info["n_pub"], *(association_r1cs_export(depth, m) for m in "ABC"),
-                      tau, alpha, beta, gamma, delta)
+    return _setup_statement(ctx, "association", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -790,19 +759,21 @@ def ptau_prepare_withdraw(ctx: Context, acc: bytes, depth: int):
     return _sized(ctx, lambda *io: lib().og_ptau_prepare_withdraw(ctx._h, acc, len(acc), depth, *io), n_out=2)
 
 
+def _ptau_prepare_statement(ctx, acc, stmt, depth):
+    info = _statement_r1cs_info(stmt, depth)
+    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(_statement_r1cs_export(stmt, depth, m) for m in "ABC"))
+
+
 def ptau_prepare_deposit(ctx: Context, acc: bytes):
-    info = deposit_r1cs_info()
-    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(deposit_r1cs_export(m) for m in "ABC"))
+    return _ptau_prepare_statement(ctx, acc, "deposit", 0)
 
 
 def ptau_prepare_transfer(ctx: Context, acc: bytes, depth: int):
-    info = transfer_r1cs_info(depth)
-    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(transfer_r1cs_export(depth, m) for m in "ABC"))
+    return _ptau_prepare_statement(ctx, acc, "transfer", depth)
 
 
 def ptau_prepare_association(ctx: Context, acc: bytes, depth: int):
-    info = association_r1cs_info(depth)
-    return ptau_prepare(ctx, acc, info["n_vars"], info["n_pub"], *(association_r1cs_export(depth, m) for m in "ABC"))
+    return _ptau_prepare_statement(ctx, acc, "association", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -865,85 +836,68 @@ class ProvingKey:
         _check(lib().og_groth16_prove(self.ctx._h, self._h, witnesses, batch, rs, out), self.ctx)
         return out.raw
 
+    def _prove_statement(self, stmt, depth, arrays, rs, want_public, batch=None):
+        """Proofs of statement `stmt` at `depth` (None: the key is not the statement's); the batch is rs's 64-byte (r, s)
+        pairs unless given."""
+        fn = f"prove_{stmt}"
+        if depth is None:
+            raise OwshenB200Error(OG_E_INVALID, f"{fn}: this key was not made for the {stmt} statement")
+        if batch is None:
+            _need(_blen(rs) is not None and _blen(rs) % 64 == 0, f"{fn}: rs must be a buffer of 64 bytes (r, s) per proof")
+            batch = _blen(rs) // 64
+        args = _statement_args(stmt, fn, batch, depth, arrays)
+        _need_len(rs, 64 * batch, f"{fn}: rs")
+        proofs = C.create_string_buffer(PROOF_BYTES * batch)
+        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
+        _check(getattr(lib(), f"og_groth16_prove_{stmt}")(self.ctx._h, self._h, *args, batch, _ptr(rs), proofs, pub), self.ctx)
+        return proofs.raw, (pub.raw if want_public else None)
+
+    def _shape_depth(self, stmt):
+        """The depth d in 1..32 whose statement `stmt` has this key's shape (n_vars, n_pub), or None."""
+        for d in range(1, 33):
+            info = _statement_r1cs_info(stmt, d)
+            if (info["n_vars"], info["n_pub"]) == (self.n_vars, self.n_pub):
+                return d
+        return None
+
     def prove_withdraw(self, nullifiers, secrets, recipients, siblings, path_bits, rs, want_public=True):
         """Host buffers in, host buffers out (H2D / D2H inside).  Buffers may be bytes or pinned
         tensors / arrays exposing data_ptr() / .ctypes.  Returns (proofs, public_inputs)."""
-        batch = len(path_bits)
         _need(self.depth >= 1, "prove_withdraw: this key was not made for the withdraw statement")
-        for name, buf, size in (("nullifiers", nullifiers, 32), ("secrets", secrets, 32), ("recipients", recipients, 32),
-                                ("siblings", siblings, 32 * self.depth), ("rs", rs, 64)):
-            _need_len(buf, size * batch, f"prove_withdraw: {name}")
-        bits = path_bits if hasattr(path_bits, "data_ptr") or hasattr(path_bits, "ctypes") else _bits_array(path_bits)
-        proofs = C.create_string_buffer(PROOF_BYTES * batch)
-        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
-        _check(lib().og_groth16_prove_withdraw(self.ctx._h, self._h, _ptr(nullifiers), _ptr(secrets), _ptr(recipients),
-                                               _ptr(siblings), _ptr(bits), batch, _ptr(rs), proofs, pub), self.ctx)
-        return proofs.raw, (pub.raw if want_public else None)
+        return self._prove_statement("withdraw", self.depth, (nullifiers, secrets, recipients, siblings, path_bits), rs, want_public,
+                                     batch=len(path_bits))
 
     def prove_deposit(self, nullifiers, secrets, depositors, rs, want_public=True):
         """Batch of deposit proofs from the secret inputs (witness generation on the GPU).  Buffers as in prove_withdraw;
         returns (proofs, public_inputs) with public inputs (commitment, depositor) per proof."""
-        _need(_blen(rs) is not None and _blen(rs) % 64 == 0, "prove_deposit: rs must be a buffer of 64 bytes (r, s) per proof")
-        batch = _blen(rs) // 64
-        for name, buf in (("nullifiers", nullifiers), ("secrets", secrets), ("depositors", depositors)):
-            _need_len(buf, 32 * batch, f"prove_deposit: {name}")
-        proofs = C.create_string_buffer(PROOF_BYTES * batch)
-        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
-        _check(lib().og_groth16_prove_deposit(self.ctx._h, self._h, _ptr(nullifiers), _ptr(secrets), _ptr(depositors), batch,
-                                              _ptr(rs), proofs, pub), self.ctx)
-        return proofs.raw, (pub.raw if want_public else None)
+        return self._prove_statement("deposit", 0, (nullifiers, secrets, depositors), rs, want_public)
 
     @property
     def transfer_depth(self):
         """The depth d whose transfer statement has this key's shape (transfer_r1cs_info), or None."""
-        for d in range(1, 33):
-            info = transfer_r1cs_info(d)
-            if (info["n_vars"], info["n_pub"]) == (self.n_vars, self.n_pub):
-                return d
-        return None
+        return self._shape_depth("transfer")
 
     def prove_transfer(self, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
                        out_nullifiers, out_secrets, out_amounts, rs, want_public=True):
         """Batch of transfer proofs from the notes (witness generation on the GPU).  Inputs as in Context.transfer_witness;
         returns (proofs, public_inputs) with public inputs (root, public_amount, token, recipient, nullifier_hash[2],
         out_commitment[2]) per proof."""
-        depth = self.transfer_depth
-        if depth is None:
-            raise OwshenB200Error(OG_E_INVALID, "prove_transfer: this key was not made for a transfer statement")
-        _need(_blen(rs) is not None and _blen(rs) % 64 == 0, "prove_transfer: rs must be a buffer of 64 bytes (r, s) per proof")
-        batch = _blen(rs) // 64
-        args = _transfer_args("prove_transfer", batch, depth, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts,
-                              in_siblings, in_path_bits, out_nullifiers, out_secrets, out_amounts)
-        proofs = C.create_string_buffer(PROOF_BYTES * batch)
-        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
-        _check(lib().og_groth16_prove_transfer(self.ctx._h, self._h, *args, batch, _ptr(rs), proofs, pub), self.ctx)
-        return proofs.raw, (pub.raw if want_public else None)
+        return self._prove_statement("transfer", self.transfer_depth, (roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts,
+                                                                       in_siblings, in_path_bits, out_nullifiers, out_secrets,
+                                                                       out_amounts), rs, want_public)
 
     @property
     def association_depth(self):
         """The depth d whose association statement has this key's shape (association_r1cs_info), or None."""
-        for d in range(1, 33):
-            info = association_r1cs_info(d)
-            if (info["n_vars"], info["n_pub"]) == (self.n_vars, self.n_pub):
-                return d
-        return None
+        return self._shape_depth("association")
 
     def prove_association(self, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits, rs,
                           want_public=True):
         """Batch of association-set withdraw proofs from the secret inputs (witness generation on the GPU).  Inputs as in
         Context.association_witness; returns (proofs, public_inputs) with public inputs (root, nullifier_hash, recipient,
         association_root) per proof."""
-        depth = self.association_depth
-        if depth is None:
-            raise OwshenB200Error(OG_E_INVALID, "prove_association: this key was not made for an association statement")
-        _need(_blen(rs) is not None and _blen(rs) % 64 == 0, "prove_association: rs must be a buffer of 64 bytes (r, s) per proof")
-        batch = _blen(rs) // 64
-        args = _association_args("prove_association", batch, depth, nullifiers, secrets, recipients, siblings, path_bits,
-                                 assoc_siblings, assoc_path_bits)
-        proofs = C.create_string_buffer(PROOF_BYTES * batch)
-        pub = C.create_string_buffer(32 * self.n_pub * batch) if want_public else None
-        _check(lib().og_groth16_prove_association(self.ctx._h, self._h, *args, batch, _ptr(rs), proofs, pub), self.ctx)
-        return proofs.raw, (pub.raw if want_public else None)
+        return self._prove_statement("association", self.association_depth,
+                                     (nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits), rs, want_public)
 
     def prover_plan(self, batch: int) -> dict:
         """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and

@@ -859,19 +859,32 @@ int32_t og_ntt(og_ctx* ctx, uint8_t* data, uint32_t log_n, uint32_t batch, int32
     return check_flag(ctx);
 }
 
-// ---- withdraw statement ----------------------------------------------------------------------------------------
-int32_t og_withdraw_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
-    if (depth == 0 || depth > 32) return OG_E_INVALID;
-    WithdrawLayout L = WithdrawLayout::make(depth);
-    if (n_constraints) *n_constraints = L.n_constraints;
-    if (n_vars) *n_vars = L.n_vars;
-    if (n_pub) *n_pub = WITHDRAW_N_PUB;
-    if (log_m) *log_m = groth16_domain_log(L.n_constraints, WITHDRAW_N_PUB);
+// ---- the statements (the statement table, mimc.cuh) -----------------------------------------------------------------
+// Every og_<statement>_* entry point packs its input arrays, in C ABI order, into a StatementInputs and calls one of these.
+// Checks run in one order for every statement: ctx, null pointers, key on this device, key of this statement, batch 0.
+static bool depth_ok(Statement s, uint32_t depth) { return STATEMENTS[s].takes_depth ? depth >= 1 && depth <= 32 : depth == 0; }
+
+static bool any_null(Statement s, const StatementInputs& in) {
+    for (uint32_t k = 0; k < STATEMENTS[s].n_inputs; k++) if (!in.p[k]) return true;
+    return false;
+}
+
+static int32_t statement_r1cs_info(Statement s, uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub,
+                                   uint32_t* log_m) {
+    if (!depth_ok(s, depth)) return OG_E_INVALID;
+    const StatementShape sh = STATEMENTS[s].shape(depth);
+    const uint32_t np = STATEMENTS[s].n_pub;
+    if (n_constraints) *n_constraints = sh.n_constraints;
+    if (n_vars) *n_vars = sh.n_vars;
+    if (n_pub) *n_pub = np;
+    if (log_m) *log_m = groth16_domain_log(sh.n_constraints, np);
     return OG_OK;
 }
-int32_t og_withdraw_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
-    if (depth == 0 || depth > 32 || which < 0 || which > 2 || !nnz) return OG_E_INVALID;
-    R1cs cs = WithdrawBuilder::build(depth);
+
+static int32_t statement_r1cs_export(Statement s, uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                     uint64_t* nnz) {
+    if (!depth_ok(s, depth) || which < 0 || which > 2 || !nnz) return OG_E_INVALID;
+    R1cs cs = statement_r1cs(s, depth);
     const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
     *nnz = M.col.size();
     if (!row_ptr || !col_idx || !coeffs) return OG_OK;
@@ -880,181 +893,117 @@ int32_t og_withdraw_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr
     for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
     return OG_OK;
 }
+
+// the host input arrays of a batch, copied into one device slot (each array 256-byte aligned)
+static int32_t stage_statement_inputs(og_ctx* ctx, Statement s, uint32_t depth, uint32_t batch, const StatementInputs& h,
+                                      StatementInputs& d) {
+    const StatementDesc& S = STATEMENTS[s];
+    uint64_t off[STATEMENT_MAX_INPUTS], tot = 0;
+    for (uint32_t k = 0; k < S.n_inputs; k++) { off[k] = tot; tot += (S.input_bytes(k, depth) * batch + 255) & ~255ull; }
+    OG_SLOT(ctx, base, uint8_t, S_IO_STATEMENT, tot);
+    for (uint32_t k = 0; k < S.n_inputs; k++) {
+        H2D(ctx, base + off[k], h.p[k], S.input_bytes(k, depth) * batch);
+        d.p[k] = base + off[k];
+    }
+    return OG_OK;
+}
+
+static int32_t statement_witness(og_ctx* ctx, Statement s, uint32_t depth, const StatementInputs& in, uint32_t batch, uint8_t* witnesses) {
+    OG_ENTER(ctx);
+    if (!depth_ok(s, depth) || any_null(s, in) || !witnesses) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    const uint64_t out_bytes = 32ull * batch * STATEMENTS[s].shape(depth).n_vars;
+    StatementInputs d;
+    OG_TRY(stage_statement_inputs(ctx, s, depth, batch, in, d));
+    OG_SLOT(ctx, dout, uint8_t, S_IO_F, out_bytes);
+    OG_TRY(clear_flag(ctx));
+    OG_TRY(statement_witness_bytes_dev(ctx, s, depth, d, batch, dout));
+    D2H(ctx, witnesses, dout, out_bytes);
+    return check_flag(ctx);
+}
+
+static int32_t statement_prove(og_ctx* ctx, const og_pk* pk, Statement s, const StatementInputs& in, uint32_t batch, const uint8_t* rs,
+                               uint8_t* proofs, uint8_t* public_out) {
+    OG_ENTER(ctx);
+    if (!pk || any_null(s, in) || !rs || !proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    const int32_t depth = statement_key_depth(pk, s);
+    if (depth < 0) return OG_E_INVALID;
+    if (batch == 0) return OG_OK;
+    uint32_t n_pub; pk_info(pk, nullptr, &n_pub, nullptr, nullptr);
+    StatementInputs d;
+    OG_TRY(stage_statement_inputs(ctx, s, (uint32_t)depth, batch, in, d));
+    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
+    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
+    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * n_pub);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, drs, rs, 64ull * batch);
+    OG_TRY(prove_statement_dev(ctx, pk, s, d, batch, drs, dpr, public_out ? dpub : nullptr));
+    D2H(ctx, proofs, dpr, 256ull * batch);
+    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * n_pub);
+    return check_flag(ctx);
+}
+
+static int32_t statement_prove_dev(og_ctx* ctx, const og_pk* pk, Statement s, const StatementInputs& d_in, uint32_t batch,
+                                   const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    OG_ENTER(ctx);
+    if (!pk || any_null(s, d_in) || !d_rs || !d_proofs) return OG_E_INVALID;
+    OG_PK_CHECK(ctx, pk);
+    return prove_statement_dev(ctx, pk, s, d_in, batch, d_rs, d_proofs, d_public_out);
+}
+
+// ---- withdraw statement ----------------------------------------------------------------------------------------
+int32_t og_withdraw_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_WITHDRAW, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_withdraw_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    return statement_r1cs_export(ST_WITHDRAW, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
 int32_t og_withdraw_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* recipients,
                             const uint8_t* siblings, const uint32_t* path_bits, uint32_t batch, uint8_t* witnesses) {
-    OG_ENTER(ctx);
-    if (!ctx || depth == 0 || depth > 32 || !nullifiers || !secrets || !recipients || !siblings || !path_bits || !witnesses) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    WithdrawLayout L = WithdrawLayout::make(depth);
-    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32ull * batch);
-    OG_SLOT(ctx, dsx, uint8_t, S_IO_B, 32ull * batch);
-    OG_SLOT(ctx, dr, uint8_t, S_IO_C, 32ull * batch);
-    OG_SLOT(ctx, dsib, uint8_t, S_IO_D, 32ull * batch * depth);
-    OG_SLOT(ctx, dbits, uint32_t, S_IO_E, 4ull * batch);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dn, nullifiers, 32ull * batch); H2D(ctx, dsx, secrets, 32ull * batch); H2D(ctx, dr, recipients, 32ull * batch);
-    H2D(ctx, dsib, siblings, 32ull * batch * depth); H2D(ctx, dbits, path_bits, 4ull * batch);
-    OG_TRY(withdraw_witness_bytes_dev(ctx, depth, dn, dsx, dr, dsib, dbits, batch, dout));
-    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
-    return check_flag(ctx);
+    return statement_witness(ctx, ST_WITHDRAW, depth, {nullifiers, secrets, recipients, siblings, path_bits}, batch, witnesses);
 }
 
 // ---- deposit statement ----------------------------------------------------------------------------------------
 int32_t og_deposit_r1cs_info(uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
-    DepositLayout L = DepositLayout::make();
-    if (n_constraints) *n_constraints = L.n_constraints;
-    if (n_vars) *n_vars = L.n_vars;
-    if (n_pub) *n_pub = DEPOSIT_N_PUB;
-    if (log_m) *log_m = groth16_domain_log(L.n_constraints, DEPOSIT_N_PUB);
-    return OG_OK;
+    return statement_r1cs_info(ST_DEPOSIT, 0, n_constraints, n_vars, n_pub, log_m);
 }
 int32_t og_deposit_r1cs_export(int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
-    if (which < 0 || which > 2 || !nnz) return OG_E_INVALID;
-    R1cs cs = DepositBuilder::build();
-    const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
-    *nnz = M.col.size();
-    if (!row_ptr || !col_idx || !coeffs) return OG_OK;
-    memcpy(row_ptr, M.row_ptr.data(), 4 * M.row_ptr.size());
-    memcpy(col_idx, M.col.data(), 4 * M.col.size());
-    for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
-    return OG_OK;
+    return statement_r1cs_export(ST_DEPOSIT, 0, which, row_ptr, col_idx, coeffs, nnz);
 }
 int32_t og_deposit_witness(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* depositors, uint32_t batch,
                            uint8_t* witnesses) {
-    OG_ENTER(ctx);
-    if (!ctx || !nullifiers || !secrets || !depositors || !witnesses) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    DepositLayout L = DepositLayout::make();
-    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32ull * batch);
-    OG_SLOT(ctx, dsx, uint8_t, S_IO_B, 32ull * batch);
-    OG_SLOT(ctx, dd, uint8_t, S_IO_C, 32ull * batch);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dn, nullifiers, 32ull * batch); H2D(ctx, dsx, secrets, 32ull * batch); H2D(ctx, dd, depositors, 32ull * batch);
-    OG_TRY(deposit_witness_bytes_dev(ctx, dn, dsx, dd, batch, dout));
-    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
-    return check_flag(ctx);
+    return statement_witness(ctx, ST_DEPOSIT, 0, {nullifiers, secrets, depositors}, batch, witnesses);
 }
 
 // ---- transfer statement ---------------------------------------------------------------------------------------
 int32_t og_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
-    if (depth == 0 || depth > 32) return OG_E_INVALID;
-    TransferLayout L = TransferLayout::make(depth);
-    if (n_constraints) *n_constraints = L.n_constraints;
-    if (n_vars) *n_vars = L.n_vars;
-    if (n_pub) *n_pub = TRANSFER_N_PUB;
-    if (log_m) *log_m = groth16_domain_log(L.n_constraints, TRANSFER_N_PUB);
-    return OG_OK;
+    return statement_r1cs_info(ST_TRANSFER, depth, n_constraints, n_vars, n_pub, log_m);
 }
 int32_t og_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
-    if (depth == 0 || depth > 32 || which < 0 || which > 2 || !nnz) return OG_E_INVALID;
-    R1cs cs = TransferBuilder::build(depth);
-    const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
-    *nnz = M.col.size();
-    if (!row_ptr || !col_idx || !coeffs) return OG_OK;
-    memcpy(row_ptr, M.row_ptr.data(), 4 * M.row_ptr.size());
-    memcpy(col_idx, M.col.data(), 4 * M.col.size());
-    for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
-    return OG_OK;
+    return statement_r1cs_export(ST_TRANSFER, depth, which, row_ptr, col_idx, coeffs, nnz);
 }
-
-// the eleven host input arrays of a transfer batch, copied into one device slot (each array 256-byte aligned)
-static int32_t stage_transfer_inputs(og_ctx* ctx, uint32_t depth, uint32_t batch, const uint8_t* roots, const uint8_t* tokens,
-                                     const uint8_t* recipients, const uint8_t* in_nullifiers, const uint8_t* in_secrets,
-                                     const uint64_t* in_amounts, const uint8_t* in_siblings, const uint32_t* in_path_bits,
-                                     const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
-                                     TransferInputs& d) {
-    const uint64_t b = batch;
-    const void* src[11] = {roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits,
-                           out_nullifiers, out_secrets, out_amounts};
-    const uint64_t bytes[11] = {32 * b, 32 * b, 32 * b, 64 * b, 64 * b, 16 * b, 64ull * depth * b, 8 * b, 64 * b, 64 * b, 16 * b};
-    uint64_t off[11], tot = 0;
-    for (int k = 0; k < 11; k++) { off[k] = tot; tot += (bytes[k] + 255) & ~255ull; }
-    OG_SLOT(ctx, base, uint8_t, S_IO_TRANSFER, tot);
-    for (int k = 0; k < 11; k++) H2D(ctx, base + off[k], src[k], bytes[k]);
-    d.roots = base + off[0]; d.tokens = base + off[1]; d.recipients = base + off[2];
-    d.in_null = base + off[3]; d.in_sec = base + off[4]; d.in_amounts = (const uint64_t*)(base + off[5]);
-    d.in_sib = base + off[6]; d.in_bits = (const uint32_t*)(base + off[7]);
-    d.out_null = base + off[8]; d.out_sec = base + off[9]; d.out_amounts = (const uint64_t*)(base + off[10]);
-    return OG_OK;
-}
-
 int32_t og_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
                             const uint8_t* in_nullifiers, const uint8_t* in_secrets, const uint64_t* in_amounts,
                             const uint8_t* in_siblings, const uint32_t* in_path_bits,
                             const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
                             uint32_t batch, uint8_t* witnesses) {
-    OG_ENTER(ctx);
-    if (depth == 0 || depth > 32 || !roots || !tokens || !recipients || !in_nullifiers || !in_secrets || !in_amounts || !in_siblings ||
-        !in_path_bits || !out_nullifiers || !out_secrets || !out_amounts || !witnesses) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    TransferLayout L = TransferLayout::make(depth);
-    TransferInputs d;
-    OG_TRY(stage_transfer_inputs(ctx, depth, batch, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
-                                 in_path_bits, out_nullifiers, out_secrets, out_amounts, d));
-    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
-    OG_TRY(clear_flag(ctx));
-    OG_TRY(transfer_witness_bytes_dev(ctx, depth, d, batch, dout));
-    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
-    return check_flag(ctx);
+    return statement_witness(ctx, ST_TRANSFER, depth, {roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
+                                                       in_path_bits, out_nullifiers, out_secrets, out_amounts}, batch, witnesses);
 }
 
 // ---- association-set withdraw statement ---------------------------------------------------------------------------
 int32_t og_association_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
-    if (depth == 0 || depth > 32) return OG_E_INVALID;
-    AssociationLayout L = AssociationLayout::make(depth);
-    if (n_constraints) *n_constraints = L.n_constraints;
-    if (n_vars) *n_vars = L.n_vars;
-    if (n_pub) *n_pub = ASSOCIATION_N_PUB;
-    if (log_m) *log_m = groth16_domain_log(L.n_constraints, ASSOCIATION_N_PUB);
-    return OG_OK;
+    return statement_r1cs_info(ST_ASSOCIATION, depth, n_constraints, n_vars, n_pub, log_m);
 }
 int32_t og_association_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
-    if (depth == 0 || depth > 32 || which < 0 || which > 2 || !nnz) return OG_E_INVALID;
-    R1cs cs = AssociationBuilder::build(depth);
-    const Csr& M = which == 0 ? cs.A : (which == 1 ? cs.B : cs.C);
-    *nnz = M.col.size();
-    if (!row_ptr || !col_idx || !coeffs) return OG_OK;
-    memcpy(row_ptr, M.row_ptr.data(), 4 * M.row_ptr.size());
-    memcpy(col_idx, M.col.data(), 4 * M.col.size());
-    for (size_t i = 0; i < M.val.size(); i++) host_store(coeffs + 32 * i, M.val[i]);
-    return OG_OK;
+    return statement_r1cs_export(ST_ASSOCIATION, depth, which, row_ptr, col_idx, coeffs, nnz);
 }
-
-// the seven host input arrays of an association batch, copied into one device slot (each array 256-byte aligned)
-static int32_t stage_association_inputs(og_ctx* ctx, uint32_t depth, uint32_t batch, const uint8_t* nullifiers, const uint8_t* secrets,
-                                        const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
-                                        const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, AssociationInputs& d) {
-    const uint64_t b = batch;
-    const void* src[7] = {nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits};
-    const uint64_t bytes[7] = {32 * b, 32 * b, 32 * b, 32ull * depth * b, 4 * b, 32ull * depth * b, 4 * b};
-    uint64_t off[7], tot = 0;
-    for (int k = 0; k < 7; k++) { off[k] = tot; tot += (bytes[k] + 255) & ~255ull; }
-    OG_SLOT(ctx, base, uint8_t, S_IO_ASSOCIATION, tot);
-    for (int k = 0; k < 7; k++) H2D(ctx, base + off[k], src[k], bytes[k]);
-    d.nullifiers = base + off[0]; d.secrets = base + off[1]; d.recipients = base + off[2];
-    d.siblings = base + off[3]; d.path_bits = (const uint32_t*)(base + off[4]);
-    d.assoc_siblings = base + off[5]; d.assoc_path_bits = (const uint32_t*)(base + off[6]);
-    return OG_OK;
-}
-
 int32_t og_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* recipients,
                                const uint8_t* siblings, const uint32_t* path_bits, const uint8_t* assoc_siblings,
                                const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses) {
-    OG_ENTER(ctx);
-    if (!ctx || depth == 0 || depth > 32 || !nullifiers || !secrets || !recipients || !siblings || !path_bits || !assoc_siblings ||
-        !assoc_path_bits || !witnesses) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    AssociationLayout L = AssociationLayout::make(depth);
-    AssociationInputs d;
-    OG_TRY(stage_association_inputs(ctx, depth, batch, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
-                                    assoc_path_bits, d));
-    OG_SLOT(ctx, dout, uint8_t, S_IO_F, 32ull * batch * L.n_vars);
-    OG_TRY(clear_flag(ctx));
-    OG_TRY(association_witness_bytes_dev(ctx, depth, d, batch, dout));
-    D2H(ctx, witnesses, dout, 32ull * batch * L.n_vars);
-    return check_flag(ctx);
+    return statement_witness(ctx, ST_ASSOCIATION, depth, {nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
+                                                          assoc_path_bits}, batch, witnesses);
 }
 
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
@@ -1118,67 +1067,25 @@ int32_t og_groth16_prove(og_ctx* ctx, const og_pk* pk, const uint8_t* witnesses,
 int32_t og_groth16_prove_withdraw_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
                                       const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits, uint32_t batch,
                                       const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
-    OG_ENTER(ctx);
-    if (!ctx || !pk || !d_nullifiers || !d_secrets || !d_recipients || !d_siblings || !d_path_bits || !d_rs || !d_proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    return prove_withdraw_dev(ctx, pk, d_nullifiers, d_secrets, d_recipients, d_siblings, d_path_bits, batch, d_rs, d_proofs, d_public_out);
+    return statement_prove_dev(ctx, pk, ST_WITHDRAW, {d_nullifiers, d_secrets, d_recipients, d_siblings, d_path_bits}, batch, d_rs,
+                               d_proofs, d_public_out);
 }
 
 int32_t og_groth16_prove_withdraw(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* recipients,
                                   const uint8_t* siblings, const uint32_t* path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
                                   uint8_t* public_out) {
-    OG_ENTER(ctx);
-    if (!ctx || !pk || !nullifiers || !secrets || !recipients || !siblings || !path_bits || !rs || !proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    if (batch == 0) return OG_OK;
-    uint32_t depth, n_pub; pk_info(pk, nullptr, &n_pub, nullptr, &depth);
-    if (depth == 0) return OG_E_INVALID;
-    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32ull * batch);
-    OG_SLOT(ctx, dsx, uint8_t, S_IO_B, 32ull * batch);
-    OG_SLOT(ctx, dr, uint8_t, S_IO_C, 32ull * batch);
-    OG_SLOT(ctx, dsib, uint8_t, S_IO_D, 32ull * batch * depth);
-    OG_SLOT(ctx, dbits, uint32_t, S_IO_E, 4ull * batch);
-    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
-    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
-    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * n_pub);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dn, nullifiers, 32ull * batch); H2D(ctx, dsx, secrets, 32ull * batch); H2D(ctx, dr, recipients, 32ull * batch);
-    H2D(ctx, dsib, siblings, 32ull * batch * depth); H2D(ctx, dbits, path_bits, 4ull * batch); H2D(ctx, drs, rs, 64ull * batch);
-    OG_TRY(prove_withdraw_dev(ctx, pk, dn, dsx, dr, dsib, dbits, batch, drs, dpr, public_out ? dpub : nullptr));
-    D2H(ctx, proofs, dpr, 256ull * batch);
-    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * n_pub);
-    return check_flag(ctx);
+    return statement_prove(ctx, pk, ST_WITHDRAW, {nullifiers, secrets, recipients, siblings, path_bits}, batch, rs, proofs, public_out);
 }
 
 int32_t og_groth16_prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
                                      const uint8_t* d_depositors, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
                                      uint8_t* d_public_out) {
-    OG_ENTER(ctx);
-    if (!ctx || !pk || !d_nullifiers || !d_secrets || !d_depositors || !d_rs || !d_proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    return prove_deposit_dev(ctx, pk, d_nullifiers, d_secrets, d_depositors, batch, d_rs, d_proofs, d_public_out);
+    return statement_prove_dev(ctx, pk, ST_DEPOSIT, {d_nullifiers, d_secrets, d_depositors}, batch, d_rs, d_proofs, d_public_out);
 }
 
 int32_t og_groth16_prove_deposit(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* depositors,
                                  uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
-    OG_ENTER(ctx);
-    if (!ctx || !pk || !nullifiers || !secrets || !depositors || !rs || !proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    if (!pk_is_deposit(pk)) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32ull * batch);
-    OG_SLOT(ctx, dsx, uint8_t, S_IO_B, 32ull * batch);
-    OG_SLOT(ctx, dd, uint8_t, S_IO_C, 32ull * batch);
-    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
-    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
-    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * DEPOSIT_N_PUB);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dn, nullifiers, 32ull * batch); H2D(ctx, dsx, secrets, 32ull * batch); H2D(ctx, dd, depositors, 32ull * batch);
-    H2D(ctx, drs, rs, 64ull * batch);
-    OG_TRY(prove_deposit_dev(ctx, pk, dn, dsx, dd, batch, drs, dpr, public_out ? dpub : nullptr));
-    D2H(ctx, proofs, dpr, 256ull * batch);
-    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * DEPOSIT_N_PUB);
-    return check_flag(ctx);
+    return statement_prove(ctx, pk, ST_DEPOSIT, {nullifiers, secrets, depositors}, batch, rs, proofs, public_out);
 }
 
 int32_t og_groth16_prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
@@ -1186,13 +1093,9 @@ int32_t og_groth16_prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_
                                       const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
                                       const uint8_t* d_out_nullifiers, const uint8_t* d_out_secrets, const uint64_t* d_out_amounts,
                                       uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
-    OG_ENTER(ctx);
-    if (!pk || !d_roots || !d_tokens || !d_recipients || !d_in_nullifiers || !d_in_secrets || !d_in_amounts || !d_in_siblings ||
-        !d_in_path_bits || !d_out_nullifiers || !d_out_secrets || !d_out_amounts || !d_rs || !d_proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    TransferInputs d{d_roots, d_tokens, d_recipients, d_in_nullifiers, d_in_secrets, d_in_amounts, d_in_siblings, d_in_path_bits,
-                     d_out_nullifiers, d_out_secrets, d_out_amounts};
-    return prove_transfer_dev(ctx, pk, d, batch, d_rs, d_proofs, d_public_out);
+    return statement_prove_dev(ctx, pk, ST_TRANSFER, {d_roots, d_tokens, d_recipients, d_in_nullifiers, d_in_secrets, d_in_amounts,
+                                                      d_in_siblings, d_in_path_bits, d_out_nullifiers, d_out_secrets, d_out_amounts},
+                               batch, d_rs, d_proofs, d_public_out);
 }
 
 int32_t og_groth16_prove_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
@@ -1200,62 +1103,24 @@ int32_t og_groth16_prove_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* r
                                   const uint8_t* in_siblings, const uint32_t* in_path_bits,
                                   const uint8_t* out_nullifiers, const uint8_t* out_secrets, const uint64_t* out_amounts,
                                   uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
-    OG_ENTER(ctx);
-    if (!pk || !roots || !tokens || !recipients || !in_nullifiers || !in_secrets || !in_amounts || !in_siblings || !in_path_bits ||
-        !out_nullifiers || !out_secrets || !out_amounts || !rs || !proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    const uint32_t depth = pk_transfer_depth(pk);
-    if (depth == 0) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    TransferInputs d;
-    OG_TRY(stage_transfer_inputs(ctx, depth, batch, roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
-                                 in_path_bits, out_nullifiers, out_secrets, out_amounts, d));
-    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
-    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
-    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * TRANSFER_N_PUB);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, drs, rs, 64ull * batch);
-    OG_TRY(prove_transfer_dev(ctx, pk, d, batch, drs, dpr, public_out ? dpub : nullptr));
-    D2H(ctx, proofs, dpr, 256ull * batch);
-    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * TRANSFER_N_PUB);
-    return check_flag(ctx);
+    return statement_prove(ctx, pk, ST_TRANSFER, {roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings,
+                                                  in_path_bits, out_nullifiers, out_secrets, out_amounts}, batch, rs, proofs, public_out);
 }
 
 int32_t og_groth16_prove_association_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
                                          const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits,
                                          const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
                                          const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
-    OG_ENTER(ctx);
-    if (!ctx || !pk || !d_nullifiers || !d_secrets || !d_recipients || !d_siblings || !d_path_bits || !d_assoc_siblings ||
-        !d_assoc_path_bits || !d_rs || !d_proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    AssociationInputs d{d_nullifiers, d_secrets, d_recipients, d_siblings, d_path_bits, d_assoc_siblings, d_assoc_path_bits};
-    return prove_association_dev(ctx, pk, d, batch, d_rs, d_proofs, d_public_out);
+    return statement_prove_dev(ctx, pk, ST_ASSOCIATION, {d_nullifiers, d_secrets, d_recipients, d_siblings, d_path_bits, d_assoc_siblings,
+                                                         d_assoc_path_bits}, batch, d_rs, d_proofs, d_public_out);
 }
 
 int32_t og_groth16_prove_association(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets,
                                      const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
                                      const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch, const uint8_t* rs,
                                      uint8_t* proofs, uint8_t* public_out) {
-    OG_ENTER(ctx);
-    if (!ctx || !pk || !nullifiers || !secrets || !recipients || !siblings || !path_bits || !assoc_siblings || !assoc_path_bits || !rs ||
-        !proofs) return OG_E_INVALID;
-    OG_PK_CHECK(ctx, pk);
-    const uint32_t depth = pk_association_depth(pk);
-    if (depth == 0) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    AssociationInputs d;
-    OG_TRY(stage_association_inputs(ctx, depth, batch, nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
-                                    assoc_path_bits, d));
-    OG_SLOT(ctx, drs, uint8_t, S_IO_F, 64ull * batch);
-    OG_SLOT(ctx, dpr, uint8_t, S_IO_G, 256ull * batch);
-    OG_SLOT(ctx, dpub, uint8_t, S_IO_H, 32ull * batch * ASSOCIATION_N_PUB);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, drs, rs, 64ull * batch);
-    OG_TRY(prove_association_dev(ctx, pk, d, batch, drs, dpr, public_out ? dpub : nullptr));
-    D2H(ctx, proofs, dpr, 256ull * batch);
-    if (public_out) D2H(ctx, public_out, dpub, 32ull * batch * ASSOCIATION_N_PUB);
-    return check_flag(ctx);
+    return statement_prove(ctx, pk, ST_ASSOCIATION, {nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits},
+                           batch, rs, proofs, public_out);
 }
 
 int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {

@@ -2,9 +2,11 @@
 // development setup.  The reference has no prover (SURVEY.md section 0); conventions are frozen in
 // DESIGN.md section 4 and checked bit-for-bit against oracle/groth16.py and oracle/cpu.
 //
-// Once per batch:  witness  k_withdraw_witness / k_deposit_witness / k_transfer_witness / k_association_witness (mimc.cu): every MiMC7 round value
-//                  -> W[batch][n_vars+2] (or full witnesses from the caller)
+// Once per batch:  statement_key_depth accepts the key as the statement's (shapes from the statement table, mimc.cuh) and
+//                  finds the depth it proves at, before any other work and whatever the batch size
 // Per chunk of B proofs (default min(1024, the lane budget / one proof's scratch); everything stays in HBM, nothing returns to the host until the proofs):
+//   witness      statement_witness_dev (mimc.cu): the statement's kernel writes every MiMC7 round value into W[B][n_vars+2]
+//                (or k_witness_in reads the caller's full witnesses)
 //   a, b, c      k_abc: sparse A.w, B.w over the CSR kept in L2, c = a*b
 //   h            3 iNTT + 3 coset NTT (ntt.cu), k_pointwise: d = a'b' - c' written straight into
 //                the scalar vector of the C multi-scalar multiplication
@@ -481,19 +483,13 @@ static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
     return msm_buckets_g2(ctx, table, b.sorted, b.offsets, b.counts, B, pk->nb[which], (uint64_t)B * n_pts * pk->n_windows[which], b.bk2, b.lvl2, b.heavy, b.cursor, totals, b.aff2);
 }
 
-// where a chunk's witness rows come from
+// where a chunk's witness rows come from: the statement's witness kernel on its inputs, or the caller's full witnesses
 struct WitnessSource {
-    enum Kind { WITHDRAW, DEPOSIT, TRANSFER, ASSOCIATION, FULL } kind = FULL;
-    const uint8_t *d_null = nullptr, *d_sec = nullptr;                       // secret inputs (prove_withdraw, prove_deposit)
-    const uint8_t *d_rec = nullptr, *d_sib = nullptr;                        // withdraw: recipients, siblings
-    const uint32_t* d_bits = nullptr;
-    const uint8_t* d_dep = nullptr;                                          // deposit: depositors
-    TransferInputs tin = {};                                                 // transfer: every input array
-    uint32_t transfer_depth = 0;
-    AssociationInputs ain = {};                                              // association: every input array
-    uint32_t association_depth = 0;
-    const uint8_t* d_wit = nullptr;                                          // or full witnesses (prove)
-    uint8_t* d_public = nullptr;
+    const uint8_t* d_wit = nullptr;      // full witnesses (prove); nullptr = the statement's inputs below
+    Statement stmt = ST_WITHDRAW;
+    uint32_t depth = 0;
+    StatementInputs in;
+    uint8_t* d_public = nullptr;         // statement proofs: the public inputs out, or nullptr
 };
 
 // proofs [off, off+B) on the current stream: witness rows -> per-proof MSM totals -> proof bytes
@@ -502,23 +498,11 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
     const uint32_t m = 1u << pk->log_m, n_priv = pk->n_vars - pk->n_pub - 1;
     Fr* W = b.W + (size_t)off * b.w_stride;
     Fr* rs_m = b.rs_m + 2 * (size_t)off;
-    if (src.kind == WitnessSource::FULL) {
+    if (src.d_wit) {
         uint64_t tot = (uint64_t)B * pk->n_vars;
         OG_LAUNCH(ctx, k_witness_in, (unsigned)((tot + 127) / 128), 128, 0, src.d_wit + 32ull * off * pk->n_vars, B, pk->n_vars, b.w_stride, W, ctx->d_flag);
     } else {
-        if (src.kind == WitnessSource::WITHDRAW) {
-            WithdrawLayout L = WithdrawLayout::make(pk->depth);
-            OG_TRY(withdraw_witness_strided_dev(ctx, L, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_rec + 32ull * off,
-                                                src.d_sib + 32ull * off * pk->depth, src.d_bits + off, B, W));
-        } else if (src.kind == WitnessSource::DEPOSIT) {
-            OG_TRY(deposit_witness_strided_dev(ctx, b.w_stride, src.d_null + 32ull * off, src.d_sec + 32ull * off, src.d_dep + 32ull * off, B, W));
-        } else if (src.kind == WitnessSource::TRANSFER) {
-            TransferLayout L = TransferLayout::make(src.transfer_depth);
-            OG_TRY(transfer_witness_strided_dev(ctx, L, b.w_stride, src.tin.at(off, src.transfer_depth), B, W));
-        } else {
-            AssociationLayout L = AssociationLayout::make(src.association_depth);
-            OG_TRY(association_witness_strided_dev(ctx, L, b.w_stride, src.ain.at(off, src.association_depth), B, W));
-        }
+        OG_TRY(statement_witness_dev(ctx, src.stmt, src.depth, b.w_stride, src.in.at(src.stmt, src.depth, off), B, W));
         if (src.d_public) OG_LAUNCH(ctx, k_public_out, (B * pk->n_pub + 127) / 128, 128, 0, W, b.w_stride, B, pk->n_pub, src.d_public + 32ull * off * pk->n_pub);
     }
     OG_LAUNCH(ctx, k_extras, (B + 127) / 128, 128, 0, d_rs + 64ull * off, B, pk->n_vars, b.w_stride, W, rs_m, ctx->d_flag);
@@ -604,78 +588,31 @@ static int32_t prove_batch(og_ctx* ctx, const og_pk* pk, const WitnessSource& sr
     return rc;
 }
 
-int32_t prove_withdraw_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_rec,
-                           const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
-                           uint8_t* d_public) {
-    if (pk->depth == 0) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    WithdrawLayout L = WithdrawLayout::make(pk->depth);
-    if (L.n_vars != pk->n_vars) return OG_E_INVALID;
-    WitnessSource src;
-    src.kind = WitnessSource::WITHDRAW;
-    src.d_null = d_null; src.d_sec = d_sec; src.d_rec = d_rec; src.d_sib = d_sib; src.d_bits = d_bits; src.d_public = d_public;
-    return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
-}
-
-bool pk_is_deposit(const og_pk* pk) {
-    DepositLayout L = DepositLayout::make();
-    return pk->n_vars == L.n_vars && pk->n_pub == DEPOSIT_N_PUB && pk->n_constraints == L.n_constraints;
-}
-
-int32_t prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
-                          const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public) {
-    if (!pk_is_deposit(pk)) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    WitnessSource src;
-    src.kind = WitnessSource::DEPOSIT;
-    src.d_null = d_null; src.d_sec = d_sec; src.d_dep = d_dep; src.d_public = d_public;
-    return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
-}
-
-uint32_t pk_transfer_depth(const og_pk* pk) {
-    if (pk->n_pub != TRANSFER_N_PUB) return 0;
-    for (uint32_t d = 1; d <= 32; d++) {
-        TransferLayout L = TransferLayout::make(d);
-        if (pk->n_vars == L.n_vars && pk->n_constraints == L.n_constraints) return d;
+int32_t statement_key_depth(const og_pk* pk, Statement s) {
+    const StatementDesc& S = STATEMENTS[s];
+    if (s == ST_WITHDRAW) return pk->depth != 0 && S.shape(pk->depth).n_vars == pk->n_vars ? (int32_t)pk->depth : -1;
+    if (pk->n_pub != S.n_pub) return -1;
+    const uint32_t d_lo = S.takes_depth ? 1 : 0, d_hi = S.takes_depth ? 32 : 0;
+    for (uint32_t d = d_lo; d <= d_hi; d++) {
+        const StatementShape sh = S.shape(d);
+        if (pk->n_vars == sh.n_vars && pk->n_constraints == sh.n_constraints) return (int32_t)d;
     }
-    return 0;
+    return -1;
 }
 
-int32_t prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const TransferInputs& in, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
-                           uint8_t* d_public) {
-    const uint32_t depth = pk_transfer_depth(pk);
-    if (depth == 0) return OG_E_INVALID;
+int32_t prove_statement_dev(og_ctx* ctx, const og_pk* pk, Statement s, const StatementInputs& in, uint32_t batch, const uint8_t* d_rs,
+                            uint8_t* d_proofs, uint8_t* d_public) {
+    const int32_t depth = statement_key_depth(pk, s);
+    if (depth < 0) return OG_E_INVALID;
     if (batch == 0) return OG_OK;
     WitnessSource src;
-    src.kind = WitnessSource::TRANSFER;
-    src.tin = in; src.transfer_depth = depth; src.d_public = d_public;
-    return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
-}
-
-uint32_t pk_association_depth(const og_pk* pk) {
-    if (pk->n_pub != ASSOCIATION_N_PUB) return 0;
-    for (uint32_t d = 1; d <= 32; d++) {
-        AssociationLayout L = AssociationLayout::make(d);
-        if (pk->n_vars == L.n_vars && pk->n_constraints == L.n_constraints) return d;
-    }
-    return 0;
-}
-
-int32_t prove_association_dev(og_ctx* ctx, const og_pk* pk, const AssociationInputs& in, uint32_t batch, const uint8_t* d_rs,
-                              uint8_t* d_proofs, uint8_t* d_public) {
-    const uint32_t depth = pk_association_depth(pk);
-    if (depth == 0) return OG_E_INVALID;
-    if (batch == 0) return OG_OK;
-    WitnessSource src;
-    src.kind = WitnessSource::ASSOCIATION;
-    src.ain = in; src.association_depth = depth; src.d_public = d_public;
+    src.stmt = s; src.depth = (uint32_t)depth; src.in = in; src.d_public = d_public;
     return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
 }
 
 int32_t prove_witness_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs) {
     if (batch == 0) return OG_OK;
     WitnessSource src;
-    src.kind = WitnessSource::FULL;
     src.d_wit = d_wit;
     return prove_batch(ctx, pk, src, batch, d_rs, d_proofs);
 }
@@ -694,45 +631,13 @@ int32_t h_evals_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint8_t*
     return mimc_from_mont_dev(ctx, b.csc + n_priv + pk->n_supp, m, d_out);
 }
 
-int32_t withdraw_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_rec,
-                                   const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, uint8_t* d_out) {
-    WithdrawLayout L = WithdrawLayout::make(depth);
-    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
+int32_t statement_witness_bytes_dev(og_ctx* ctx, Statement s, uint32_t depth, const StatementInputs& in, uint32_t batch, uint8_t* d_out) {
+    const uint32_t nv = STATEMENTS[s].shape(depth).n_vars;
+    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * nv);
     if (!W) return OG_E_NOMEM;
-    OG_TRY(withdraw_witness_strided_dev(ctx, L, L.n_vars, d_null, d_sec, d_rec, d_sib, d_bits, batch, W));
-    uint64_t tot = (uint64_t)batch * L.n_vars;
-    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
-    return OG_OK;
-}
-
-int32_t deposit_witness_bytes_dev(og_ctx* ctx, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
-                                  uint8_t* d_out) {
-    DepositLayout L = DepositLayout::make();
-    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
-    if (!W) return OG_E_NOMEM;
-    OG_TRY(deposit_witness_strided_dev(ctx, L.n_vars, d_null, d_sec, d_dep, batch, W));
-    uint64_t tot = (uint64_t)batch * L.n_vars;
-    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
-    return OG_OK;
-}
-
-int32_t transfer_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const TransferInputs& in, uint32_t batch, uint8_t* d_out) {
-    TransferLayout L = TransferLayout::make(depth);
-    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
-    if (!W) return OG_E_NOMEM;
-    OG_TRY(transfer_witness_strided_dev(ctx, L, L.n_vars, in, batch, W));
-    uint64_t tot = (uint64_t)batch * L.n_vars;
-    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
-    return OG_OK;
-}
-
-int32_t association_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const AssociationInputs& in, uint32_t batch, uint8_t* d_out) {
-    AssociationLayout L = AssociationLayout::make(depth);
-    Fr* W = (Fr*)ctx->slot(S_PR_WIT, sizeof(Fr) * (size_t)batch * L.n_vars);
-    if (!W) return OG_E_NOMEM;
-    OG_TRY(association_witness_strided_dev(ctx, L, L.n_vars, in, batch, W));
-    uint64_t tot = (uint64_t)batch * L.n_vars;
-    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, L.n_vars, L.n_vars, d_out);
+    OG_TRY(statement_witness_dev(ctx, s, depth, nv, in, batch, W));
+    uint64_t tot = (uint64_t)batch * nv;
+    OG_LAUNCH(ctx, k_witness_out, (unsigned)((tot + 127) / 128), 128, 0, W, batch, nv, nv, d_out);
     return OG_OK;
 }
 

@@ -11,33 +11,21 @@ void pk_free(og_pk* pk);
 // true iff the key's tables live on the device `ctx` runs on (a key is bound to the device of the ctx that loaded it)
 bool pk_on_device_of(const og_pk* pk, const og_ctx* ctx);
 void pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m, uint32_t* depth);
-// true iff the key has the deposit statement's shape (n_vars, n_pub, n_constraints): its layout is fixed, so the shape identifies it
-bool pk_is_deposit(const og_pk* pk);
 // window bits of the A (G1), B (G2) and C' (G1) MSMs the key was loaded with
 void pk_window_bits(const og_pk* pk, uint32_t* c3);
-int32_t prove_withdraw_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_rec,
-                           const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
-                           uint8_t* d_public);
-int32_t prove_deposit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
-                          const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public);
-// the depth d in 1..32 whose transfer layout matches the key's n_vars, n_constraints and n_pub = 8; 0 = not a transfer key
-uint32_t pk_transfer_depth(const og_pk* pk);
-int32_t prove_transfer_dev(og_ctx* ctx, const og_pk* pk, const TransferInputs& in, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
-                           uint8_t* d_public);
-// the depth d in 1..32 whose association layout matches the key's n_vars, n_constraints and n_pub = 4; 0 = not an association key
-uint32_t pk_association_depth(const og_pk* pk);
-int32_t prove_association_dev(og_ctx* ctx, const og_pk* pk, const AssociationInputs& in, uint32_t batch, const uint8_t* d_rs,
-                              uint8_t* d_proofs, uint8_t* d_public);
+// The depth the key proves statement s at, or -1 when it is not that statement's key.  A withdraw key records its depth
+// (setup_withdraw, ptau_prepare_withdraw); every other statement's key is recognised by its shape (n_pub, n_vars,
+// n_constraints): deposit's is fixed, transfer and association take the first depth in 1..32 whose layout matches.
+int32_t statement_key_depth(const og_pk* pk, Statement s);
+// a batch of statement s's proofs from its device inputs; OG_E_INVALID for another statement's key, whatever the batch
+int32_t prove_statement_dev(og_ctx* ctx, const og_pk* pk, Statement s, const StatementInputs& in, uint32_t batch, const uint8_t* d_rs,
+                            uint8_t* d_proofs, uint8_t* d_public);
 // the chunk size and lanes prove_batch uses for `batch` proofs with this key, and the scratch bytes of one lane
 void pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane);
 int32_t prove_witness_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs);
 int32_t h_evals_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_wit, uint8_t* d_out);
-int32_t withdraw_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_rec,
-                                   const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, uint8_t* d_out);
-int32_t deposit_witness_bytes_dev(og_ctx* ctx, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep, uint32_t batch,
-                                  uint8_t* d_out);
-int32_t transfer_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const TransferInputs& in, uint32_t batch, uint8_t* d_out);
-int32_t association_witness_bytes_dev(og_ctx* ctx, uint32_t depth, const AssociationInputs& in, uint32_t batch, uint8_t* d_out);
+// statement s's full witnesses at `depth` as canonical bytes, n_vars * 32 per proof
+int32_t statement_witness_bytes_dev(og_ctx* ctx, Statement s, uint32_t depth, const StatementInputs& in, uint32_t batch, uint8_t* d_out);
 // byte offsets of a serialized pk's sections (og_load_pk's layout); false if the header or a section is malformed
 struct PkLayout {
     uint32_t depth, n_constraints, n_vars, n_pub, log_m;

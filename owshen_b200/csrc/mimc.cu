@@ -339,36 +339,33 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
     return OG_OK;
 }
 
-int32_t withdraw_witness_strided_dev(og_ctx* ctx, const WithdrawLayout& L, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec,
-                                     const uint8_t* d_rec, const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, Fr* d_W) {
+// One CTA covers 32 proofs in every statement's kernel; the transfer and association kernels give a proof more than one warp.
+int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
+                              Fr* d_W) {
     if (batch == 0) return OG_OK;
-    if (w_stride < L.n_vars) return OG_E_INVALID;
-    OG_LAUNCH(ctx, k_withdraw_witness, (batch + 31) / 32, 32, 0, L, w_stride, d_null, d_sec, d_rec, d_sib, d_bits, batch, d_W, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep,
-                                    uint32_t batch, Fr* d_W) {
-    if (batch == 0) return OG_OK;
-    DepositLayout L = DepositLayout::make();
-    if (w_stride < L.n_vars) return OG_E_INVALID;
-    OG_LAUNCH(ctx, k_deposit_witness, (batch + 31) / 32, 32, 0, L, w_stride, d_null, d_sec, d_dep, batch, d_W, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint32_t w_stride, const TransferInputs& in, uint32_t batch,
-                                     Fr* d_W) {
-    if (batch == 0) return OG_OK;
-    if (w_stride < L.n_vars) return OG_E_INVALID;
-    OG_LAUNCH(ctx, k_transfer_witness, (batch + 31) / 32, 128, 0, L, w_stride, in, batch, d_W, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t association_witness_strided_dev(og_ctx* ctx, const AssociationLayout& L, uint32_t w_stride, const AssociationInputs& in,
-                                        uint32_t batch, Fr* d_W) {
-    if (batch == 0) return OG_OK;
-    if (w_stride < L.n_vars) return OG_E_INVALID;
-    OG_LAUNCH(ctx, k_association_witness, (batch + 31) / 32, 64, 0, L, w_stride, in, batch, d_W, ctx->d_flag);
+    if (w_stride < STATEMENTS[s].shape(depth).n_vars) return OG_E_INVALID;
+    const uint8_t* const* a = in.p;
+    const uint32_t grid = (batch + 31) / 32;
+    switch (s) {
+    case ST_WITHDRAW:
+        OG_LAUNCH(ctx, k_withdraw_witness, grid, 32, 0, WithdrawLayout::make(depth), w_stride, a[0], a[1], a[2], a[3],
+                  (const uint32_t*)a[4], batch, d_W, ctx->d_flag);
+        break;
+    case ST_DEPOSIT:
+        OG_LAUNCH(ctx, k_deposit_witness, grid, 32, 0, DepositLayout::make(), w_stride, a[0], a[1], a[2], batch, d_W, ctx->d_flag);
+        break;
+    case ST_TRANSFER: {
+        const TransferInputs t{a[0], a[1], a[2], a[3], a[4], (const uint64_t*)a[5], a[6], (const uint32_t*)a[7], a[8], a[9],
+                               (const uint64_t*)a[10]};
+        OG_LAUNCH(ctx, k_transfer_witness, grid, 128, 0, TransferLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
+        break;
+    }
+    case ST_ASSOCIATION: {
+        const AssociationInputs t{a[0], a[1], a[2], a[3], (const uint32_t*)a[4], a[5], (const uint32_t*)a[6]};
+        OG_LAUNCH(ctx, k_association_witness, grid, 64, 0, AssociationLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
+        break;
+    }
+    }
     return OG_OK;
 }
 

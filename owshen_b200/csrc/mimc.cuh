@@ -2,6 +2,7 @@
 // withdraw, deposit, transfer and association statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
 // oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout and oracle/association_circuit.py: Layout).
 #pragma once
+#include <initializer_list>
 #include "common.cuh"
 
 namespace og {
@@ -72,8 +73,8 @@ struct TransferLayout {
     OG_HD uint32_t out(uint32_t j) const { return out_base + j * out_size; }
 };
 
-// the caller's inputs of a batch of transfers; per proof, input (output) 0 then 1 in the in_* (out_*) arrays,
-// in_siblings holds 2 * depth elements (input 0's path, then input 1's) and in_path_bits 2 words
+// the caller's inputs of a batch of transfers (k_transfer_witness's argument); per proof, input (output) 0 then 1 in the
+// in_* (out_*) arrays, in_siblings holds 2 * depth elements (input 0's path, then input 1's) and in_path_bits 2 words
 struct TransferInputs {
     const uint8_t *roots, *tokens, *recipients;
     const uint8_t *in_null, *in_sec;
@@ -82,15 +83,6 @@ struct TransferInputs {
     const uint32_t* in_bits;
     const uint8_t *out_null, *out_sec;
     const uint64_t* out_amounts;
-    // the same inputs from proof `off` on
-    TransferInputs at(uint32_t off, uint32_t depth) const {
-        TransferInputs t = *this;
-        t.roots += 32ull * off; t.tokens += 32ull * off; t.recipients += 32ull * off;
-        t.in_null += 64ull * off; t.in_sec += 64ull * off; t.in_amounts += 2ull * off;
-        t.in_sib += 64ull * depth * off; t.in_bits += 2ull * off;
-        t.out_null += 64ull * off; t.out_sec += 64ull * off; t.out_amounts += 2ull * off;
-        return t;
-    }
 };
 
 constexpr uint32_t ASSOCIATION_N_PUB = 4;
@@ -115,20 +107,61 @@ struct AssociationLayout {
     }
 };
 
-// the caller's inputs of a batch of association-set withdrawals: per proof 32 B each of nullifier, secret, recipient,
-// depth siblings per tree and one path-bits word per tree
+// the caller's inputs of a batch of association-set withdrawals (k_association_witness's argument): per proof 32 B each of
+// nullifier, secret, recipient, depth siblings per tree and one path-bits word per tree
 struct AssociationInputs {
     const uint8_t *nullifiers, *secrets, *recipients, *siblings;
     const uint32_t* path_bits;
     const uint8_t* assoc_siblings;
     const uint32_t* assoc_path_bits;
+};
+
+// ---- the statement table ------------------------------------------------------------------------------------------------
+// What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
+// statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
+// statement_witness_dev) and its og_* forwarders (capi.cu).
+enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION };
+constexpr uint32_t STATEMENT_MAX_INPUTS = 11;
+
+struct StatementShape { uint32_t n_vars, n_constraints; };
+template <class Layout> StatementShape layout_shape(uint32_t depth) { const Layout L = Layout::make(depth); return {L.n_vars, L.n_constraints}; }
+template <> inline StatementShape layout_shape<DepositLayout>(uint32_t) { const DepositLayout L = DepositLayout::make(); return {L.n_vars, L.n_constraints}; }
+
+struct StatementDesc {
+    uint32_t n_pub;
+    StatementShape (*shape)(uint32_t depth);
+    bool takes_depth;                                   // false: one fixed shape, depth 0 throughout
+    uint32_t n_inputs;
+    // the input arrays in C ABI order: bytes per proof = fixed[k] + per_level[k] * depth
+    uint32_t fixed[STATEMENT_MAX_INPUTS], per_level[STATEMENT_MAX_INPUTS];
+    uint64_t input_bytes(uint32_t k, uint32_t depth) const { return fixed[k] + (uint64_t)per_level[k] * depth; }
+};
+
+constexpr StatementDesc STATEMENTS[] = {
+    // withdraw: nullifiers, secrets, recipients, siblings, path_bits
+    {WITHDRAW_N_PUB, layout_shape<WithdrawLayout>, true, 5, {32, 32, 32, 0, 4}, {0, 0, 0, 32, 0}},
+    // deposit: nullifiers, secrets, depositors
+    {DEPOSIT_N_PUB, layout_shape<DepositLayout>, false, 3, {32, 32, 32}, {0, 0, 0}},
+    // transfer: roots, tokens, recipients, in_nullifiers, in_secrets, in_amounts, in_siblings, in_path_bits, out_nullifiers,
+    // out_secrets, out_amounts
+    {TRANSFER_N_PUB, layout_shape<TransferLayout>, true, 11, {32, 32, 32, 64, 64, 16, 0, 8, 64, 64, 16}, {0, 0, 0, 0, 0, 0, 64, 0, 0, 0, 0}},
+    // association: nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits
+    {ASSOCIATION_N_PUB, layout_shape<AssociationLayout>, true, 7, {32, 32, 32, 0, 4, 0, 4}, {0, 0, 0, 32, 0, 32, 0}},
+};
+
+// the input arrays of a batch in the statement's C ABI order (host or device pointers)
+struct StatementInputs {
+    const uint8_t* p[STATEMENT_MAX_INPUTS] = {};
+    StatementInputs() = default;
+    StatementInputs(std::initializer_list<const void*> xs) {
+        uint32_t k = 0;
+        for (const void* x : xs) p[k++] = static_cast<const uint8_t*>(x);
+    }
     // the same inputs from proof `off` on
-    AssociationInputs at(uint32_t off, uint32_t depth) const {
-        AssociationInputs a = *this;
-        a.nullifiers += 32ull * off; a.secrets += 32ull * off; a.recipients += 32ull * off;
-        a.siblings += 32ull * depth * off; a.path_bits += off;
-        a.assoc_siblings += 32ull * depth * off; a.assoc_path_bits += off;
-        return a;
+    StatementInputs at(Statement s, uint32_t depth, uint32_t off) const {
+        StatementInputs r = *this;
+        for (uint32_t k = 0; k < STATEMENTS[s].n_inputs; k++) r.p[k] += STATEMENTS[s].input_bytes(k, depth) * off;
+        return r;
     }
 };
 
@@ -139,15 +172,10 @@ int32_t mimc_to_mont_dev(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Fr* d_out
 int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_out);
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves);
 int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64_t n, const Fr* h_aux, Fr* d_nodes);
-// W rows are w_stride elements apart (the prover keeps two extra scalars after every witness)
-int32_t withdraw_witness_strided_dev(og_ctx* ctx, const WithdrawLayout& L, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec,
-                                     const uint8_t* d_rec, const uint8_t* d_sib, const uint32_t* d_bits, uint32_t batch, Fr* d_W);
-int32_t deposit_witness_strided_dev(og_ctx* ctx, uint32_t w_stride, const uint8_t* d_null, const uint8_t* d_sec, const uint8_t* d_dep,
-                                    uint32_t batch, Fr* d_W);
-int32_t transfer_witness_strided_dev(og_ctx* ctx, const TransferLayout& L, uint32_t w_stride, const TransferInputs& in, uint32_t batch,
-                                     Fr* d_W);
-int32_t association_witness_strided_dev(og_ctx* ctx, const AssociationLayout& L, uint32_t w_stride, const AssociationInputs& in,
-                                        uint32_t batch, Fr* d_W);
+// the statement's witness kernel on device inputs; W rows are w_stride elements apart (the prover keeps two extra scalars
+// after every witness)
+int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
+                              Fr* d_W);
 
 // BabyJubJub batch verification (bjj_impl.cuh); out[i] in {0, 1, 2 = public key does not decompress}
 int32_t bjj_verify_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_odd, const uint8_t* d_msgs, const uint8_t* d_sigs,

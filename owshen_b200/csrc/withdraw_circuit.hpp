@@ -2,7 +2,8 @@
 // R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these are the
 // product's own definitions, checked entry for entry against the independently written
 // oracle/withdraw_circuit.py, oracle/deposit_circuit.py, oracle/transfer_circuit.py and oracle/association_circuit.py
-// through og_withdraw_r1cs_export, og_deposit_r1cs_export, og_transfer_r1cs_export and og_association_r1cs_export.
+// through og_withdraw_r1cs_export, og_deposit_r1cs_export, og_transfer_r1cs_export and og_association_r1cs_export
+// (statement_r1cs below).
 //
 // withdraw
 //   public : root, nullifier_hash, recipient
@@ -227,6 +228,17 @@ struct AssociationBuilder {
         return b.cs;
     }
 };
+
+// the statement's R1CS at `depth` (ignored by deposit)
+inline R1cs statement_r1cs(Statement s, uint32_t depth) {
+    switch (s) {
+    case ST_WITHDRAW: return WithdrawBuilder::build(depth);
+    case ST_DEPOSIT: return DepositBuilder::build();
+    case ST_TRANSFER: return TransferBuilder::build(depth);
+    case ST_ASSOCIATION: return AssociationBuilder::build(depth);
+    }
+    return R1cs();
+}
 
 inline uint32_t groth16_domain_log(uint32_t n_constraints, uint32_t n_pub) {
     uint32_t need = n_constraints + n_pub + 1, k = 0;

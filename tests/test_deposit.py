@@ -269,11 +269,14 @@ def _generic_key(ctx, n_vars, n_pub, rng):
 
 @pytest.mark.gpu
 def test_prove_deposit_and_withdraw_refuse_each_others_keys(ctx, deposit_keys):
+    import torch
     pk_d = deposit_keys[0]
     rng = random.Random(35)
     nul, sec, dep = rand_deposits(rng, 2)
     rs = cport.frs([rng.randrange(R) for _ in range(4)])
     tw = [rng.randrange(1, R) for _ in range(5)]
+    d_buf = torch.zeros(1 << 16, dtype=torch.uint8, device="cuda")
+    d = api._ptr(d_buf)      # every device argument of the _dev entry points
     others = [ob.setup_withdraw(ctx, 2, *tw)[0], _generic_key(ctx, 735, 2, rng), _generic_key(ctx, 735, 1, rng)]
     for pk in others:
         PK = ob.ProvingKey(ctx, pk)
@@ -281,8 +284,10 @@ def test_prove_deposit_and_withdraw_refuse_each_others_keys(ctx, deposit_keys):
             with pytest.raises(ob.OwshenB200Error) as e:
                 PK.prove_deposit(nul, sec, dep, rs)
             assert e.value.code == api.OG_E_INVALID
-            # batch 0 is refused too: the key is wrong whatever the batch
-            assert api.lib().og_groth16_prove_deposit(ctx._h, PK._h, nul, sec, dep, 0, rs, bytes(256), None) == api.OG_E_INVALID
+            for b in (2, 0):      # the key is wrong whatever the batch
+                rc = api.lib().og_groth16_prove_deposit(ctx._h, PK._h, nul, sec, dep, b, rs, api.C.create_string_buffer(512), None)
+                assert rc == api.OG_E_INVALID, b
+                assert api.lib().og_groth16_prove_deposit_dev(ctx._h, PK._h, d, d, d, b, d, d, None) == api.OG_E_INVALID, b
         finally:
             PK.close()
     PK = ob.ProvingKey(ctx, pk_d)
@@ -291,8 +296,11 @@ def test_prove_deposit_and_withdraw_refuse_each_others_keys(ctx, deposit_keys):
         with pytest.raises(ValueError):
             ob.prove(PK, nul, sec, dep, bytes(64), [0, 0], rs)
         bits = (api.C.c_uint32 * 2)(0, 0)
-        rc = api.lib().og_groth16_prove_withdraw(ctx._h, PK._h, nul, sec, dep, bytes(64), bits, 2, rs, api.C.create_string_buffer(512), None)
-        assert rc == api.OG_E_INVALID
+        for b in (2, 0):
+            rc = api.lib().og_groth16_prove_withdraw(ctx._h, PK._h, nul, sec, dep, bytes(64), bits, b, rs, api.C.create_string_buffer(512),
+                                                     None)
+            assert rc == api.OG_E_INVALID, b
+            assert api.lib().og_groth16_prove_withdraw_dev(ctx._h, PK._h, d, d, d, d, d, b, d, d, None) == api.OG_E_INVALID, b
         assert len(PK.prove_deposit(nul, sec, dep, rs)[0]) == 512          # the context is still usable
     finally:
         PK.close()

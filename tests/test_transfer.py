@@ -421,6 +421,9 @@ def _generic_key(ctx, n_vars, n_pub, rng):
 
 @pytest.mark.gpu
 def test_transfer_and_other_provers_refuse_each_others_keys(ctx):
+    import torch
+    d_buf = torch.zeros(1 << 16, dtype=torch.uint8, device="cuda")
+    d = api._ptr(d_buf)      # every device argument of the _dev entry points
     rng = random.Random(45)
     pk_t = transfer_keys(ctx, 2)[0]
     rows = random_rows(rng, 2, 2)
@@ -442,14 +445,17 @@ def test_transfer_and_other_provers_refuse_each_others_keys(ctx):
                 rc = api.lib().og_groth16_prove_transfer(ctx._h, PK._h, *[api._ptr(x) for x in args], b, rs,
                                                          api.C.create_string_buffer(512), None)
                 assert rc == api.OG_E_INVALID, b
+                assert api.lib().og_groth16_prove_transfer_dev(ctx._h, PK._h, *[d] * 11, b, d, d, None) == api.OG_E_INVALID, b
         finally:
             PK.close()
     PK = ob.ProvingKey(ctx, pk_t)
     try:
         nul, sec, rec = (cport.frs([rng.randrange(R) for _ in range(2)]) for _ in range(3))
-        rc = api.lib().og_groth16_prove_withdraw(ctx._h, PK._h, nul, sec, rec, bytes(128), (api.C.c_uint32 * 2)(0, 0), 2, rs,
-                                                 api.C.create_string_buffer(512), None)
-        assert rc == api.OG_E_INVALID
+        for b in (2, 0):
+            rc = api.lib().og_groth16_prove_withdraw(ctx._h, PK._h, nul, sec, rec, bytes(128), (api.C.c_uint32 * 2)(0, 0), b, rs,
+                                                     api.C.create_string_buffer(512), None)
+            assert rc == api.OG_E_INVALID, b
+            assert api.lib().og_groth16_prove_withdraw_dev(ctx._h, PK._h, d, d, d, d, d, b, d, d, None) == api.OG_E_INVALID, b
         with pytest.raises(ob.OwshenB200Error) as e:
             PK.prove_deposit(nul, sec, rec, rs)
         assert e.value.code == api.OG_E_INVALID
