@@ -510,8 +510,9 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
     OG_LAUNCH(ctx, k_abc, dim3((m + 127) / 128, B), 128, 0, A, Bm, pk->n_constraints, pk->n_pub, pk->log_m, W, b.w_stride, B, b.abc);
     OG_TRY(ntt_mont_dev(ctx, b.abc, b.ntt_tmp, pk->log_m, 3 * B, 1, 0, 1));      // 1/n folded into ...
     OG_TRY(ntt_mont_dev(ctx, b.abc, b.ntt_tmp, pk->log_m, 3 * B, 0, 1, 2));      // ... the coset factors of the forward transform
+    // at least one block: its thread 0 writes the fixed terms, also for a key with no private variable and no B support
     uint32_t mx = n_priv > pk->n_supp ? n_priv : pk->n_supp;
-    OG_LAUNCH(ctx, k_compose, dim3((mx + 127) / 128, B), 128, 0, W, b.w_stride, rs_m, pk->supp, pk->n_supp, pk->n_vars, pk->n_pub, m,
+    OG_LAUNCH(ctx, k_compose, dim3(mx ? (mx + 127) / 128 : 1, B), 128, 0, W, b.w_stride, rs_m, pk->supp, pk->n_supp, pk->n_vars, pk->n_pub, m,
               b.bsc, b.bsc_stride, b.csc, b.csc_stride);
     OG_LAUNCH(ctx, k_pointwise, dim3((m + 127) / 128, B), 128, 0, b.abc, pk->log_m, B, b.csc, b.csc_stride, n_priv + pk->n_supp);
     OG_TRY(run_msm_g1(ctx, pk, 0, b, B, pk->tabA, pk->nA, W, b.w_stride, b.totA + off));
@@ -522,12 +523,14 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
     return OG_OK;
 }
 
-// offsets into the sorted digit lists and bucket keys are 32-bit: bound the chunk so they cannot overflow
+// offsets into the sorted digit lists and bucket keys are 32-bit: bound the chunk so they cannot overflow.  The chunk's
+// kernels put its proofs on grid.y, the NTT three transforms per proof, and grid.y is at most 65535.
 static uint32_t chunk_limit(const og_pk* pk) {
     uint64_t max_pts = pk->nC > pk->nA ? pk->nC : pk->nA;
     uint64_t by_entries = 0xF0000000ull / (max_pts * pk->max_windows);
     uint64_t by_keys = 0x7FFFFFFFull / pk->max_nb;
     uint64_t lim = by_entries < by_keys ? by_entries : by_keys;
+    if (lim > 65535 / 3) lim = 65535 / 3;
     return (uint32_t)(lim < 1 ? 1 : lim);
 }
 
