@@ -158,18 +158,6 @@ __global__ void __launch_bounds__(128) k_gather_rows(const uint8_t* __restrict__
 // ---- host helpers around the kernels --------------------------------------------------------------------------------
 static unsigned blocks(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
-template <class F> static int32_t to_mont(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Affine<F>* d_out) {
-    if constexpr (sizeof(F) == sizeof(Fq)) return g1_bytes_to_mont(ctx, d_in, n, d_out);
-    else return g2_bytes_to_mont(ctx, d_in, n, d_out);
-}
-template <class F> static int32_t to_bytes(og_ctx* ctx, const Affine<F>* d_in, uint64_t n, uint8_t* d_out) {
-    if constexpr (sizeof(F) == sizeof(Fq)) return g1_mont_to_bytes(ctx, d_in, n, d_out);
-    else return g2_mont_to_bytes(ctx, d_in, n, d_out);
-}
-template <class F> static int32_t msm_bytes(og_ctx* ctx, const uint8_t* d_pts, const uint8_t* d_sc, uint64_t n, uint8_t* d_out) {
-    if constexpr (sizeof(F) == sizeof(Fq)) return msm_g1_dev(ctx, d_pts, d_sc, n, d_out);
-    else return msm_g2_dev(ctx, d_pts, d_sc, n, d_out);
-}
 template <class F> static F curve_b() {
     if constexpr (sizeof(F) == sizeof(Fq)) return Fq::from_u32(3);
     else return Fq2{Fq::from_u32(3), Fq::zero()} * Fq2{Fq::from_u32(9), Fq::from_u32(1)}.inv();
@@ -211,9 +199,9 @@ static int32_t scale_bytes_host(og_ctx* ctx, const uint8_t* in, uint64_t n, cons
     OG_ALLOC(ctx, db, PB * n); OG_ALLOC(ctx, dm, PB * n); OG_ALLOC(ctx, ds, sizeof(Fr));
     OG_CUDA(ctx, cudaMemcpyAsync(db.p, in, PB * n, cudaMemcpyHostToDevice, ctx->stream));
     OG_CUDA(ctx, cudaMemcpyAsync(ds.p, &s, sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
-    OG_TRY(to_mont<F>(ctx, db.as<uint8_t>(), n, dm.as<Affine<F>>()));
+    OG_TRY(points_bytes_to_mont(ctx, db.as<uint8_t>(), n, dm.as<Affine<F>>()));
     OG_TRY(scale<F>(ctx, dm.as<Affine<F>>(), ds.as<Fr>(), n, 0, dm.as<Affine<F>>()));
-    OG_TRY(to_bytes<F>(ctx, dm.as<Affine<F>>(), n, db.as<uint8_t>()));
+    OG_TRY(points_mont_to_bytes(ctx, dm.as<Affine<F>>(), n, db.as<uint8_t>()));
     OG_CUDA(ctx, cudaMemcpyAsync(out, db.p, PB * n, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaMemsetAsync(ds.p, 0, sizeof(Fr), ctx->stream));
     return check_flag(ctx);
@@ -226,13 +214,13 @@ static int32_t gen_mul(og_ctx* ctx, const Fr* xs, int n, uint8_t* g1_out, uint8_
     std::vector<uint8_t> s(32 * n);
     for (int i = 0; i < n; i++) host_store(s.data() + 32 * i, xs[i]);
     OG_CUDA(ctx, cudaMemcpyAsync(ds.p, s.data(), 32 * n, cudaMemcpyHostToDevice, ctx->stream));
-    OG_TRY(fixed_base_mul_g1(ctx, ds.as<uint8_t>(), n, dp.as<G1Affine>()));
-    OG_TRY(g1_mont_to_bytes(ctx, dp.as<G1Affine>(), n, db.as<uint8_t>()));
+    OG_TRY(fixed_base_mul(ctx, ds.as<uint8_t>(), n, dp.as<G1Affine>()));
+    OG_TRY(points_mont_to_bytes(ctx, dp.as<G1Affine>(), n, db.as<uint8_t>()));
     OG_CUDA(ctx, cudaMemcpyAsync(g1_out, db.p, 64 * n, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (g2_out) {
-        OG_TRY(fixed_base_mul_g2(ctx, ds.as<uint8_t>(), n, dp.as<G2Affine>()));
-        OG_TRY(g2_mont_to_bytes(ctx, dp.as<G2Affine>(), n, db.as<uint8_t>()));
+        OG_TRY(fixed_base_mul(ctx, ds.as<uint8_t>(), n, dp.as<G2Affine>()));
+        OG_TRY(points_mont_to_bytes(ctx, dp.as<G2Affine>(), n, db.as<uint8_t>()));
         OG_CUDA(ctx, cudaMemcpyAsync(g2_out, db.p, 128 * n, cudaMemcpyDeviceToHost, ctx->stream));
     }
     OG_CUDA(ctx, cudaMemsetAsync(ds.p, 0, 32 * n, ctx->stream));
@@ -319,8 +307,8 @@ static int32_t shifted_sums(og_ctx* ctx, const uint8_t* d_pts, uint64_t n, const
     const uint64_t PB = sizeof(Affine<F>);
     DevBuf out;
     OG_ALLOC(ctx, out, 2 * PB);
-    OG_TRY(msm_bytes<F>(ctx, d_pts, d_rho, n - 1, out.as<uint8_t>()));
-    OG_TRY(msm_bytes<F>(ctx, d_pts + PB, d_rho, n - 1, out.as<uint8_t>() + PB));
+    OG_TRY(msm_dev<F>(ctx, d_pts, d_rho, n - 1, out.as<uint8_t>()));
+    OG_TRY(msm_dev<F>(ctx, d_pts + PB, d_rho, n - 1, out.as<uint8_t>() + PB));
     OG_CUDA(ctx, cudaMemcpyAsync(s0, out.p, PB, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaMemcpyAsync(s1, out.as<uint8_t>() + PB, PB, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -346,7 +334,7 @@ static int32_t check_points(og_ctx* ctx, const uint8_t* d_bytes, uint64_t n, int
     OG_ALLOC(ctx, bad, sizeof(int));
     OG_CUDA(ctx, cudaMemsetAsync(bad.p, 0, sizeof(int), ctx->stream));
     OG_TRY(clear_flag(ctx));
-    OG_TRY(to_mont<F>(ctx, d_bytes, n, dm.as<Affine<F>>()));
+    OG_TRY(points_bytes_to_mont(ctx, d_bytes, n, dm.as<Affine<F>>()));
     const int subgroup = sizeof(F) != sizeof(Fq);
     if (n) OG_LAUNCH(ctx, k_check_points<F>, blocks(n, 128), 128, 0, dm.as<Affine<F>>(), n, curve_b<F>(), allow_inf, subgroup, bad.as<int>());
     int h = 0;
@@ -394,8 +382,8 @@ int32_t ptau_contribute(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, const
             OG_ALLOC(ctx, s1, sizeof(Fr) * n1); OG_ALLOC(ctx, s2, sizeof(Fr) * n2);
             OG_TRY(clear_flag(ctx));
             OG_CUDA(ctx, cudaMemcpyAsync(db.p, acc, acc_len, cudaMemcpyHostToDevice, ctx->stream));
-            OG_TRY(g1_bytes_to_mont(ctx, db.as<uint8_t>() + L.tau1, n1, d1.as<G1Affine>()));
-            OG_TRY(g2_bytes_to_mont(ctx, db.as<uint8_t>() + L.tau2, n2, d2.as<G2Affine>()));
+            OG_TRY(points_bytes_to_mont(ctx, db.as<uint8_t>() + L.tau1, n1, d1.as<G1Affine>()));
+            OG_TRY(points_bytes_to_mont(ctx, db.as<uint8_t>() + L.tau2, n2, d2.as<G2Affine>()));
             // G1 scalars: t^i (2M), a t^i (M), b t^i (M); G2 scalars: t^i (M), b
             Fr* S1 = s1.as<Fr>(); Fr* S2 = s2.as<Fr>();
             OG_TRY(powers(ctx, Fr::one(), x[0], 2 * M, S1));
@@ -407,8 +395,8 @@ int32_t ptau_contribute(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, const
             OG_TRY(scale<Fq2>(ctx, d2.as<G2Affine>(), S2, n2, 1, d2.as<G2Affine>()));
             OG_CUDA(ctx, cudaMemsetAsync(s1.p, 0, sizeof(Fr) * n1, ctx->stream));
             OG_CUDA(ctx, cudaMemsetAsync(s2.p, 0, sizeof(Fr) * n2, ctx->stream));
-            OG_TRY(g1_mont_to_bytes(ctx, d1.as<G1Affine>(), n1, db.as<uint8_t>() + L.tau1));
-            OG_TRY(g2_mont_to_bytes(ctx, d2.as<G2Affine>(), n2, db.as<uint8_t>() + L.tau2));
+            OG_TRY(points_mont_to_bytes(ctx, d1.as<G1Affine>(), n1, db.as<uint8_t>() + L.tau1));
+            OG_TRY(points_mont_to_bytes(ctx, d2.as<G2Affine>(), n2, db.as<uint8_t>() + L.tau2));
             OG_CUDA(ctx, cudaMemcpyAsync(acc_out + PT_HDR, db.as<uint8_t>() + PT_HDR, acc_len - PT_HDR, cudaMemcpyDeviceToHost, ctx->stream));
             OG_TRY(check_flag(ctx));
             memcpy(acc_out, acc, PT_HDR);
@@ -516,7 +504,7 @@ static int32_t column_sums(og_ctx* ctx, const Affine<F>* d_pts, const uint8_t* d
     }
     OG_LAUNCH(ctx, k_colsum<F>, blocks(n_cols, 128), 128, 0, d_pts, dptr.as<uint32_t>(), didx.as<uint32_t>(), dval.as<uint32_t>(), n_cols,
               COL_HEAVY, dm.as<Affine<F>>());
-    OG_TRY(to_bytes<F>(ctx, dm.as<Affine<F>>(), n_cols, db.as<uint8_t>()));
+    OG_TRY(points_mont_to_bytes(ctx, dm.as<Affine<F>>(), n_cols, db.as<uint8_t>()));
     uint32_t longest = 0;
     for (uint32_t i = 0; i < n_cols; i++) longest = std::max(longest, c.ptr[i + 1] - c.ptr[i]);
     if (longest > COL_HEAVY) {
@@ -525,7 +513,7 @@ static int32_t column_sums(og_ctx* ctx, const Affine<F>* d_pts, const uint8_t* d
             const uint32_t b = c.ptr[i], n = c.ptr[i + 1] - b;
             if (n <= COL_HEAVY) continue;
             OG_LAUNCH(ctx, k_gather_rows, blocks(n, 128), 128, 0, d_pts_bytes, (uint32_t)PB, didx.as<uint32_t>() + b, n, stage.as<uint8_t>());
-            OG_TRY(msm_bytes<F>(ctx, stage.as<uint8_t>(), dval.as<uint8_t>() + 32ull * b, n, db.as<uint8_t>() + PB * i));
+            OG_TRY(msm_dev<F>(ctx, stage.as<uint8_t>(), dval.as<uint8_t>() + 32ull * b, n, db.as<uint8_t>() + PB * i));
         }
     }
     OG_CUDA(ctx, cudaMemcpyAsync(out_host, db.p, PB * n_cols, cudaMemcpyDeviceToHost, ctx->stream));
@@ -555,18 +543,18 @@ int32_t ptau_prepare(og_ctx* ctx, const uint8_t* acc, uint64_t acc_len, const R1
     OG_CUDA(ctx, cudaMemcpyAsync(db.p, acc, acc_len, cudaMemcpyHostToDevice, ctx->stream));
     const uint8_t* d = db.as<uint8_t>();
     G1Affine* p1 = P1.as<G1Affine>();
-    OG_TRY(g1_bytes_to_mont(ctx, d + L.tau1, m, p1));
-    OG_TRY(g1_bytes_to_mont(ctx, d + L.alpha1, m, p1 + m));
-    OG_TRY(g1_bytes_to_mont(ctx, d + L.beta1, m, p1 + 2 * m));
-    OG_TRY(g1_bytes_to_mont(ctx, d + L.tau1, 2 * m, H2.as<G1Affine>()));
-    OG_TRY(g2_bytes_to_mont(ctx, d + L.tau2, m, Q2.as<G2Affine>()));
+    OG_TRY(points_bytes_to_mont(ctx, d + L.tau1, m, p1));
+    OG_TRY(points_bytes_to_mont(ctx, d + L.alpha1, m, p1 + m));
+    OG_TRY(points_bytes_to_mont(ctx, d + L.beta1, m, p1 + 2 * m));
+    OG_TRY(points_bytes_to_mont(ctx, d + L.tau1, 2 * m, H2.as<G1Affine>()));
+    OG_TRY(points_bytes_to_mont(ctx, d + L.tau2, m, Q2.as<G2Affine>()));
     OG_TRY(check_flag(ctx));
     for (int k = 0; k < 3; k++) OG_TRY(intt<Fq>(ctx, p1 + k * m, log_m));
     OG_TRY(intt<Fq>(ctx, H2.as<G1Affine>(), log_m + 1));
     OG_TRY(intt<Fq2>(ctx, Q2.as<G2Affine>(), log_m));
-    OG_TRY(g1_mont_to_bytes(ctx, p1, 3 * m, P1b.as<uint8_t>()));
-    OG_TRY(g2_mont_to_bytes(ctx, Q2.as<G2Affine>(), m, Q2b.as<uint8_t>()));
-    OG_TRY(g1_mont_to_bytes(ctx, H2.as<G1Affine>(), 2 * m, db.as<uint8_t>()));   // the accumulator copy is no longer needed
+    OG_TRY(points_mont_to_bytes(ctx, p1, 3 * m, P1b.as<uint8_t>()));
+    OG_TRY(points_mont_to_bytes(ctx, Q2.as<G2Affine>(), m, Q2b.as<uint8_t>()));
+    OG_TRY(points_mont_to_bytes(ctx, H2.as<G1Affine>(), 2 * m, db.as<uint8_t>()));   // the accumulator copy is no longer needed
     std::vector<uint8_t> h2(64 * 2 * m), qh(64 * m);
     OG_CUDA(ctx, cudaMemcpyAsync(h2.data(), db.p, 64 * 2 * m, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -678,8 +666,8 @@ int32_t phase2_verify(og_ctx* ctx, const uint8_t* pk0, uint64_t pk0_len, const u
     std::vector<uint8_t> k0(pk0, pk0 + pk0_len);
     k0.insert(k0.end(), vk0, vk0 + vk0_len);
     OG_TRY(rho_powers(ctx, fs_rho(k0.data(), k0.size(), k1.data(), k1.size(), rec, rec_len), n_lh, rho));
-    OG_TRY(msm_g1_dev(ctx, db.as<uint8_t>(), rho.as<uint8_t>(), n_lh, out.as<uint8_t>()));
-    OG_TRY(msm_g1_dev(ctx, db.as<uint8_t>() + 64 * n_lh, rho.as<uint8_t>(), n_lh, out.as<uint8_t>() + 64));
+    OG_TRY(msm_dev<Fq>(ctx, db.as<uint8_t>(), rho.as<uint8_t>(), n_lh, out.as<uint8_t>()));
+    OG_TRY(msm_dev<Fq>(ctx, db.as<uint8_t>() + 64 * n_lh, rho.as<uint8_t>(), n_lh, out.as<uint8_t>() + 64));
     uint8_t s[128];
     OG_CUDA(ctx, cudaMemcpyAsync(s, out.p, 128, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -697,13 +685,13 @@ int32_t scale_points_dev(og_ctx* ctx, int g2, const uint8_t* d_points, const uin
     OG_ALLOC(ctx, pm, (g2 ? sizeof(G2Affine) : sizeof(G1Affine)) * n);
     OG_TRY(mimc_to_mont_dev(ctx, d_scalars, ns, s.as<Fr>()));
     if (g2) {
-        OG_TRY(g2_bytes_to_mont(ctx, d_points, n, pm.as<G2Affine>()));
+        OG_TRY(points_bytes_to_mont(ctx, d_points, n, pm.as<G2Affine>()));
         OG_TRY(scale<Fq2>(ctx, pm.as<G2Affine>(), s.as<Fr>(), n, per_point, pm.as<G2Affine>()));
-        OG_TRY(g2_mont_to_bytes(ctx, pm.as<G2Affine>(), n, d_out));
+        OG_TRY(points_mont_to_bytes(ctx, pm.as<G2Affine>(), n, d_out));
     } else {
-        OG_TRY(g1_bytes_to_mont(ctx, d_points, n, pm.as<G1Affine>()));
+        OG_TRY(points_bytes_to_mont(ctx, d_points, n, pm.as<G1Affine>()));
         OG_TRY(scale<Fq>(ctx, pm.as<G1Affine>(), s.as<Fr>(), n, per_point, pm.as<G1Affine>()));
-        OG_TRY(g1_mont_to_bytes(ctx, pm.as<G1Affine>(), n, d_out));
+        OG_TRY(points_mont_to_bytes(ctx, pm.as<G1Affine>(), n, d_out));
     }
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return OG_OK;
@@ -714,13 +702,13 @@ int32_t intt_points_dev(og_ctx* ctx, int g2, uint8_t* d_points, uint32_t log_m) 
     DevBuf pm;
     OG_ALLOC(ctx, pm, (g2 ? sizeof(G2Affine) : sizeof(G1Affine)) * m);
     if (g2) {
-        OG_TRY(g2_bytes_to_mont(ctx, d_points, m, pm.as<G2Affine>()));
+        OG_TRY(points_bytes_to_mont(ctx, d_points, m, pm.as<G2Affine>()));
         OG_TRY(intt<Fq2>(ctx, pm.as<G2Affine>(), log_m));
-        OG_TRY(g2_mont_to_bytes(ctx, pm.as<G2Affine>(), m, d_points));
+        OG_TRY(points_mont_to_bytes(ctx, pm.as<G2Affine>(), m, d_points));
     } else {
-        OG_TRY(g1_bytes_to_mont(ctx, d_points, m, pm.as<G1Affine>()));
+        OG_TRY(points_bytes_to_mont(ctx, d_points, m, pm.as<G1Affine>()));
         OG_TRY(intt<Fq>(ctx, pm.as<G1Affine>(), log_m));
-        OG_TRY(g1_mont_to_bytes(ctx, pm.as<G1Affine>(), m, d_points));
+        OG_TRY(points_mont_to_bytes(ctx, pm.as<G1Affine>(), m, d_points));
     }
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return OG_OK;

@@ -101,8 +101,7 @@ enum Slot {
     S_SETUP_A, S_SETUP_B, S_SETUP_C,
     // lane 1 copies of the per-chunk prover scratch (same order as S_PR_ABC .. S_PR_HEAVY) and of S_MSM_MISC
     S_L1_ABC, S_L1_SCALARS, S_L1_SORTED, S_L1_COUNTS, S_L1_OFFSETS, S_L1_CURSOR, S_L1_BUCKETS, S_L1_SEG, S_L1_HEAVY, S_L1_MSM_MISC,
-    S_PR_AFF, S_L1_AFF, S_MSM_AFF,
-    S_PR_SORT_STAGE, S_L1_SORT_STAGE, S_PR_SORT_TILES, S_L1_SORT_TILES,   // only for keys whose sort scratch outgrows bk2 / heavy
+    S_PR_SORT_STAGE, S_L1_SORT_STAGE, S_PR_SORT_TILES, S_L1_SORT_TILES,   // only for keys whose sort scratch outgrows the buckets / heavy scratch
     S_IO_STATEMENT,                                                         // the staged input arrays of a statement's batch
     S_IO_NOTE, S_NOTE_KEYS, S_NOTE_PREP,                                    // note encryption / scanning (note_impl.cuh)
     S_COUNT

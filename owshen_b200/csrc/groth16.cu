@@ -236,6 +236,19 @@ static uint32_t prover_window_bits(uint32_t n) {
     return best;
 }
 
+// One fixed-base table of a key: n boundary points -> *table, n * n_windows affine Montgomery points (msm_build_table).
+// The caller frees *table (pk_free) also when this fails.
+template <class F>
+static int32_t upload_table(og_ctx* ctx, const std::vector<uint8_t>& points, uint32_t n, uint32_t c, uint32_t n_windows, Affine<F>** table) {
+    uint8_t* stage;
+    OG_TRY(upload(ctx, &stage, points.data(), points.size()));
+    if (cudaMalloc(table, sizeof(Affine<F>) * (size_t)n * n_windows) != cudaSuccess) { cudaFree(stage); return OG_E_NOMEM; }
+    int32_t rc = points_bytes_to_mont(ctx, stage, n, *table);
+    if (rc == OG_OK) rc = msm_build_table(ctx, *table, n, c, n_windows);
+    cudaStreamSynchronize(ctx->stream); cudaFree(stage);
+    return rc;
+}
+
 void pk_free(og_pk* pk) {
     if (!pk) return;
     if (pk->device >= 0) cudaSetDevice(pk->device);    // the key may outlive the context that loaded it
@@ -307,33 +320,9 @@ int32_t pk_load(og_ctx* ctx, const uint8_t* bytes, uint64_t len, og_pk** out) {
     int32_t rc = OG_OK;
     auto fail = [&](int32_t code) { pk_free(pk); return code; };
     if ((rc = clear_flag(ctx)) != OG_OK) return fail(rc);
-    {
-        uint8_t* stage;
-        if ((rc = upload(ctx, &stage, hA.data(), hA.size())) != OG_OK) return fail(rc);
-        if (cudaMalloc(&pk->tabA, sizeof(G1Affine) * (size_t)pk->nA * pk->n_windows[0]) != cudaSuccess) { cudaFree(stage); return fail(OG_E_NOMEM); }
-        rc = g1_bytes_to_mont(ctx, stage, pk->nA, pk->tabA);
-        if (rc == OG_OK) rc = msm_build_table_g1(ctx, pk->tabA, pk->nA, pk->c[0], pk->n_windows[0]);
-        cudaStreamSynchronize(ctx->stream); cudaFree(stage);
-        if (rc != OG_OK) return fail(rc);
-    }
-    {
-        uint8_t* stage;
-        if ((rc = upload(ctx, &stage, hC.data(), hC.size())) != OG_OK) return fail(rc);
-        if (cudaMalloc(&pk->tabC, sizeof(G1Affine) * (size_t)pk->nC * pk->n_windows[2]) != cudaSuccess) { cudaFree(stage); return fail(OG_E_NOMEM); }
-        rc = g1_bytes_to_mont(ctx, stage, pk->nC, pk->tabC);
-        if (rc == OG_OK) rc = msm_build_table_g1(ctx, pk->tabC, pk->nC, pk->c[2], pk->n_windows[2]);
-        cudaStreamSynchronize(ctx->stream); cudaFree(stage);
-        if (rc != OG_OK) return fail(rc);
-    }
-    {
-        uint8_t* stage;
-        if ((rc = upload(ctx, &stage, hB.data(), hB.size())) != OG_OK) return fail(rc);
-        if (cudaMalloc(&pk->tabB, sizeof(G2Affine) * (size_t)pk->nB * pk->n_windows[1]) != cudaSuccess) { cudaFree(stage); return fail(OG_E_NOMEM); }
-        rc = g2_bytes_to_mont(ctx, stage, pk->nB, pk->tabB);
-        if (rc == OG_OK) rc = msm_build_table_g2(ctx, pk->tabB, pk->nB, pk->c[1], pk->n_windows[1]);
-        cudaStreamSynchronize(ctx->stream); cudaFree(stage);
-        if (rc != OG_OK) return fail(rc);
-    }
+    if ((rc = upload_table(ctx, hA, pk->nA, pk->c[0], pk->n_windows[0], &pk->tabA)) != OG_OK) return fail(rc);
+    if ((rc = upload_table(ctx, hC, pk->nC, pk->c[2], pk->n_windows[2], &pk->tabC)) != OG_OK) return fail(rc);
+    if ((rc = upload_table(ctx, hB, pk->nB, pk->c[1], pk->n_windows[1], &pk->tabB)) != OG_OK) return fail(rc);
     if ((rc = upload(ctx, &pk->supp, supp.data(), 4ull * supp.size())) != OG_OK) return fail(rc);
     cudaStreamSynchronize(ctx->stream);
     if ((rc = upload_csr(ctx, rd, pk->n_constraints, nv, &pk->a_ptr, &pk->a_col, &pk->a_val)) != OG_OK) return fail(rc);
@@ -361,29 +350,21 @@ void pk_info(const og_pk* pk, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m
 struct ChunkBufs {
     Fr *W, *rs_m, *abc, *ntt_tmp, *bsc, *csc;
     uint32_t *counts, *offsets, *cursor, *sorted, *heavy;
-    uint32_t *sort_stage, *sort_tiles;    // scratch of the digit sort (msm.cuh): inside bk2 and heavy unless a key outgrows them
-    G1XYZZ *bk1, *lvl1, *totA, *totC;
-    G2XYZZ *bk2, *lvl2, *totB;
-    void *aff1, *aff2;                    // batched-affine scratch (nullptr = XYZZ accumulation): G1 MSMs / G2 MSM
+    uint32_t *sort_stage, *sort_tiles;    // scratch of the digit sort (msm.cuh): inside buckets and heavy unless a key outgrows them
+    void *buckets, *lvl;                  // XYZZ scratch of msm_buckets, sized for G2: the G1 and G2 MSMs of a chunk run one after another
+    G1XYZZ *totA, *totC;
+    G2XYZZ* totB;
     uint32_t w_stride, bsc_stride, csc_stride;
 };
-
-// experiment builds only (-DOG_EXPERIMENT_AFFINE, csrc/experiments/bucket_affine.cuh): OG_AFFINE bit 0 = batched-affine
-// accumulation for the G1 MSMs of the prover, bit 1 = for the G2 MSM.  The shipped library has no such path.
-#ifdef OG_EXPERIMENT_AFFINE
-static uint32_t affine_mode() { return env_u32("OG_AFFINE", 0); }
-#else
-static uint32_t affine_mode() { return 0; }
-#endif
 
 // Bytes of the prover's scratch for `batch` proofs in chunks of B: what one lane allocates for its chunk, and what the
 // batch shares (witness rows, (r, s), per-proof MSM totals).  alloc_chunk allocates exactly these and the chunk rule
 // (prover_plan) budgets with them.
 struct ProverScratch {
-    size_t abc, scalars, sorted, counts, offsets, cursor, heavy, buckets, seg, aff;      // per lane
+    size_t abc, scalars, sorted, counts, offsets, cursor, heavy, buckets, seg;           // per lane
     size_t stage, tiles;   // per lane, 0 when the sort's staging / tile counters fit in the buckets / heavy scratch
     size_t wit, misc, sums;                                                               // per batch
-    size_t lane() const { return abc + scalars + sorted + counts + offsets + cursor + heavy + buckets + seg + aff + stage + tiles; }
+    size_t lane() const { return abc + scalars + sorted + counts + offsets + cursor + heavy + buckets + seg + stage + tiles; }
 };
 
 static ProverScratch prover_scratch(const og_pk* pk, uint32_t batch, uint32_t B) {
@@ -403,9 +384,6 @@ static ProverScratch prover_scratch(const og_pk* pk, uint32_t batch, uint32_t B)
     s.heavy = 4 * (2 * n_keys + 4);
     s.buckets = sizeof(G2XYZZ) * n_keys;
     s.seg = sizeof(G2XYZZ) * msm_lvl_elems(B, pk->max_nb);
-    s.aff = 0;
-    if (affine_mode() & 1) s.aff = msm_aff_scratch_bytes_g1(n_keys);
-    if ((affine_mode() & 2) && msm_aff_scratch_bytes_g2((size_t)B * pk->nb[1]) > s.aff) s.aff = msm_aff_scratch_bytes_g2((size_t)B * pk->nb[1]);
     // The sort's staging lives in the bucket array: nothing writes it before the accumulation of the same MSM, and the
     // previous MSM's reduction, which reads it, runs earlier on the same stream.  Its per-tile counters live in the heavy-bucket
     // scratch, which msm_buckets uses only after the sort.  Only a key that outgrows either gets its own slot.
@@ -434,32 +412,25 @@ static int32_t alloc_chunk(og_ctx* ctx, const og_pk* pk, uint32_t batch, uint32_
     b.offsets = (uint32_t*)ctx->slot(S(S_PR_OFFSETS, S_L1_OFFSETS), s.offsets);
     b.cursor = (uint32_t*)ctx->slot(S(S_PR_CURSOR, S_L1_CURSOR), s.cursor);
     b.heavy = (uint32_t*)ctx->slot(S(S_PR_HEAVY, S_L1_HEAVY), s.heavy);
-    b.bk2 = (G2XYZZ*)ctx->slot(S(S_PR_BUCKETS, S_L1_BUCKETS), s.buckets);
-    b.lvl2 = (G2XYZZ*)ctx->slot(S(S_PR_SEG, S_L1_SEG), s.seg);
+    b.buckets = ctx->slot(S(S_PR_BUCKETS, S_L1_BUCKETS), s.buckets);
+    b.lvl = ctx->slot(S(S_PR_SEG, S_L1_SEG), s.seg);
     b.totA = (G1XYZZ*)ctx->slot(S_PR_SUMS, s.sums);
-    if (!b.W || !b.rs_m || !b.abc || !b.bsc || !b.sorted || !b.counts || !b.offsets || !b.cursor || !b.heavy || !b.bk2 || !b.lvl2 || !b.totA)
+    if (!b.W || !b.rs_m || !b.abc || !b.bsc || !b.sorted || !b.counts || !b.offsets || !b.cursor || !b.heavy || !b.buckets || !b.lvl || !b.totA)
         return OG_E_NOMEM;
-    b.aff1 = b.aff2 = nullptr;
-    if (affine_mode()) {
-        void* a = ctx->slot(S(S_PR_AFF, S_L1_AFF), s.aff);
-        if (!a) return OG_E_NOMEM;
-        if (affine_mode() & 1) b.aff1 = a;
-        if (affine_mode() & 2) b.aff2 = a;
-    }
     b.ntt_tmp = b.abc + (size_t)B * 3 * m;
     b.csc = b.bsc + (size_t)B * b.bsc_stride;
-    b.sort_stage = !s.stage ? (uint32_t*)b.bk2 : (uint32_t*)ctx->slot(S(S_PR_SORT_STAGE, S_L1_SORT_STAGE), s.stage);
+    b.sort_stage = !s.stage ? (uint32_t*)b.buckets : (uint32_t*)ctx->slot(S(S_PR_SORT_STAGE, S_L1_SORT_STAGE), s.stage);
     b.sort_tiles = !s.tiles ? b.heavy : (uint32_t*)ctx->slot(S(S_PR_SORT_TILES, S_L1_SORT_TILES), s.tiles);
     if (!b.sort_stage || !b.sort_tiles) return OG_E_NOMEM;
-    b.bk1 = reinterpret_cast<G1XYZZ*>(b.bk2);       // the G1 and G2 MSMs of a chunk run one after another
-    b.lvl1 = reinterpret_cast<G1XYZZ*>(b.lvl2);
     b.totC = b.totA + batch;
     b.totB = reinterpret_cast<G2XYZZ*>(b.totC + batch);
     return OG_OK;
 }
 
-static int32_t run_msm_g1(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b, uint32_t B, const G1Affine* table, uint32_t n_pts,
-                          const Fr* scalars, uint32_t stride, G1XYZZ* totals) {
+// one of the chunk's three MSMs (which: 0 = A, 1 = B, 2 = C'); they run one after another and share the bucket and level scratch
+template <class F>
+static int32_t run_msm(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b, uint32_t B, const Affine<F>* table, uint32_t n_pts,
+                       const Fr* scalars, uint32_t stride, XYZZ<F>* totals) {
     DigitPlan plan;
     plan.scalars = reinterpret_cast<const uint32_t*>(scalars);
     plan.n = n_pts; plan.scalar_stride = stride; plan.n_problems = B;
@@ -468,19 +439,8 @@ static int32_t run_msm_g1(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b,
     plan.montgomery = 1;
     uint32_t n_keys = B * pk->nb[which];
     OG_TRY(msm_sort_digits(ctx, plan, n_keys, b.counts, b.offsets, nullptr, b.sorted, b.sort_stage, b.sort_tiles));
-    return msm_buckets_g1(ctx, table, b.sorted, b.offsets, b.counts, B, pk->nb[which], (uint64_t)B * n_pts * pk->n_windows[which], b.bk1, b.lvl1, b.heavy, b.cursor, totals, b.aff1);
-}
-static int32_t run_msm_g2(og_ctx* ctx, const og_pk* pk, int which, ChunkBufs& b, uint32_t B, const G2Affine* table, uint32_t n_pts,
-                          const Fr* scalars, uint32_t stride, G2XYZZ* totals) {
-    DigitPlan plan;
-    plan.scalars = reinterpret_cast<const uint32_t*>(scalars);
-    plan.n = n_pts; plan.scalar_stride = stride; plan.n_problems = B;
-    plan.c = pk->c[which]; plan.n_windows = pk->n_windows[which]; plan.nb = pk->nb[which];
-    plan.key_stride_problem = 1; plan.key_stride_window = 0; plan.tidx_window_stride = n_pts;
-    plan.montgomery = 1;
-    uint32_t n_keys = B * pk->nb[which];
-    OG_TRY(msm_sort_digits(ctx, plan, n_keys, b.counts, b.offsets, nullptr, b.sorted, b.sort_stage, b.sort_tiles));
-    return msm_buckets_g2(ctx, table, b.sorted, b.offsets, b.counts, B, pk->nb[which], (uint64_t)B * n_pts * pk->n_windows[which], b.bk2, b.lvl2, b.heavy, b.cursor, totals, b.aff2);
+    return msm_buckets(ctx, table, b.sorted, b.offsets, b.counts, B, pk->nb[which], (uint64_t)B * n_pts * pk->n_windows[which],
+                       static_cast<XYZZ<F>*>(b.buckets), static_cast<XYZZ<F>*>(b.lvl), b.heavy, b.cursor, totals);
 }
 
 // where a chunk's witness rows come from: the statement's witness kernel on its inputs, or the caller's full witnesses
@@ -515,9 +475,9 @@ static int32_t prove_chunk(og_ctx* ctx, const og_pk* pk, ChunkBufs& b, const Wit
     OG_LAUNCH(ctx, k_compose, dim3(mx ? (mx + 127) / 128 : 1, B), 128, 0, W, b.w_stride, rs_m, pk->supp, pk->n_supp, pk->n_vars, pk->n_pub, m,
               b.bsc, b.bsc_stride, b.csc, b.csc_stride);
     OG_LAUNCH(ctx, k_pointwise, dim3((m + 127) / 128, B), 128, 0, b.abc, pk->log_m, B, b.csc, b.csc_stride, n_priv + pk->n_supp);
-    OG_TRY(run_msm_g1(ctx, pk, 0, b, B, pk->tabA, pk->nA, W, b.w_stride, b.totA + off));
-    OG_TRY(run_msm_g1(ctx, pk, 2, b, B, pk->tabC, pk->nC, b.csc, b.csc_stride, b.totC + off));
-    OG_TRY(run_msm_g2(ctx, pk, 1, b, B, pk->tabB, pk->nB, b.bsc, b.bsc_stride, b.totB + off));
+    OG_TRY(run_msm(ctx, pk, 0, b, B, pk->tabA, pk->nA, W, b.w_stride, b.totA + off));
+    OG_TRY(run_msm(ctx, pk, 2, b, B, pk->tabC, pk->nC, b.csc, b.csc_stride, b.totC + off));
+    OG_TRY(run_msm(ctx, pk, 1, b, B, pk->tabB, pk->nB, b.bsc, b.bsc_stride, b.totB + off));
     OG_LAUNCH(ctx, k_assemble_g1, (B + 31) / 32, 32, 0, b.totA + off, b.totC + off, rs_m, B, d_proofs + 256ull * off);
     OG_LAUNCH(ctx, k_assemble_g2, (B + 31) / 32, 32, 0, b.totB + off, B, d_proofs + 256ull * off);
     return OG_OK;

@@ -56,34 +56,19 @@ __global__ void __launch_bounds__(128) k_points_from_mont(const Affine<F>* __res
     FieldIO<F>::store(out + 2 * B * i + B, p.y);
 }
 
-#ifdef OG_MSM_G1
-int32_t g1_bytes_to_mont(og_ctx* ctx, const uint8_t* d_in, uint64_t n, G1Affine* d_out) {
-    if (n) OG_LAUNCH(ctx, k_points_to_mont<Fq>, (unsigned)((n + 127) / 128), 128, 0, d_in, n, d_out, ctx->d_flag);
+// (launch names carry the curve, so that og_profile reports the G1 and the G2 conversions apart)
+template <class F>
+int32_t points_bytes_to_mont(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Affine<F>* d_out) {
+    if (n) OG_LAUNCHN(ctx, sizeof(F) == 32 ? "k_points_to_mont<Fq>" : "k_points_to_mont<Fq2>", k_points_to_mont<F>, (unsigned)((n + 127) / 128), 128, 0,
+                      d_in, n, d_out, ctx->d_flag);
     return OG_OK;
 }
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t g2_bytes_to_mont(og_ctx* ctx, const uint8_t* d_in, uint64_t n, G2Affine* d_out) {
-    if (n) OG_LAUNCH(ctx, k_points_to_mont<Fq2>, (unsigned)((n + 127) / 128), 128, 0, d_in, n, d_out, ctx->d_flag);
+template <class F>
+int32_t points_mont_to_bytes(og_ctx* ctx, const Affine<F>* d_in, uint64_t n, uint8_t* d_out) {
+    if (n) OG_LAUNCHN(ctx, sizeof(F) == 32 ? "k_points_from_mont<Fq>" : "k_points_from_mont<Fq2>", k_points_from_mont<F>, (unsigned)((n + 127) / 128), 128, 0,
+                      d_in, n, d_out);
     return OG_OK;
 }
-#endif  // OG_MSM_G2
-
-#ifdef OG_MSM_G1
-int32_t g1_mont_to_bytes(og_ctx* ctx, const G1Affine* d_in, uint64_t n, uint8_t* d_out) {
-    if (n) OG_LAUNCH(ctx, k_points_from_mont<Fq>, (unsigned)((n + 127) / 128), 128, 0, d_in, n, d_out);
-    return OG_OK;
-}
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t g2_mont_to_bytes(og_ctx* ctx, const G2Affine* d_in, uint64_t n, uint8_t* d_out) {
-    if (n) OG_LAUNCH(ctx, k_points_from_mont<Fq2>, (unsigned)((n + 127) / 128), 128, 0, d_in, n, d_out);
-    return OG_OK;
-}
-#endif  // OG_MSM_G2
-
 
 #ifdef OG_MSM_G1
 // ---- 1/3: digits -> histogram / scatter ---------------------------------------------------------------
@@ -581,11 +566,6 @@ __global__ void __launch_bounds__(128, OG_ACC1_MINB) k_field_probe_g1(int32_t op
     const Fq x = a[i], y = b[i];
     out[i] = op == 0 ? OG_ACC_MUL(x, y) : op == 1 ? OG_ACC_SQR(x) : op == 2 ? x - y : x.dbl();
 }
-int32_t field_probe_raw_g1(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out) {
-    if (n) OG_LAUNCH(ctx, k_field_probe_g1, (unsigned)((n + 127) / 128), 128, 0, op, reinterpret_cast<const Fq*>(d_a),
-                     reinterpret_cast<const Fq*>(d_b), n, reinterpret_cast<Fq*>(d_out));
-    return OG_OK;
-}
 #endif
 
 #ifdef OG_MSM_G2
@@ -665,12 +645,20 @@ __global__ void __launch_bounds__(128, OG_ACC2_MINB) k_field_probe_g2(int32_t op
     }
     out[i] = z;
 }
-int32_t field_probe_raw_g2(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out) {
-    if (n) OG_LAUNCH(ctx, k_field_probe_g2, (unsigned)((n + 127) / 128), 128, 0, op, reinterpret_cast<const Fq2*>(d_a),
-                     reinterpret_cast<const Fq2*>(d_b), n, reinterpret_cast<Fq2*>(d_out));
+#endif
+
+template <class F>
+int32_t field_probe_raw(og_ctx* ctx, int32_t op, const uint8_t* d_a, const uint8_t* d_b, uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    const F *a = reinterpret_cast<const F*>(d_a), *b = reinterpret_cast<const F*>(d_b);
+#ifdef OG_MSM_G1
+    OG_LAUNCH(ctx, k_field_probe_g1, grid, 128, 0, op, a, b, n, reinterpret_cast<F*>(d_out));
+#else
+    OG_LAUNCH(ctx, k_field_probe_g2, grid, 128, 0, op, a, b, n, reinterpret_cast<F*>(d_out));
+#endif
     return OG_OK;
 }
-#endif
 
 // Heavy buckets (lists above the cap: witness-like scalars put 30 % of all points into bucket "1" of window 0) are cut
 // into segments of `seg` entries; every segment gets a CTA, a second kernel adds the partial sums of each bucket.
@@ -753,10 +741,6 @@ __global__ void __launch_bounds__(32) k_heavy_combine(const XYZZ<F>* __restrict_
         __syncwarp();
     }
 }
-
-#ifdef OG_EXPERIMENT_AFFINE
-#include "experiments/bucket_affine.cuh"      // rejected experiment; not in the shipped library
-#endif
 
 constexpr uint32_t RED_FAN_LOG2 = 3, RED_FAN = 1u << RED_FAN_LOG2;   // 8 children per parent: more threads, shorter chains
 // ---- 5: weighted reduction, RED_FAN children per parent -------------------------------------------------------
@@ -979,10 +963,9 @@ __global__ void __launch_bounds__(TAIL_THREADS) k_tail_finish(const XYZZ<F>* __r
 }
 
 template <class F>
-static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t* d_sorted, const uint32_t* d_offsets,
-                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, XYZZ<F>* d_buckets,
-                           XYZZ<F>* d_lvl, uint32_t* d_heavy, uint32_t* d_perm, XYZZ<F>* d_totals, void* aff_scratch = nullptr,
-                           bool few_groups = false) {
+int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t* d_sorted, const uint32_t* d_offsets, const uint32_t* d_counts,
+                    uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, XYZZ<F>* d_buckets, XYZZ<F>* d_lvl, uint32_t* d_heavy,
+                    uint32_t* d_perm, XYZZ<F>* d_totals, bool few_groups) {
     uint32_t n_keys = n_groups * nb;
     constexpr int HT = sizeof(F) == 32 ? 256 : 128;
     OG_CUDA(ctx, cudaMemsetAsync(d_heavy, 0, sizeof(uint32_t), ctx->stream));
@@ -991,11 +974,6 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
     // (skewed scalars: witness 0/1 values, short scalars whose top window has few distinct digits)
     uint64_t avg = n_entries_max / (n_keys ? n_keys : 1);
     uint32_t cap = msm_heavy_cap(avg);
-#ifdef OG_EXPERIMENT_AFFINE
-    if (aff_scratch) {
-        OG_TRY((bucket_acc_affine<F>(ctx, d_table, d_sorted, d_offsets, d_counts, n_keys, cap, avg, d_buckets, d_heavy, d_perm, aff_scratch)));
-    } else
-#endif
     {
         // the long issue-bound kernel of the MSM: on the lane's low-priority stream when the prover runs chunks in flight
         const char* kn = sizeof(F) == 32 ? "k_bucket_acc_g1" : "k_bucket_acc_g2";
@@ -1074,32 +1052,6 @@ static int32_t msm_buckets(og_ctx* ctx, const Affine<F>* d_table, const uint32_t
     return OG_OK;
 }
 
-#ifdef OG_MSM_G1
-int32_t msm_buckets_g1(og_ctx* ctx, const G1Affine* d_table, const uint32_t* d_sorted, const uint32_t* d_offsets,
-                       const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, G1XYZZ* d_buckets,
-                       G1XYZZ* d_lvl, uint32_t* d_heavy, uint32_t* d_perm, G1XYZZ* d_totals, void* aff_scratch) {
-    return msm_buckets<Fq>(ctx, d_table, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, d_buckets, d_lvl, d_heavy, d_perm, d_totals, aff_scratch);
-}
-#ifdef OG_EXPERIMENT_AFFINE
-size_t msm_aff_scratch_bytes_g1(uint64_t n_keys) { return aff_scratch_bytes_t<Fq>(n_keys); }
-#else
-size_t msm_aff_scratch_bytes_g1(uint64_t) { return 0; }
-#endif
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t msm_buckets_g2(og_ctx* ctx, const G2Affine* d_table, const uint32_t* d_sorted, const uint32_t* d_offsets,
-                       const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, G2XYZZ* d_buckets,
-                       G2XYZZ* d_lvl, uint32_t* d_heavy, uint32_t* d_perm, G2XYZZ* d_totals, void* aff_scratch) {
-    return msm_buckets<Fq2>(ctx, d_table, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, d_buckets, d_lvl, d_heavy, d_perm, d_totals, aff_scratch);
-}
-#ifdef OG_EXPERIMENT_AFFINE
-size_t msm_aff_scratch_bytes_g2(uint64_t n_keys) { return aff_scratch_bytes_t<Fq2>(n_keys); }
-#else
-size_t msm_aff_scratch_bytes_g2(uint64_t) { return 0; }
-#endif
-#endif  // OG_MSM_G2
-
 // ---- test/debug probe (og_msm_bucket_sums): msm_buckets on bucket lists the caller gives -------------------------------------
 template <class F>
 __global__ void __launch_bounds__(128) k_xyzz_to_bytes(const XYZZ<F>* __restrict__ in, uint64_t n, uint8_t* __restrict__ out) {
@@ -1113,9 +1065,9 @@ __global__ void __launch_bounds__(128) k_xyzz_to_bytes(const XYZZ<F>* __restrict
 }
 
 template <class F>
-static int32_t msm_bucket_sums_t(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted,
-                                 const uint32_t* d_offsets, const uint32_t* d_counts, uint32_t n_groups, uint32_t nb,
-                                 uint64_t n_entries_max, bool few_groups, uint8_t* d_out_totals, uint8_t* d_out_buckets) {
+int32_t msm_bucket_sums(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
+                        const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
+                        uint8_t* d_out_totals, uint8_t* d_out_buckets) {
     const uint32_t n_keys = n_groups * nb;
     OG_SLOT(ctx, pts, Affine<F>, S_MSM_POINTS, sizeof(Affine<F>) * (size_t)n_points);
     OG_SLOT(ctx, buckets, XYZZ<F>, S_MSM_BUCKETS, sizeof(XYZZ<F>) * (size_t)n_keys);
@@ -1125,30 +1077,12 @@ static int32_t msm_bucket_sums_t(og_ctx* ctx, const uint8_t* d_points, uint32_t 
     OG_SLOT(ctx, totals, XYZZ<F>, S_MSM_OUT, sizeof(XYZZ<F>) * (size_t)n_groups);
     if (n_points) OG_LAUNCH(ctx, k_points_to_mont<F>, (n_points + 127) / 128, 128, 0, d_points, (uint64_t)n_points, pts, ctx->d_flag);
     OG_TRY((msm_buckets<F>(ctx, pts, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, buckets, lvl, heavy, perm, totals,
-                           nullptr, few_groups)));
+                           few_groups)));
     OG_LAUNCH(ctx, k_xyzz_to_bytes<F>, (n_groups + 127) / 128, 128, 0, totals, (uint64_t)n_groups, d_out_totals);
     // the buckets as the reduction read them: accumulated, heavy ones combined
     if (d_out_buckets) OG_LAUNCH(ctx, k_xyzz_to_bytes<F>, (n_keys + 127) / 128, 128, 0, buckets, (uint64_t)n_keys, d_out_buckets);
     return OG_OK;
 }
-
-#ifdef OG_MSM_G1
-int32_t msm_bucket_sums_g1(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
-                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
-                           uint8_t* d_out_totals, uint8_t* d_out_buckets) {
-    return msm_bucket_sums_t<Fq>(ctx, d_points, n_points, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, few_groups,
-                                 d_out_totals, d_out_buckets);
-}
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t msm_bucket_sums_g2(og_ctx* ctx, const uint8_t* d_points, uint32_t n_points, const uint32_t* d_sorted, const uint32_t* d_offsets,
-                           const uint32_t* d_counts, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, bool few_groups,
-                           uint8_t* d_out_totals, uint8_t* d_out_buckets) {
-    return msm_bucket_sums_t<Fq2>(ctx, d_points, n_points, d_sorted, d_offsets, d_counts, n_groups, nb, n_entries_max, few_groups,
-                                  d_out_totals, d_out_buckets);
-}
-#endif  // OG_MSM_G2
 
 
 // ---- 6: one-shot MSM = Horner over the window totals ------------------------------------------------------
@@ -1261,7 +1195,7 @@ static uint32_t pick_window(uint64_t n) {
 }
 
 template <class F>
-static int32_t msm_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_scalars, uint64_t n, uint8_t* d_out) {
+int32_t msm_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_scalars, uint64_t n, uint8_t* d_out) {
     constexpr int PB = 2 * FieldIO<F>::BYTES;
     if (n >= (1ull << 28)) return OG_E_INVALID;
     if (!aligned32(d_points) || !aligned32(d_scalars)) return OG_E_INVALID;
@@ -1301,29 +1235,10 @@ static int32_t msm_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_sc
     plan.key_stride_problem = 0; plan.key_stride_window = 1; plan.tidx_window_stride = 0;
     plan.montgomery = 0;
     OG_TRY(msm_sort_digits(ctx, plan, n_keys, counts, offsets, cursor, sorted));
-    void* aff = nullptr;
-#ifdef OG_EXPERIMENT_AFFINE
-    {   // OG_AFFINE_ONESHOT=1 routes one-shot MSMs through the experiment so that the edge-case tests exercise it
-        const char* v = getenv("OG_AFFINE_ONESHOT");
-        if (v && atoi(v) > 0) { aff = ctx->slot(S_MSM_AFF, aff_scratch_bytes_t<F>(n_keys)); if (!aff) return OG_E_NOMEM; }
-    }
-#endif
-    OG_TRY((msm_buckets<F>(ctx, pts, sorted, offsets, counts, W, nb, n * W, buckets, lvl, heavy, cursor, totals, aff, true)));
+    OG_TRY((msm_buckets<F>(ctx, pts, sorted, offsets, counts, W, nb, n * W, buckets, lvl, heavy, cursor, totals, true)));
     OG_LAUNCH(ctx, k_horner<F>, 1, 128, 0, totals, W, c, d_out);
     return OG_OK;
 }
-
-#ifdef OG_MSM_G1
-int32_t msm_g1_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_scalars, uint64_t n, uint8_t* d_out64) {
-    return msm_dev<Fq>(ctx, d_points, d_scalars, n, d_out64);
-}
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t msm_g2_dev(og_ctx* ctx, const uint8_t* d_points, const uint8_t* d_scalars, uint64_t n, uint8_t* d_out128) {
-    return msm_dev<Fq2>(ctx, d_points, d_scalars, n, d_out128);
-}
-#endif  // OG_MSM_G2
 
 
 // ---- plain sum of affine points (post all-gather combine in the sharded MSM) ------------------------------------
@@ -1351,22 +1266,12 @@ __global__ void __launch_bounds__(THREADS) k_sum_points(const uint8_t* __restric
         FieldIO<F>::store(out + B, a.y);
     }
 }
-#ifdef OG_MSM_G1
-int32_t sum_g1_dev(og_ctx* ctx, const uint8_t* d_points, uint64_t n, uint8_t* d_out64) {
-    auto k = k_sum_points<Fq, 128>;
-    OG_LAUNCH(ctx, k, 1, 128, 128 * sizeof(G1XYZZ), d_points, n, d_out64, ctx->d_flag);
+template <class F>
+int32_t sum_dev(og_ctx* ctx, const uint8_t* d_points, uint64_t n, uint8_t* d_out) {
+    auto k = k_sum_points<F, 128>;
+    OG_LAUNCH(ctx, k, 1, 128, 128 * sizeof(XYZZ<F>), d_points, n, d_out, ctx->d_flag);
     return OG_OK;
 }
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t sum_g2_dev(og_ctx* ctx, const uint8_t* d_points, uint64_t n, uint8_t* d_out128) {
-    auto k = k_sum_points<Fq2, 128>;
-    OG_LAUNCH(ctx, k, 1, 128, 128 * sizeof(G2XYZZ), d_points, n, d_out128, ctx->d_flag);
-    return OG_OK;
-}
-#endif  // OG_MSM_G2
-
 
 // ---- fixed-base window tables ------------------------------------------------------------------------------------
 template <class F>
@@ -1381,20 +1286,11 @@ __global__ void __launch_bounds__(64) k_build_table(Affine<F>* __restrict__ tabl
         table[(size_t)w * n + i] = p;
     }
 }
-#ifdef OG_MSM_G1
-int32_t msm_build_table_g1(og_ctx* ctx, G1Affine* d_table, uint32_t n, uint32_t c, uint32_t n_windows) {
-    if (n) OG_LAUNCH(ctx, k_build_table<Fq>, (n + 63) / 64, 64, 0, d_table, n, c, n_windows);
+template <class F>
+int32_t msm_build_table(og_ctx* ctx, Affine<F>* d_table, uint32_t n, uint32_t c, uint32_t n_windows) {
+    if (n) OG_LAUNCHN(ctx, sizeof(F) == 32 ? "k_build_table<Fq>" : "k_build_table<Fq2>", k_build_table<F>, (n + 63) / 64, 64, 0, d_table, n, c, n_windows);
     return OG_OK;
 }
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t msm_build_table_g2(og_ctx* ctx, G2Affine* d_table, uint32_t n, uint32_t c, uint32_t n_windows) {
-    if (n) OG_LAUNCH(ctx, k_build_table<Fq2>, (n + 63) / 64, 64, 0, d_table, n, c, n_windows);
-    return OG_OK;
-}
-#endif  // OG_MSM_G2
-
 
 // ---- fixed-base multiplication by the generators (development setup only) ------------------------------------------
 // gen_table[w * 255 + d - 1] = d * 2^(8w) * G,  w < 32, d in 1..255
@@ -1433,42 +1329,50 @@ __global__ void __launch_bounds__(128) k_fixed_mul(const Affine<F>* __restrict__
     out[i] = r;
 }
 
+template <class F> static Affine<F> generator();
+#ifdef OG_MSM_G1
+template <> Affine<Fq> generator<Fq>() { return {Fq::from_u32(1), Fq::from_u32(2)}; }
+#endif
 #ifdef OG_MSM_G2
 static const uint32_t G2_GEN_X0[8] = {0xd992f6edu, 0x46debd5cu, 0xf75edaddu, 0x674322d4u, 0x5e5c4479u, 0x426a0066u, 0x121f1e76u, 0x1800deefu};
 static const uint32_t G2_GEN_X1[8] = {0xaef312c2u, 0x97e485b7u, 0x35a9e712u, 0xf1aa4933u, 0x31fb5d25u, 0x7260bfb7u, 0x920d483au, 0x198e9393u};
 static const uint32_t G2_GEN_Y0[8] = {0x66fa7daau, 0x4ce6cc01u, 0x0c43d37bu, 0xe3d1e769u, 0x8dcb408fu, 0x4aab7180u, 0xdb8c6debu, 0x12c85ea5u};
 static const uint32_t G2_GEN_Y1[8] = {0xd122975bu, 0x55acdadcu, 0x70b38ef3u, 0xbc4b3133u, 0x690c3395u, 0xec9e99adu, 0x585ff075u, 0x090689d0u};
-#endif  // OG_MSM_G2
+template <> Affine<Fq2> generator<Fq2>() {
+    return {Fq2{Fq::from_canonical(G2_GEN_X0), Fq::from_canonical(G2_GEN_X1)}, Fq2{Fq::from_canonical(G2_GEN_Y0), Fq::from_canonical(G2_GEN_Y1)}};
+}
+#endif
 
+template <class F>
+int32_t fixed_base_mul(og_ctx* ctx, const uint8_t* d_scalars, uint64_t n, Affine<F>* d_out) {
+    void*& fixed = sizeof(F) == 32 ? ctx->g1_fixed : ctx->g2_fixed;
+    if (!fixed) {
+        Affine<F>* tab;
+        OG_CUDA(ctx, cudaMalloc(&tab, sizeof(Affine<F>) * 32 * 255));
+        OG_LAUNCHN(ctx, sizeof(F) == 32 ? "k_gen_table<Fq>" : "k_gen_table<Fq2>", k_gen_table<F>, 1, 32, 0, generator<F>(), tab);
+        fixed = tab;
+    }
+    if (n) OG_LAUNCHN(ctx, sizeof(F) == 32 ? "k_fixed_mul<Fq>" : "k_fixed_mul<Fq2>", k_fixed_mul<F>, (unsigned)((n + 127) / 128), 128, 0,
+                      (const Affine<F>*)fixed, d_scalars, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
 
+// ---- the interface of msm.cuh, for this unit's curve ----------------------------------------------------------------------------------
 #ifdef OG_MSM_G1
-int32_t fixed_base_mul_g1(og_ctx* ctx, const uint8_t* d_scalars, uint64_t n, G1Affine* d_out) {
-    if (!ctx->g1_fixed) {
-        G1Affine* tab;
-        OG_CUDA(ctx, cudaMalloc(&tab, sizeof(G1Affine) * 32 * 255));
-        G1Affine gen{Fq::from_u32(1), Fq::from_u32(2)};
-        OG_LAUNCH(ctx, k_gen_table<Fq>, 1, 32, 0, gen, tab);
-        ctx->g1_fixed = tab;
-    }
-    if (n) OG_LAUNCH(ctx, k_fixed_mul<Fq>, (unsigned)((n + 127) / 128), 128, 0, (const G1Affine*)ctx->g1_fixed, d_scalars, n, d_out, ctx->d_flag);
-    return OG_OK;
-}
-#endif  // OG_MSM_G1
-
-#ifdef OG_MSM_G2
-int32_t fixed_base_mul_g2(og_ctx* ctx, const uint8_t* d_scalars, uint64_t n, G2Affine* d_out) {
-    if (!ctx->g2_fixed) {
-        G2Affine* tab;
-        OG_CUDA(ctx, cudaMalloc(&tab, sizeof(G2Affine) * 32 * 255));
-        G2Affine gen{Fq2{Fq::from_canonical(G2_GEN_X0), Fq::from_canonical(G2_GEN_X1)},
-                     Fq2{Fq::from_canonical(G2_GEN_Y0), Fq::from_canonical(G2_GEN_Y1)}};
-        OG_LAUNCH(ctx, k_gen_table<Fq2>, 1, 32, 0, gen, tab);
-        ctx->g2_fixed = tab;
-    }
-    if (n) OG_LAUNCH(ctx, k_fixed_mul<Fq2>, (unsigned)((n + 127) / 128), 128, 0, (const G2Affine*)ctx->g2_fixed, d_scalars, n, d_out, ctx->d_flag);
-    return OG_OK;
-}
-#endif  // OG_MSM_G2
-
+using UnitField = Fq;
+#else
+using UnitField = Fq2;
+#endif
+template int32_t msm_buckets<UnitField>(og_ctx*, const Affine<UnitField>*, const uint32_t*, const uint32_t*, const uint32_t*, uint32_t, uint32_t,
+                                        uint64_t, XYZZ<UnitField>*, XYZZ<UnitField>*, uint32_t*, uint32_t*, XYZZ<UnitField>*, bool);
+template int32_t msm_bucket_sums<UnitField>(og_ctx*, const uint8_t*, uint32_t, const uint32_t*, const uint32_t*, const uint32_t*, uint32_t, uint32_t,
+                                            uint64_t, bool, uint8_t*, uint8_t*);
+template int32_t field_probe_raw<UnitField>(og_ctx*, int32_t, const uint8_t*, const uint8_t*, uint64_t, uint8_t*);
+template int32_t msm_dev<UnitField>(og_ctx*, const uint8_t*, const uint8_t*, uint64_t, uint8_t*);
+template int32_t sum_dev<UnitField>(og_ctx*, const uint8_t*, uint64_t, uint8_t*);
+template int32_t points_bytes_to_mont<UnitField>(og_ctx*, const uint8_t*, uint64_t, Affine<UnitField>*);
+template int32_t points_mont_to_bytes<UnitField>(og_ctx*, const Affine<UnitField>*, uint64_t, uint8_t*);
+template int32_t msm_build_table<UnitField>(og_ctx*, Affine<UnitField>*, uint32_t, uint32_t, uint32_t);
+template int32_t fixed_base_mul<UnitField>(og_ctx*, const uint8_t*, uint64_t, Affine<UnitField>*);
 
 }  // namespace og

@@ -2,7 +2,7 @@
 // the clear": tau, alpha, beta, gamma, delta are inputs, so that every pk/vk byte is reproducible and
 // can be compared with oracle/groth16.py).  A production deployment would load a ceremony's key with
 // og_load_pk instead.  QAP evaluation at tau is ~10^5 host field operations for the depth-32 withdraw key;
-// its ~1.6*10^5 fixed-base scalar multiplications run on the GPU (msm.cu: fixed_base_mul_*).
+// its ~1.6*10^5 fixed-base scalar multiplications run on the GPU (msm.cu: fixed_base_mul).
 // Conventions: DESIGN.md section 4 (domain, input-consistency rows, coset-Lagrange H query).
 #include "groth16.cuh"
 #include "msm.cuh"
@@ -146,13 +146,13 @@ static int32_t setup_r1cs(og_ctx* ctx, const R1cs& cs, uint32_t depth, const uin
     OG_SLOT(ctx, d_bytes, uint8_t, S_SETUP_C, 128 * (n1 > n2 ? n1 : n2));
     std::vector<uint8_t> p1(64 * n1), p2(128 * n2);
     OG_CUDA(ctx, cudaMemcpyAsync(d_s, s1.data(), 32 * n1, cudaMemcpyHostToDevice, ctx->stream));
-    OG_TRY(fixed_base_mul_g1(ctx, d_s, n1, reinterpret_cast<G1Affine*>(d_pts)));
-    OG_TRY(g1_mont_to_bytes(ctx, reinterpret_cast<G1Affine*>(d_pts), n1, d_bytes));
+    OG_TRY(fixed_base_mul(ctx, d_s, n1, reinterpret_cast<G1Affine*>(d_pts)));
+    OG_TRY(points_mont_to_bytes(ctx, reinterpret_cast<G1Affine*>(d_pts), n1, d_bytes));
     OG_CUDA(ctx, cudaMemcpyAsync(p1.data(), d_bytes, 64 * n1, cudaMemcpyDeviceToHost, ctx->stream));
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     OG_CUDA(ctx, cudaMemcpyAsync(d_s, s2.data(), 32 * n2, cudaMemcpyHostToDevice, ctx->stream));
-    OG_TRY(fixed_base_mul_g2(ctx, d_s, n2, reinterpret_cast<G2Affine*>(d_pts)));
-    OG_TRY(g2_mont_to_bytes(ctx, reinterpret_cast<G2Affine*>(d_pts), n2, d_bytes));
+    OG_TRY(fixed_base_mul(ctx, d_s, n2, reinterpret_cast<G2Affine*>(d_pts)));
+    OG_TRY(points_mont_to_bytes(ctx, reinterpret_cast<G2Affine*>(d_pts), n2, d_bytes));
     OG_CUDA(ctx, cudaMemcpyAsync(p2.data(), d_bytes, 128 * n2, cudaMemcpyDeviceToHost, ctx->stream));
     OG_TRY(check_flag(ctx));
 
