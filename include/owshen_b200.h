@@ -235,6 +235,27 @@ int32_t og_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nulli
                                const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
                                const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses);
 
+/* ---- the exclusion withdraw statement (DESIGN.md section 3): a note in the pool and not on a published blocklist ---- */
+/* Public inputs (root, nullifier_hash, recipient, exclusion_root); the first three are the withdraw statement's.  A
+ * provider's blocklist names pool leaf indices i_1 < ... < i_n; its tree (same depth as the pool's, 1..32) has leaf
+ * j = MultiMiMC7([k_j, k_{j+1}], 0) over the keys k_0 = 0, k_j = i_j + 1, k_{n+1} = 2^32 + 1.  The note's commitment reaches
+ * root along the pool path, its index i (the path bits) satisfies excl_low < i + 1 < excl_next (33-bit range checks), and the
+ * leaf of (excl_low, excl_next) reaches exclusion_root along the exclusion path.  At depth 32: 48 812 variables,
+ * 48 746 constraints, domain 2^16. */
+int32_t og_exclusion_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_exclusion_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                 uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: nullifier, secret, recipient 32 B each; siblings
+ * and excl_siblings depth * 32 B each (leaf level first); path_bits and excl_path_bits one word each (bit l set when the
+ * level-l node is a right child; only the low depth bits count); excl_low and excl_next one uint64 each.  Both roots are
+ * derived from the paths; a flagged note, a leaf that does not bracket the note, or a key of 2^33 or more gives a witness
+ * that does not satisfy the R1CS. */
+int32_t og_exclusion_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifiers, const uint8_t* secrets,
+                             const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
+                             const uint64_t* excl_low, const uint64_t* excl_next, const uint8_t* excl_siblings,
+                             const uint32_t* excl_path_bits, uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -310,6 +331,20 @@ int32_t og_groth16_prove_association_dev(og_ctx* ctx, const og_pk* pk, const uin
                                          const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits,
                                          const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
                                          const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of exclusion withdraw proofs, witness generation on the GPU; inputs as in og_exclusion_witness.  OG_E_INVALID
+ * unless the key has an exclusion statement's shape (the depth is recognised from it).  public_out (optional):
+ * batch * 4 * 32 B = root, nullifier_hash, recipient, exclusion_root. */
+int32_t og_groth16_prove_exclusion(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets,
+                                   const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits,
+                                   const uint64_t* excl_low, const uint64_t* excl_next, const uint8_t* excl_siblings,
+                                   const uint32_t* excl_path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
+                                   uint8_t* public_out);
+/* same with every buffer already in HBM; no synchronisation */
+int32_t og_groth16_prove_exclusion_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                       const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits,
+                                       const uint64_t* d_excl_low, const uint64_t* d_excl_next, const uint8_t* d_excl_siblings,
+                                       const uint32_t* d_excl_path_bits, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
+                                       uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

@@ -7,6 +7,7 @@ little-endian (/root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.r
 All hashing, witness generation, NTTs and MSMs run in the CUDA library; nothing here computes.
 """
 import array
+import bisect
 import ctypes as C
 import os
 import secrets as _rand
@@ -102,6 +103,9 @@ _SIGS = {
     "og_association_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_association_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_association_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p]),
+    "og_exclusion_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_exclusion_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_exclusion_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -118,6 +122,8 @@ _SIGS = {
     "og_groth16_prove_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_association": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_association_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_exclusion": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_exclusion_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -234,6 +240,9 @@ _STATEMENTS = {
                         ("out_amounts", 16, 0, _u64_array))),
     "association": (True, (("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("recipients", 32, 0, None), ("siblings", 0, 32, None),
                            ("path_bits", 4, 0, _u32_array), ("assoc_siblings", 0, 32, None), ("assoc_path_bits", 4, 0, _u32_array))),
+    "exclusion": (True, (("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("recipients", 32, 0, None), ("siblings", 0, 32, None),
+                         ("path_bits", 4, 0, _u32_array), ("excl_low", 8, 0, _u64_array), ("excl_next", 8, 0, _u64_array),
+                         ("excl_siblings", 0, 32, None), ("excl_path_bits", 4, 0, _u32_array))),
 }
 
 
@@ -578,6 +587,16 @@ class Context:
         return self._statement_witness("association", depth, (nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings,
                                                               assoc_path_bits))
 
+    def exclusion_witness(self, depth, nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings,
+                          excl_path_bits) -> bytes:
+        """Full assignments of the depth-`depth` exclusion withdraw statement, n_vars * 32 bytes per proof, computed on the
+        GPU.  Per proof: nullifier, secret, recipient 32 bytes each; siblings and excl_siblings depth elements each (the pool
+        path and the blocklist-tree path, leaf level first); path_bits and excl_path_bits one word each; excl_low and
+        excl_next one uint64 each (8-byte little-endian buffers, uint64 arrays or ints), the keys of the blocklist leaf that
+        brackets the note (ExclusionSet.witness)."""
+        return self._statement_witness("exclusion", depth, (nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next,
+                                                            excl_siblings, excl_path_bits))
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -641,6 +660,15 @@ def association_r1cs_export(depth: int, which: str):
     return _statement_r1cs_export("association", depth, which)
 
 
+def exclusion_r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("exclusion", depth)
+
+
+def exclusion_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` exclusion R1CS."""
+    return _statement_r1cs_export("exclusion", depth, which)
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -694,6 +722,12 @@ def setup_association(ctx: Context, depth: int, tau: int, alpha: int, beta: int,
     """Development setup of the depth-`depth` association-set withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS
     through setup_r1cs.  The key records depth 0; the prover recognises it as an association key by its shape."""
     return _setup_statement(ctx, "association", depth, (tau, alpha, beta, gamma, delta))
+
+
+def setup_exclusion(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` exclusion withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS through
+    setup_r1cs.  The key records depth 0; the prover recognises it as an exclusion key by its shape."""
+    return _setup_statement(ctx, "exclusion", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -774,6 +808,10 @@ def ptau_prepare_transfer(ctx: Context, acc: bytes, depth: int):
 
 def ptau_prepare_association(ctx: Context, acc: bytes, depth: int):
     return _ptau_prepare_statement(ctx, acc, "association", depth)
+
+
+def ptau_prepare_exclusion(ctx: Context, acc: bytes, depth: int):
+    return _ptau_prepare_statement(ctx, acc, "exclusion", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -898,6 +936,20 @@ class ProvingKey:
         association_root) per proof."""
         return self._prove_statement("association", self.association_depth,
                                      (nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits), rs, want_public)
+
+    @property
+    def exclusion_depth(self):
+        """The depth d whose exclusion statement has this key's shape (exclusion_r1cs_info), or None."""
+        return self._shape_depth("exclusion")
+
+    def prove_exclusion(self, nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings, excl_path_bits,
+                        rs, want_public=True):
+        """Batch of exclusion withdraw proofs from the secret inputs (witness generation on the GPU).  Inputs as in
+        Context.exclusion_witness; returns (proofs, public_inputs) with public inputs (root, nullifier_hash, recipient,
+        exclusion_root) per proof."""
+        return self._prove_statement("exclusion", self.exclusion_depth,
+                                     (nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings,
+                                      excl_path_bits), rs, want_public)
 
     def prover_plan(self, batch: int) -> dict:
         """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and
@@ -1077,3 +1129,51 @@ class MerkleTree:
         len(indices) x depth x 32 bytes, proof-major, and one path_bits word per leaf."""
         got = [self.path(i) for i in indices]
         return b"".join(s for s, _ in got), [b for _, b in got]
+
+
+EXCLUSION_KEY_MAX = (1 << 32) + 1        # the blocklist tree's last key: above every note key (leaf index + 1 <= 2^32)
+
+
+class ExclusionSet:
+    """A compliance provider's blocklist of pool leaf indices as the exclusion statement's tree (DESIGN.md section 3).
+
+    The flagged indices i_1 < ... < i_n (validated, sorted, deduplicated; each below 2^depth, at most 2^depth - 1 of them)
+    give the keys k_0 = 0, k_j = i_j + 1, k_{n+1} = 2^32 + 1 and the leaves MultiMiMC7([k_j, k_{j+1}], 0), j = 0..n, in one
+    og_mimc7_hash2 call; one MerkleTree.insert_batch of the pool's depth builds the tree on the GPU.  A new blocklist version
+    is a new ExclusionSet.  witness(indices) gives what prove_exclusion takes for unflagged notes."""
+
+    def __init__(self, ctx: Context, depth: int, flagged_indices, store=None):
+        _need(1 <= depth <= 32, "ExclusionSet: depth must be in 1..32")
+        flagged = sorted(set(int(i) for i in flagged_indices))
+        _need(not flagged or (flagged[0] >= 0 and flagged[-1] < 1 << depth),
+              f"ExclusionSet: flagged indices are pool leaf indices in [0, 2^{depth})")
+        _need(len(flagged) < 1 << depth, f"ExclusionSet: a depth-{depth} tree holds at most 2^{depth} - 1 flagged indices")
+        self.depth, self.flagged = depth, flagged
+        self.keys = [0] + [i + 1 for i in flagged] + [EXCLUSION_KEY_MAX]
+        self._flagged_set = frozenset(flagged)
+        self.tree = MerkleTree(ctx, depth, store, prefix=b"xs/")
+        _need(self.tree.n_leaves == 0, "ExclusionSet: the store already holds a blocklist tree")
+        enc = lambda ks: b"".join(k.to_bytes(32, "little") for k in ks)
+        leaves = ctx.mimc7_hash2(enc(self.keys[:-1]), enc(self.keys[1:]))
+        self.tree.insert_batch([leaves[32 * j:32 * j + 32] for j in range(len(self.keys) - 1)])
+
+    def root(self) -> bytes:
+        return self.tree.root()
+
+    def __contains__(self, index) -> bool:
+        return index in self._flagged_set
+
+    def __len__(self) -> int:
+        return len(self.flagged)
+
+    def witness(self, indices):
+        """(excl_low, excl_next, excl_siblings, excl_path_bits) for the notes at pool leaf `indices`: the keys of the leaf
+        that brackets each (lists of ints), its paths (len(indices) x depth x 32 bytes) and path words.  ValueError names
+        any flagged index."""
+        indices = [int(i) for i in indices]
+        _need(all(0 <= i < 1 << self.depth for i in indices), f"ExclusionSet.witness: indices must be in [0, 2^{self.depth})")
+        bad = sorted(set(i for i in indices if i in self._flagged_set))
+        _need(not bad, f"ExclusionSet.witness: pool leaves {bad} are on the blocklist")
+        js = [bisect.bisect_left(self.keys, i + 1) - 1 for i in indices]
+        sibs, bits = self.tree.paths(js)
+        return [self.keys[j] for j in js], [self.keys[j + 1] for j in js], sibs, bits

@@ -976,6 +976,20 @@ int32_t og_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nulli
                                                           assoc_path_bits}, batch, witnesses);
 }
 
+// ---- exclusion withdraw statement ----------------------------------------------------------------------------------
+int32_t og_exclusion_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_EXCLUSION, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_exclusion_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    return statement_r1cs_export(ST_EXCLUSION, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
+int32_t og_exclusion_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifiers, const uint8_t* secrets, const uint8_t* recipients,
+                             const uint8_t* siblings, const uint32_t* path_bits, const uint64_t* excl_low, const uint64_t* excl_next,
+                             const uint8_t* excl_siblings, const uint32_t* excl_path_bits, uint32_t batch, uint8_t* witnesses) {
+    return statement_witness(ctx, ST_EXCLUSION, depth, {nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next,
+                                                        excl_siblings, excl_path_bits}, batch, witnesses);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1091,6 +1105,23 @@ int32_t og_groth16_prove_association(og_ctx* ctx, const og_pk* pk, const uint8_t
                                      uint8_t* proofs, uint8_t* public_out) {
     return statement_prove(ctx, pk, ST_ASSOCIATION, {nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits},
                            batch, rs, proofs, public_out);
+}
+
+int32_t og_groth16_prove_exclusion_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                       const uint8_t* d_recipients, const uint8_t* d_siblings, const uint32_t* d_path_bits,
+                                       const uint64_t* d_excl_low, const uint64_t* d_excl_next, const uint8_t* d_excl_siblings,
+                                       const uint32_t* d_excl_path_bits, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
+                                       uint8_t* d_public_out) {
+    return statement_prove_dev(ctx, pk, ST_EXCLUSION, {d_nullifiers, d_secrets, d_recipients, d_siblings, d_path_bits, d_excl_low,
+                                                       d_excl_next, d_excl_siblings, d_excl_path_bits}, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_exclusion(og_ctx* ctx, const og_pk* pk, const uint8_t* nullifiers, const uint8_t* secrets,
+                                   const uint8_t* recipients, const uint8_t* siblings, const uint32_t* path_bits, const uint64_t* excl_low,
+                                   const uint64_t* excl_next, const uint8_t* excl_siblings, const uint32_t* excl_path_bits, uint32_t batch,
+                                   const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
+    return statement_prove(ctx, pk, ST_EXCLUSION, {nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings,
+                                                   excl_path_bits}, batch, rs, proofs, public_out);
 }
 
 int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {

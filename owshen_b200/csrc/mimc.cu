@@ -1,6 +1,6 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
 // paths (BASELINE config 2), level-by-level tree build, and the witness generators of the withdraw,
-// deposit, transfer and association statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
+// deposit, transfer, association and exclusion statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -120,7 +120,7 @@ __global__ void __launch_bounds__(32) k_merkle_paths(const uint8_t* __restrict__
 
 // The witness of a Merkle path from the leaf `cur`: `depth` level blocks (sibling, bit, left, perm1[perm], perm2[perm], out)
 // written from v on, lvl_size elements apart, with the siblings from sp (32 B canonical each) and bit l of `bits` set when
-// the node is a right child.  Returns the root.  Shared by the withdraw, transfer and association witness kernels.
+// the node is a right child.  Returns the root.  Shared by the withdraw, transfer, association and exclusion witness kernels.
 __device__ __forceinline__ Fr witness_path(Fr cur, Fr* v, uint32_t depth, uint32_t lvl_size, uint32_t perm, const uint8_t* sp,
                                            uint32_t bits, int* flag) {
     const Fr one = Fr::one();
@@ -249,6 +249,23 @@ __global__ void __launch_bounds__(128) k_transfer_witness(TransferLayout L, uint
     }
 }
 
+// The withdraw chain of the association and exclusion statements, whose rows share its variables: ONE, recipient (3),
+// nullifier (5), secret (6), recipient_sq (7), the nullifier hash (2) with its permutation just below the commitment block,
+// the commitment with its round values, the pool path from L.pool_base, root (1).
+template <class Layout>
+__device__ __forceinline__ void withdraw_chain_witness(const Layout& L, Fr* w, const Fr& nu, const Fr& se, const uint8_t* recipient,
+                                                       const uint8_t* sp, uint32_t bits, int* flag) {
+    Fr re = load_canonical<Fr>(recipient, flag);
+    Fr one = Fr::one();
+    w[0] = one; w[3] = re; w[5] = nu; w[6] = se;
+    w[7] = re.sqr();
+    // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
+    w[2] = one + nu + mimc7_hash<true>(nu, one, w + L.cm_base - L.perm);
+    Fr cm = mimc7_hash2<true>(nu, se, w + L.cm_base, w + L.cm_base + L.perm);
+    w[L.cm_out] = cm;
+    w[1] = witness_path(cm, w + L.pool_base, L.depth, L.lvl_size, L.perm, sp, bits, flag);
+}
+
 // Witness of the association-set withdraw statement, layout of DESIGN.md section 3 (== oracle/association_circuit.py); row p
 // starts at W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with two warps, one per independent chain of a proof,
 // so no warp diverges and a proof's critical path stays at about one withdraw path:
@@ -264,19 +281,63 @@ __global__ void __launch_bounds__(64) k_association_witness(AssociationLayout L,
     Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
     Fr se = load_canonical<Fr>(in.secrets + 32ull * p, flag);
     if (role == 0) {
-        Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
-        Fr one = Fr::one();
-        w[0] = one; w[3] = re; w[5] = nu; w[6] = se;
-        w[7] = re.sqr();
-        // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
-        w[2] = one + nu + mimc7_hash<true>(nu, one, w + 8);
-        Fr cm = mimc7_hash2<true>(nu, se, w + L.cm_base, w + L.cm_base + L.perm);
-        w[L.cm_out] = cm;
-        w[1] = witness_path(cm, w + L.pool_base, L.depth, L.lvl_size, L.perm, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
+        withdraw_chain_witness(L, w, nu, se, in.recipients + 32ull * p, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
     } else {
         Fr cm = mimc7_hash2<false>(nu, se, nullptr, nullptr);
         w[4] = witness_path(cm, w + L.assoc_base, L.depth, L.lvl_size, L.perm, in.assoc_siblings + 32ull * L.depth * p,
                             in.assoc_path_bits[p], flag);
+    }
+}
+
+// the 33 low bits of the canonical representative of (a - b - 1) mod r, for a, b < 2^64: when a <= b the difference is
+// r - (b + 1 - a), whose low 64 bits are r's low 64 bits minus (b + 1 - a), all mod 2^64
+__device__ __forceinline__ uint64_t gap_bits(uint64_t a, uint64_t b) {
+    constexpr uint64_t R_LO64 = 0x43e1f593f0000001ull;
+    return a - b - 1 + (a > b ? 0 : R_LO64);
+}
+
+// the EXCLUSION_RANGE_BITS low bits of v as field elements 0 / 1, LSB first
+__device__ __forceinline__ void store_range_bits(Fr* out, uint64_t v) {
+    const Fr one = Fr::one(), zero = Fr::zero();
+#pragma unroll 1
+    for (uint32_t k = 0; k < EXCLUSION_RANGE_BITS; k++) out[k] = ((v >> k) & 1) ? one : zero;
+}
+
+// Witness of the exclusion withdraw statement, layout of DESIGN.md section 3 (== oracle/exclusion_circuit.py); row p starts
+// at W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with two warps, one per independent chain of a proof, so no
+// warp diverges and a proof's critical path stays at about one withdraw path:
+//   warp 0   the withdraw chain (withdraw_chain_witness): 67 permutations at depth 32
+//   warp 1   low and next, the low / next / gap_lo / gap_hi bits from integer arithmetic on the path word, the blocklist
+//            leaf MultiMiMC7([low, next], 0) with its round values, the exclusion path, exclusion_root: 66 permutations
+// The warps write disjoint variables, so no barrier is needed.  Only the low `depth` bits of the path word count, as in
+// witness_path; x = 1 + that index is at most 2^32.
+__global__ void __launch_bounds__(64) k_exclusion_witness(ExclusionLayout L, uint32_t w_stride, ExclusionInputs in, uint32_t batch,
+                                                          Fr* __restrict__ W, int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    if (p >= batch) return;
+    Fr* w = W + (uint64_t)p * w_stride;
+    if (role == 0) {
+        Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
+        Fr se = load_canonical<Fr>(in.secrets + 32ull * p, flag);
+        withdraw_chain_witness(L, w, nu, se, in.recipients + 32ull * p, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
+    } else {
+        const uint64_t lo = in.low[p], nx = in.next[p];
+        const uint64_t mask = L.depth >= 32 ? 0xffffffffull : (1ull << L.depth) - 1;
+        const uint64_t x = 1 + (in.path_bits[p] & mask);
+        store_range_bits(w + L.low_bits, lo);
+        store_range_bits(w + L.next_bits, nx);
+        store_range_bits(w + L.gap_lo_bits, gap_bits(x, lo));
+        store_range_bits(w + L.gap_hi_bits, gap_bits(nx, x));
+        uint32_t c[8] = {(uint32_t)lo, (uint32_t)(lo >> 32), 0, 0, 0, 0, 0, 0};
+        const Fr flo = Fr::from_canonical(c);
+        c[0] = (uint32_t)nx; c[1] = (uint32_t)(nx >> 32);
+        const Fr fnx = Fr::from_canonical(c);
+        w[8] = flo; w[9] = fnx;
+        Fr leaf = mimc7_hash2<true>(flo, fnx, w + L.leaf_base, w + L.leaf_base + L.perm);
+        w[L.leaf_out] = leaf;
+        w[4] = witness_path(leaf, w + L.excl_base, L.depth, L.lvl_size, L.perm, in.excl_siblings + 32ull * L.depth * p,
+                            in.excl_path_bits[p], flag);
     }
 }
 
@@ -339,7 +400,8 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
     return OG_OK;
 }
 
-// One CTA covers 32 proofs in every statement's kernel; the transfer and association kernels give a proof more than one warp.
+// One CTA covers 32 proofs in every statement's kernel; the transfer, association and exclusion kernels give a proof more than
+// one warp.
 int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
                               Fr* d_W) {
     if (batch == 0) return OG_OK;
@@ -363,6 +425,12 @@ int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t
     case ST_ASSOCIATION: {
         const AssociationInputs t{a[0], a[1], a[2], a[3], (const uint32_t*)a[4], a[5], (const uint32_t*)a[6]};
         OG_LAUNCH(ctx, k_association_witness, grid, 64, 0, AssociationLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
+        break;
+    }
+    case ST_EXCLUSION: {
+        const ExclusionInputs t{a[0], a[1], a[2], a[3], (const uint32_t*)a[4], (const uint64_t*)a[5], (const uint64_t*)a[6], a[7],
+                                (const uint32_t*)a[8]};
+        OG_LAUNCH(ctx, k_exclusion_witness, grid, 64, 0, ExclusionLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
         break;
     }
     }

@@ -1,6 +1,7 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit, transfer and association statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
-// oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout and oracle/association_circuit.py: Layout).
+// withdraw, deposit, transfer, association and exclusion statements (DESIGN.md section 3; must equal
+// oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout,
+// oracle/association_circuit.py: Layout and oracle/exclusion_circuit.py: Layout).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -116,11 +117,53 @@ struct AssociationInputs {
     const uint32_t* assoc_path_bits;
 };
 
+constexpr uint32_t EXCLUSION_N_PUB = 4;
+constexpr uint32_t EXCLUSION_RANGE_BITS = 33;
+
+// 0 ONE | 1 root | 2 nullifier_hash | 3 recipient | 4 exclusion_root | 5 nullifier | 6 secret | 7 recipient_sq | 8 low | 9 next
+// | 10.. nullifier-hash permutation | commitment perm1, perm2, out | depth pool levels | low, next, gap_lo, gap_hi bits (33 each,
+// LSB first) | leaf perm1, perm2, out | depth exclusion levels (oracle/exclusion_circuit.py); a level block is the withdraw
+// statement's.
+struct ExclusionLayout {
+    uint32_t depth, perm, cm_base, cm_out, pool_base, low_bits, next_bits, gap_lo_bits, gap_hi_bits, leaf_base, leaf_out, excl_base,
+        lvl_size, n_vars, n_constraints;
+    static ExclusionLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        ExclusionLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        L.cm_base = 10 + L.perm;
+        L.cm_out = L.cm_base + 2 * L.perm;
+        L.lvl_size = 2 * L.perm + 4;
+        L.pool_base = L.cm_out + 1;
+        L.low_bits = L.pool_base + depth * L.lvl_size;
+        L.next_bits = L.low_bits + EXCLUSION_RANGE_BITS;
+        L.gap_lo_bits = L.next_bits + EXCLUSION_RANGE_BITS;
+        L.gap_hi_bits = L.gap_lo_bits + EXCLUSION_RANGE_BITS;
+        L.leaf_base = L.gap_hi_bits + EXCLUSION_RANGE_BITS;
+        L.leaf_out = L.leaf_base + 2 * L.perm;
+        L.excl_base = L.leaf_out + 1;
+        L.n_vars = L.excl_base + depth * L.lvl_size;
+        L.n_constraints = 142 + 5 * L.perm + depth * (4 * L.perm + 6);
+        return L;
+    }
+};
+
+// the caller's inputs of a batch of exclusion withdrawals (k_exclusion_witness's argument): per proof 32 B each of nullifier,
+// secret, recipient, depth siblings per tree, one path-bits word per tree, and the keys low, next (u64) of the blocklist leaf
+// that brackets the note
+struct ExclusionInputs {
+    const uint8_t *nullifiers, *secrets, *recipients, *siblings;
+    const uint32_t* path_bits;
+    const uint64_t *low, *next;
+    const uint8_t* excl_siblings;
+    const uint32_t* excl_path_bits;
+};
+
 // ---- the statement table ------------------------------------------------------------------------------------------------
 // What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
 // statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
 // statement_witness_dev) and its og_* forwarders (capi.cu).
-enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION };
+enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION };
 constexpr uint32_t STATEMENT_MAX_INPUTS = 11;
 
 struct StatementShape { uint32_t n_vars, n_constraints; };
@@ -147,6 +190,8 @@ constexpr StatementDesc STATEMENTS[] = {
     {TRANSFER_N_PUB, layout_shape<TransferLayout>, true, 11, {32, 32, 32, 64, 64, 16, 0, 8, 64, 64, 16}, {0, 0, 0, 0, 0, 0, 64, 0, 0, 0, 0}},
     // association: nullifiers, secrets, recipients, siblings, path_bits, assoc_siblings, assoc_path_bits
     {ASSOCIATION_N_PUB, layout_shape<AssociationLayout>, true, 7, {32, 32, 32, 0, 4, 0, 4}, {0, 0, 0, 32, 0, 32, 0}},
+    // exclusion: nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings, excl_path_bits
+    {EXCLUSION_N_PUB, layout_shape<ExclusionLayout>, true, 9, {32, 32, 32, 0, 4, 8, 8, 0, 4}, {0, 0, 0, 32, 0, 0, 0, 32, 0}},
 };
 
 // the input arrays of a batch in the statement's C ABI order (host or device pointers)

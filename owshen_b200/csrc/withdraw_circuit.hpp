@@ -1,9 +1,9 @@
-// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit, transfer and association statements'
-// R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these are the
+// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit, transfer, association and exclusion
+// statements' R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these are the
 // product's own definitions, checked entry for entry against the independently written
-// oracle/withdraw_circuit.py, oracle/deposit_circuit.py, oracle/transfer_circuit.py and oracle/association_circuit.py
-// through og_withdraw_r1cs_export, og_deposit_r1cs_export, og_transfer_r1cs_export and og_association_r1cs_export
-// (statement_r1cs below).
+// oracle/withdraw_circuit.py, oracle/deposit_circuit.py, oracle/transfer_circuit.py, oracle/association_circuit.py and
+// oracle/exclusion_circuit.py through og_withdraw_r1cs_export, og_deposit_r1cs_export, og_transfer_r1cs_export,
+// og_association_r1cs_export and og_exclusion_r1cs_export (statement_r1cs below).
 //
 // withdraw
 //   public : root, nullifier_hash, recipient
@@ -24,6 +24,12 @@
 //   private: nullifier, secret, siblings[depth], bits[depth], assoc_siblings[depth], assoc_bits[depth]
 //   withdraw's nullifier hash and commitment; the commitment reaches root along the pool path and association_root along
 //   the association path (one depth for both trees); recipient^2 bound.
+// exclusion
+//   public : root, nullifier_hash, recipient, exclusion_root
+//   private: nullifier, secret, siblings[depth], bits[depth], low, next, excl_siblings[depth], excl_bits[depth]
+//   withdraw's nullifier hash, commitment and pool path; with x = ONE + sum 2^l bits[l] (leaf index + 1), low, next,
+//   x - low - 1 and next - x - 1 range-checked to 33 bits, and MultiMiMC7([low, next], 0) reaching exclusion_root along the
+//   exclusion path (one depth for both trees); recipient^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -65,7 +71,7 @@ struct R1cs {
     uint32_t n_constraints() const { return A.rows(); }
 };
 
-// the MiMC7 gadgets both statements are made of
+// the MiMC7, Merkle-path and range gadgets the statements are made of
 struct Mimc7Builder {
     R1cs cs;
     Fr consts[MIMC_ROUNDS];
@@ -120,6 +126,19 @@ struct Mimc7Builder {
         }
         return cur;
     }
+    // n_bits range rows: bit_k * (bit_k - ONE) = 0 for the variables bits + k, then (sum 2^k bit_k - value) * ONE = 0
+    void range(const LC& value, uint32_t bits, uint32_t n_bits) {
+        LC m1 = lc_neg_var(0), packed;
+        for (auto& kv : value) lc_add_term(packed, kv.first, kv.second.neg());
+        Fr pow2 = Fr::one();
+        for (uint32_t k = 0; k < n_bits; k++) {
+            LC vbit = lc_var(bits + k);
+            cs.add(vbit, lc_sum({&vbit, &m1}), LC());
+            lc_add_term(packed, bits + k, pow2);
+            pow2 = pow2 + pow2;
+        }
+        cs.add(packed, lc_var(0), LC());
+    }
 };
 
 struct WithdrawBuilder {
@@ -156,18 +175,6 @@ struct DepositBuilder {
 };
 
 struct TransferBuilder {
-    // the 64 range rows bit_k * (bit_k - ONE) = 0 and (sum 2^k bit_k - amount) * ONE = 0 of the note block at `v`
-    static void range(Mimc7Builder& b, uint32_t v) {
-        LC m1 = lc_neg_var(0), packed = lc_neg_var(v + 2);
-        Fr pow2 = Fr::one();
-        for (uint32_t k = 0; k < TRANSFER_AMOUNT_BITS; k++) {
-            LC vbit = lc_var(v + 3 + k);
-            b.cs.add(vbit, lc_sum({&vbit, &m1}), LC());
-            lc_add_term(packed, v + 3 + k, pow2);
-            pow2 = pow2 + pow2;
-        }
-        b.cs.add(packed, lc_var(0), LC());
-    }
     // commitment = MultiMiMC7([nullifier, secret, token, amount], 0) of the note block at `v`, rounds from `cm`
     static void commitment(Mimc7Builder& b, uint32_t v, uint32_t cm, uint32_t cm_out, uint32_t P) {
         LC nu = lc_var(v), se = lc_var(v + 1), tok = lc_var(3), am = lc_var(v + 2);
@@ -186,7 +193,7 @@ struct TransferBuilder {
             const uint32_t v = L.inp(i);
             LC nu = lc_var(v);
             b.multi_hash({&nu}, lc_var(V_ONE), {v + L.nh_perm}, V_NH + i);
-            range(b, v);
+            b.range(lc_var(v + 2), v + 3, TRANSFER_AMOUNT_BITS);
             commitment(b, v, v + L.in_cm, v + L.in_cm_out, P);
             const uint32_t cur = b.merkle_path(v + L.in_cm_out, v + L.lvl_base, L.lvl_size, depth);
             LC vroot = lc_var(V_ROOT), ncur = lc_neg_var(cur);
@@ -194,7 +201,7 @@ struct TransferBuilder {
         }
         for (uint32_t j = 0; j < 2; j++) {
             const uint32_t v = L.out(j);
-            range(b, v);
+            b.range(lc_var(v + 2), v + 3, TRANSFER_AMOUNT_BITS);
             commitment(b, v, v + L.out_cm, v + L.out_cm_out, P);
             LC vout = lc_var(v + L.out_cm_out), ncm = lc_neg_var(V_OUT_CM + j);
             b.cs.add(lc_sum({&vout, &ncm}), lc_var(V_ONE), LC());
@@ -229,6 +236,42 @@ struct AssociationBuilder {
     }
 };
 
+struct ExclusionBuilder {
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        ExclusionLayout L = ExclusionLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = EXCLUSION_N_PUB;
+        const uint32_t V_ONE = 0, V_ROOT = 1, V_NHASH = 2, V_RECIP = 3, V_XROOT = 4, V_NULL = 5, V_SECRET = 6, V_RSQ = 7, V_LOW = 8,
+                       V_NEXT = 9, V_NH_PERM = 10;
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        LC nu = lc_var(V_NULL);
+        b.multi_hash({&nu}, lc_var(V_ONE), {V_NH_PERM}, V_NHASH);
+        b.hash2(lc_var(V_NULL), lc_var(V_SECRET), L.cm_base, L.cm_base + L.perm, L.cm_out);
+        const uint32_t pool_root = b.merkle_path(L.cm_out, L.pool_base, L.lvl_size, depth);
+        LC vpool = lc_var(pool_root), nroot = lc_neg_var(V_ROOT);
+        b.cs.add(lc_sum({&vpool, &nroot}), lc_var(V_ONE), LC());
+        // x = ONE + sum 2^l bit_l over the pool levels' bits: the note's leaf index + 1, its key in the blocklist tree
+        LC x = lc_var(V_ONE), nx;
+        Fr pow2 = Fr::one();
+        for (uint32_t l = 0; l < depth; l++) {
+            lc_add_term(x, L.pool_base + l * L.lvl_size + 1, pow2);
+            pow2 = pow2 + pow2;
+        }
+        for (auto& kv : x) lc_add_term(nx, kv.first, kv.second.neg());
+        LC low = lc_var(V_LOW), next = lc_var(V_NEXT), nlow = lc_neg_var(V_LOW), m1 = lc_neg_var(V_ONE);
+        b.range(low, L.low_bits, EXCLUSION_RANGE_BITS);
+        b.range(next, L.next_bits, EXCLUSION_RANGE_BITS);
+        b.range(lc_sum({&x, &nlow, &m1}), L.gap_lo_bits, EXCLUSION_RANGE_BITS);      // x - low - 1
+        b.range(lc_sum({&next, &nx, &m1}), L.gap_hi_bits, EXCLUSION_RANGE_BITS);     // next - x - 1
+        b.hash2(low, next, L.leaf_base, L.leaf_base + L.perm, L.leaf_out);
+        const uint32_t excl_root = b.merkle_path(L.leaf_out, L.excl_base, L.lvl_size, depth);
+        LC vexcl = lc_var(excl_root), nxroot = lc_neg_var(V_XROOT);
+        b.cs.add(lc_sum({&vexcl, &nxroot}), lc_var(V_ONE), LC());
+        return b.cs;
+    }
+};
+
 // the statement's R1CS at `depth` (ignored by deposit)
 inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     switch (s) {
@@ -236,6 +279,7 @@ inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     case ST_DEPOSIT: return DepositBuilder::build();
     case ST_TRANSFER: return TransferBuilder::build(depth);
     case ST_ASSOCIATION: return AssociationBuilder::build(depth);
+    case ST_EXCLUSION: return ExclusionBuilder::build(depth);
     }
     return R1cs();
 }
