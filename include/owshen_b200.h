@@ -399,7 +399,9 @@ int32_t og_msm_bucket_sums(og_ctx* ctx, int32_t g2, const uint8_t* points, uint3
                            const uint32_t* entries, uint32_t n_groups, uint32_t nb, uint64_t n_entries_max, int32_t few_groups,
                            uint8_t* out_totals, uint8_t* out_buckets);
 /* Element-wise arithmetic of the MSM units on raw Montgomery limbs (no conversion, no range check), through the functions the bucket
- * kernels call (the same source and PTX; the compiler gives each kernel its own machine-code copy of them).  unit 0 (G1 unit, Fq, 32 B per operand): op 0 a * b, 1 a^2 (the out-of-line squarer), 2 a - b, 3 a + a.
+ * kernels call (the same source and PTX; the compiler gives each kernel its own machine-code copy of them).  unit 0 (G1 unit, Fq, 32 B per operand): op 0 a * b, 1 a^2, 2 a - b, 3 a + a
+ * (canonical forms), 8 lazy a * b, 9 lazy a^2 (the out-of-line squarer), 10 lazy a + b, 11 lazy a - b, 12 a reduced to [0, p),
+ * 13 "a == 0 mod p" (1 or 0 in the first byte, the rest zero), 14 lazy a^2 + (2p - b)^2 with one reduction; ops 4-7 are invalid.
  * unit 1 (G2 unit, Fq2, 64 B): op 0 lazy a * b, 1 lazy a^2, 2 lazy a + b, 3 lazy a - b, 4 a reduced to [0, p), 5 a * b,
  * 6 a^2, 7 "a == 0 mod p" (1 or 0 in the first byte, the rest zero).  b is read for every op. */
 int32_t og_field_probe_raw(og_ctx* ctx, int32_t unit, int32_t op, const uint8_t* a, const uint8_t* b, uint64_t n, uint8_t* out);

@@ -359,13 +359,14 @@ class Context:
         return out.raw
 
     # ops of field_probe_raw per unit (include/owshen_b200.h: og_field_probe_raw)
-    FIELD_PROBE_OPS = {"g1": ("mul", "sqr", "sub", "dbl"),
+    FIELD_PROBE_OPS = {"g1": ("mul", "sqr", "sub", "dbl", None, None, None, None,
+                              "mul_lazy", "sqr_lazy", "add_lazy", "sub_lazy", "canonical", "is_zero_lazy", "mul_sum_lazy"),
                        "g2": ("mul_lazy", "sqr_lazy", "add_lazy", "sub_lazy", "canonical", "mul", "sqr", "is_zero_lazy")}
 
     def field_probe_raw(self, unit: str, op: str, a: bytes, b: bytes = None) -> bytes:
         """Test/debug probe: element-wise arithmetic of the G1 ("g1": Fq, 32 B per operand) or G2 ("g2": Fq2, 64 B) MSM unit on
         raw Montgomery limbs, through the functions its bucket kernels call (the probe kernel's own compiled copies); raw limbs out."""
-        _need(unit in self.FIELD_PROBE_OPS and op in self.FIELD_PROBE_OPS[unit], "field_probe_raw: unknown unit or op")
+        _need(unit in self.FIELD_PROBE_OPS and op is not None and op in self.FIELD_PROBE_OPS[unit], "field_probe_raw: unknown unit or op")
         eb = 32 if unit == "g1" else 64
         b = a if b is None else b
         _need(len(a) % eb == 0 and len(b) == len(a), f"field_probe_raw: a and b must be equally long multiples of {eb} bytes")

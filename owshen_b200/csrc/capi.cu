@@ -1289,7 +1289,8 @@ int32_t og_msm_bucket_sums(og_ctx* ctx, int32_t g2, const uint8_t* points, uint3
 
 int32_t og_field_probe_raw(og_ctx* ctx, int32_t unit, int32_t op, const uint8_t* a, const uint8_t* b, uint64_t n, uint8_t* out) {
     OG_ENTER(ctx);
-    if (unit < 0 || unit > 1 || op < 0 || op > (unit ? 7 : 3) || (n && (!a || !b || !out))) return OG_E_INVALID;
+    const bool op_ok = unit ? (op >= 0 && op <= 7) : ((op >= 0 && op <= 3) || (op >= 8 && op <= 14));   // G1: 4-7 unused
+    if (unit < 0 || unit > 1 || !op_ok || (n && (!a || !b || !out))) return OG_E_INVALID;
     if (n == 0) return OG_OK;
     const uint64_t eb = unit ? 64 : 32;
     OG_SLOT(ctx, da, uint8_t, S_IO_A, eb * n);

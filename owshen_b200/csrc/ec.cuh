@@ -151,6 +151,32 @@ OG_HD bool g2_madd_lazy(const Acc& A, const Affine<Fq2>& q) {
     return true;
 }
 
+// ---- G1 mixed addition over lazily reduced Fq (bounds at fp.cuh: Fq2::add_lazy) ----------------------------------------
+// g2_madd_lazy's contract on Fq: acc += q for a finite accumulator held by A (every coordinate in [0, 2p)) and a finite affine q
+// with canonical coordinates; false when the sum is infinity (A is then left as it was).  The squarings go through fq_sqr_lazy
+// (one out-of-line copy in the G1 MSM unit); Y3 = r (q1 - x3) - Y1 ppp is one sum of two products with a single reduction.
+template <class Acc>
+OG_HD bool g1_madd_lazy(const Acc& A, const Affine<Fq>& q) {
+    Fq p = Fq::sub_lazy(Fq::mul_lazy(q.x, A.ld(2)), A.ld(0));
+    Fq r = Fq::sub_lazy(Fq::mul_lazy(q.y, A.ld(3)), A.ld(1));
+    if (p.is_zero_lazy()) {
+        if (!r.is_zero_lazy()) return false;                  // acc == -q
+        XYZZ<Fq> d = XYZZ<Fq>::dbl_affine(q);                 // acc == q (rare): canonical values are lazy values too
+        A.st(0, d.x); A.st(1, d.y); A.st(2, d.zz); A.st(3, d.zzz);
+        return true;
+    }
+    // ordered so that few temporaries are live at a time: zz and zzz are updated as soon as pp / ppp exist
+    Fq pp = fq_sqr_lazy(p);
+    A.st(2, Fq::mul_lazy(A.ld(2), pp));
+    Fq ppp = Fq::mul_lazy(p, pp);
+    A.st(3, Fq::mul_lazy(A.ld(3), ppp));
+    Fq q1 = Fq::mul_lazy(A.ld(0), pp);
+    Fq x3 = Fq::sub_lazy(Fq::sub_lazy(fq_sqr_lazy(r), ppp), Fq::add_lazy(q1, q1));
+    A.st(0, x3);
+    A.st(1, Fq::mul_sum_lazy(r, Fq::sub_lazy(q1, x3), A.ld(1).neg_raw(), ppp));
+    return true;
+}
+
 // Out-of-line copies for kernels where a group operation is not the inner loop (reductions, table
 // builds, finalisation): one body per field instead of one per call site keeps ptxas time sane.
 #if defined(__CUDACC__)

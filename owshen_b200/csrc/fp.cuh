@@ -109,8 +109,9 @@ OG_HD void final_sub(uint32_t* r) {
 //    injected with add.cc(s, 0xffffffff) into the q*p chain on E, which starts at limb 1.
 // No limb ripples through a whole array, so successive rows overlap and the dependency chain per product
 // is short (this kernel family is latency-bound at 4 warps/scheduler).
-template <class P>
-OG_HD void mont_row(uint32_t* E, uint32_t* O, const uint32_t* a, uint32_t bi, bool first) {
+// The row is split in its product step (mont_row_mul, which returns the orphan) and its reduction step (mont_row_redc) so that
+// mont_mul_sum_lazy can add a second product (mont_row_addmul) to the window in between.
+OG_HD uint32_t mont_row_mul(uint32_t* E, uint32_t* O, const uint32_t* a, uint32_t bi, bool first) {
     CC cc;
     uint32_t orphan = 0;
     if (first) {
@@ -143,6 +144,34 @@ OG_HD void mont_row(uint32_t* E, uint32_t* O, const uint32_t* a, uint32_t bi, bo
         }
         O[7] = addc(O[7], 0u, cc);
     }
+    return orphan;
+}
+
+// E, O += c * di at the window of the current row (between mont_row_mul and mont_row_redc): E at limbs 0..7, O at limbs 1..8
+OG_HD void mont_row_addmul(uint32_t* E, uint32_t* O, const uint32_t* c, uint32_t di) {
+    CC cc;
+    O[0] = mad_lo_cc(c[1], di, O[0], cc);
+    O[1] = madc_hi_cc(c[1], di, O[1], cc);
+#pragma unroll
+    for (int j = 2; j < 6; j += 2) {
+        O[j] = madc_lo_cc(c[j + 1], di, O[j], cc);
+        O[j + 1] = madc_hi_cc(c[j + 1], di, O[j + 1], cc);
+    }
+    O[6] = madc_lo_cc(c[7], di, O[6], cc);
+    O[7] = madc_hi(c[7], di, O[7], cc);               // limb 8: the caller keeps the running sum below 2^288
+    E[0] = mad_lo_cc(c[0], di, E[0], cc);
+    E[1] = madc_hi_cc(c[0], di, E[1], cc);
+#pragma unroll
+    for (int j = 2; j < 8; j += 2) {
+        E[j] = madc_lo_cc(c[j], di, E[j], cc);
+        E[j + 1] = madc_hi_cc(c[j], di, E[j + 1], cc);
+    }
+    O[7] = addc(O[7], 0u, cc);
+}
+
+template <class P>
+OG_HD void mont_row_redc(uint32_t* E, uint32_t* O, uint32_t orphan) {
+    CC cc;
     uint32_t s = add_cc(E[0], orphan, cc);            // carry -> limb 1
     uint32_t q = mul_lo(s, P::INV);
     O[0] = madc_lo_cc(P::mod(1), q, O[0], cc);
@@ -165,6 +194,12 @@ OG_HD void mont_row(uint32_t* E, uint32_t* O, const uint32_t* a, uint32_t bi, bo
     E[0] = 0;                                         // dead from here on
 }
 
+template <class P>
+OG_HD void mont_row(uint32_t* E, uint32_t* O, const uint32_t* a, uint32_t bi, bool first) {
+    uint32_t orphan = mont_row_mul(E, O, a, bi, first);
+    mont_row_redc<P>(E, O, orphan);
+}
+
 // 2p as limbs (p < 2^254, so 2p < 2^255)
 template <class P>
 OG_HD constexpr uint32_t mod2(int i) { return (P::mod(i) << 1) | (i ? P::mod(i - 1) >> 31 : 0u); }
@@ -183,6 +218,56 @@ OG_HD void cond_sub_2p(uint32_t* r) {
     for (int j = 0; j < 8; j++) r[j] = borrow ? r[j] : t[j];
 }
 
+// ---- lazily reduced limbs: values in [0, 2p) instead of [0, p), shared by Fp and Fq2 (bounds at Fq2::add_lazy) ------------------
+template <class P>
+OG_HD void add_lazy_limbs(uint32_t* r, const uint32_t* a, const uint32_t* b) {       // a + b < 4p -> [0, 2p)
+    CC cc;
+    r[0] = add_cc(a[0], b[0], cc);
+#pragma unroll
+    for (int j = 1; j < 7; j++) r[j] = addc_cc(a[j], b[j], cc);
+    r[7] = addc(a[7], b[7], cc);
+    cond_sub_2p<P>(r);
+}
+template <class P>
+OG_HD void sub_lazy_limbs(uint32_t* r, const uint32_t* a, const uint32_t* b) {       // a - b in (-2p, 2p) -> [0, 2p)
+    CC cc;
+    r[0] = sub_cc(a[0], b[0], cc);
+#pragma unroll
+    for (int j = 1; j < 8; j++) r[j] = subc_cc(a[j], b[j], cc);
+    uint32_t borrow = subc(0u, 0u, cc);
+    r[0] = add_cc(r[0], mod2<P>(0) & borrow, cc);
+#pragma unroll
+    for (int j = 1; j < 7; j++) r[j] = addc_cc(r[j], mod2<P>(j) & borrow, cc);
+    r[7] = addc(r[7], mod2<P>(7) & borrow, cc);
+}
+template <class P>
+OG_HD void sub_raw_limbs(uint32_t* r, const uint32_t* a, const uint32_t* b) {        // a + 2p - b in (0, 4p), a, b < 2p
+    CC cc;
+    r[0] = add_cc(a[0], mod2<P>(0), cc);
+#pragma unroll
+    for (int j = 1; j < 7; j++) r[j] = addc_cc(a[j], mod2<P>(j), cc);
+    r[7] = addc(a[7], mod2<P>(7), cc);
+    r[0] = sub_cc(r[0], b[0], cc);
+#pragma unroll
+    for (int j = 1; j < 7; j++) r[j] = subc_cc(r[j], b[j], cc);
+    r[7] = subc(r[7], b[7], cc);
+}
+template <class P>
+OG_HD void neg_raw_limbs(uint32_t* r, const uint32_t* a) {                          // 2p - a in (0, 2p], a < 2p
+    CC cc;
+    r[0] = sub_cc(mod2<P>(0), a[0], cc);
+#pragma unroll
+    for (int j = 1; j < 7; j++) r[j] = subc_cc(mod2<P>(j), a[j], cc);
+    r[7] = subc(mod2<P>(7), a[7], cc);
+}
+template <class P>
+OG_HD bool is_zero_lazy_limbs(const uint32_t* a) {                                  // a == 0 mod p, a < 2p
+    uint32_t z = 0, q = 0;
+#pragma unroll
+    for (int j = 0; j < 8; j++) { z |= a[j]; q |= a[j] ^ P::mod(j); }
+    return z == 0 || q == 0;
+}
+
 // r = (a * b + m * p) / 2^256 with m < 2^256, i.e. r == a * b * 2^-256 (mod p) and r < a * b / 2^256 + p.  For a, b < 2p
 // that is r < (4p / 2^256 + 1) p < 1.76 p (p < 0.19 * 2^256): products of values in [0, 2p) stay in [0, 2p) without any final
 // subtraction, and no running sum leaves 2^288 (a + p < 2^256).  r may alias a or b.
@@ -197,6 +282,28 @@ OG_HD void mont_mul_lazy(uint32_t* r, const uint32_t* a, const uint32_t* b) {
     mont_row<P>(O, E, a, b[5], false);
     mont_row<P>(E, O, a, b[6], false);
     mont_row<P>(O, E, a, b[7], false);
+    CC cc;
+    r[0] = add_cc(E[0], O[1], cc);
+#pragma unroll
+    for (int j = 1; j < 7; j++) r[j] = addc_cc(E[j], O[j + 1], cc);
+    r[7] = addc(E[7], 0u, cc);
+}
+
+// r = (a * b + c * d + m * p) / 2^256: the sum of two products with ONE Montgomery reduction, interleaved row by row like
+// mont_mul_lazy (two product chains and one reduction chain per row, 192 instead of 256 wide multiply-adds for two reduced
+// products).  Every running sum stays below (a + c + p) 2^32 < 2^288 for a + c + p < 2^256, and r < (a b + c d) / 2^256 + p.
+// The bound of its use in the G1 group law is derived at Fq2::add_lazy.  r may not alias an operand.
+template <class P>
+OG_HD void mont_mul_sum_lazy(uint32_t* r, const uint32_t* a, const uint32_t* b, const uint32_t* c, const uint32_t* d) {
+    uint32_t E[8], O[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        uint32_t* X = (i & 1) ? O : E;
+        uint32_t* Y = (i & 1) ? E : O;
+        uint32_t orphan = mont_row_mul(X, Y, a, b[i], i == 0);
+        mont_row_addmul(X, Y, c, d[i]);
+        mont_row_redc<P>(X, Y, orphan);
+    }
     CC cc;
     r[0] = add_cc(E[0], O[1], cc);
 #pragma unroll
@@ -422,6 +529,16 @@ struct alignas(32) Fp {
     // value < 4p -> [0, 2p)  /  value < 2p -> [0, p)
     OG_HD Fp reduce_4p_to_2p() const { Fp r = *this; cond_sub_2p<P>(r.l); return r; }
     OG_HD Fp reduce_2p_to_p() const { Fp r = *this; final_sub<P>(r.l); return r; }
+    // the rest of the lazy forms (G1 group law): operands and results in [0, 2p), bounds at Fq2::add_lazy
+    OG_HD static Fp add_lazy(const Fp& a, const Fp& b) { Fp r; add_lazy_limbs<P>(r.l, a.l, b.l); return r; }
+    OG_HD static Fp sub_lazy(const Fp& a, const Fp& b) { Fp r; sub_lazy_limbs<P>(r.l, a.l, b.l); return r; }
+    OG_HD Fp neg_raw() const { Fp r; neg_raw_limbs<P>(r.l, l); return r; }                  // 2p - a in (0, 2p]
+    OG_HD bool is_zero_lazy() const { return is_zero_lazy_limbs<P>(l); }
+    OG_HD Fp canonical() const { return reduce_2p_to_p(); }
+    // a b + c d with one reduction: operands in [0, 2p] (a b + c d < 8p^2), result in [0, 2p)
+    OG_HD static Fp mul_sum_lazy(const Fp& a, const Fp& b, const Fp& c, const Fp& d) {
+        Fp r; mont_mul_sum_lazy<P>(r.l, a.l, b.l, c.l, d.l); cond_sub_2p<P>(r.l); return r;
+    }
 
     OG_HD friend Fp operator+(const Fp& a, const Fp& b) {
         Fp r; CC cc;
@@ -566,45 +683,17 @@ struct Fq2 {
     //                    u v < 8p^2, r < 2.52p, one conditional subtraction of 2p                  -> [0, 2p)
     // Zero has two lazy forms per coordinate (0 and p): is_zero_lazy tests "== 0 mod p", canonical() maps to [0, p).
     // Values in [0, p) are valid lazy values, so canonical inputs (table points, one()) enter without conversion.
-    OG_HD static void add_lazy_fq(uint32_t* r, const uint32_t* a, const uint32_t* b) {
-        CC cc;
-        r[0] = add_cc(a[0], b[0], cc);
-#pragma unroll
-        for (int j = 1; j < 7; j++) r[j] = addc_cc(a[j], b[j], cc);
-        r[7] = addc(a[7], b[7], cc);
-        cond_sub_2p<FqParams>(r);
-    }
-    OG_HD static void sub_lazy_fq(uint32_t* r, const uint32_t* a, const uint32_t* b) {
-        CC cc;
-        r[0] = sub_cc(a[0], b[0], cc);
-#pragma unroll
-        for (int j = 1; j < 8; j++) r[j] = subc_cc(a[j], b[j], cc);
-        uint32_t borrow = subc(0u, 0u, cc);
-        r[0] = add_cc(r[0], mod2<FqParams>(0) & borrow, cc);
-#pragma unroll
-        for (int j = 1; j < 7; j++) r[j] = addc_cc(r[j], mod2<FqParams>(j) & borrow, cc);
-        r[7] = addc(r[7], mod2<FqParams>(7) & borrow, cc);
-    }
-    OG_HD static void sub_raw_fq(uint32_t* r, const uint32_t* a, const uint32_t* b) {     // a + 2p - b, a, b < 2p
-        CC cc;
-        r[0] = add_cc(a[0], mod2<FqParams>(0), cc);
-#pragma unroll
-        for (int j = 1; j < 7; j++) r[j] = addc_cc(a[j], mod2<FqParams>(j), cc);
-        r[7] = addc(a[7], mod2<FqParams>(7), cc);
-        r[0] = sub_cc(r[0], b[0], cc);
-#pragma unroll
-        for (int j = 1; j < 7; j++) r[j] = subc_cc(r[j], b[j], cc);
-        r[7] = subc(r[7], b[7], cc);
-    }
-    OG_HD static bool is_zero_lazy_fq(const uint32_t* a) {
-        uint32_t z = 0, q = 0;
-#pragma unroll
-        for (int j = 0; j < 8; j++) { z |= a[j]; q |= a[j] ^ FqParams::mod(j); }
-        return z == 0 || q == 0;
-    }
-    OG_HD static Fq2 add_lazy(const Fq2& a, const Fq2& b) { Fq2 r; add_lazy_fq(r.c0.l, a.c0.l, b.c0.l); add_lazy_fq(r.c1.l, a.c1.l, b.c1.l); return r; }
-    OG_HD static Fq2 sub_lazy(const Fq2& a, const Fq2& b) { Fq2 r; sub_lazy_fq(r.c0.l, a.c0.l, b.c0.l); sub_lazy_fq(r.c1.l, a.c1.l, b.c1.l); return r; }
-    OG_HD bool is_zero_lazy() const { return is_zero_lazy_fq(c0.l) && is_zero_lazy_fq(c1.l); }
+    // The same limb routines (add_lazy_limbs, sub_lazy_limbs, sub_raw_limbs, is_zero_lazy_limbs) are Fp's lazy forms, which the
+    // G1 group law (ec.cuh: g1_madd_lazy) runs on.  Its bounds, for values in [0, 2p):
+    //   Fp::mul_lazy   r < 4p^2 / 2^256 + p < 1.76p                                        -> [0, 2p) without a subtraction
+    //   Fp::sqr_lazy   the same bound through sqr_wide and mont_reduce_wide_lazy             -> [0, 2p)
+    //   Fp::mul_sum_lazy, the one-reduction Y3 = r (q1 - x3) - Y1 ppp:  - Y1 ppp is written (2p - Y1) ppp (neg_raw, 2p - Y1 in
+    //                  (0, 2p]), so both products are < 4p^2 and their sum T < 8p^2; reduced once (mont_mul_sum_lazy, whose running
+    //                  sums stay below (2p + 2p + p) 2^32 < 2^288), r < T / 2^256 + p < 1.52p + p = 2.52p; one conditional
+    //                  subtraction of 2p                                                    -> [0, 2p)
+    OG_HD static Fq2 add_lazy(const Fq2& a, const Fq2& b) { Fq2 r; add_lazy_limbs<FqParams>(r.c0.l, a.c0.l, b.c0.l); add_lazy_limbs<FqParams>(r.c1.l, a.c1.l, b.c1.l); return r; }
+    OG_HD static Fq2 sub_lazy(const Fq2& a, const Fq2& b) { Fq2 r; sub_lazy_limbs<FqParams>(r.c0.l, a.c0.l, b.c0.l); sub_lazy_limbs<FqParams>(r.c1.l, a.c1.l, b.c1.l); return r; }
+    OG_HD bool is_zero_lazy() const { return is_zero_lazy_limbs<FqParams>(c0.l) && is_zero_lazy_limbs<FqParams>(c1.l); }
     OG_HD Fq2 canonical() const { Fq2 r = *this; final_sub<FqParams>(r.c0.l); final_sub<FqParams>(r.c1.l); return r; }
 
     // Operands in [0, 2p), result in [0, 2p).  Ordered so that at most two 16-limb products are live at a time: c0 is reduced
@@ -653,9 +742,9 @@ struct Fq2 {
         Fq2 r;
         mul_wide(T, a.c0.l, a.c1.l);
         mont_reduce_wide_lazy<FqParams>(r.c1.l, T);
-        add_lazy_fq(r.c1.l, r.c1.l, r.c1.l);
-        add_lazy_fq(u, a.c0.l, a.c1.l);
-        sub_raw_fq(v, a.c0.l, a.c1.l);
+        add_lazy_limbs<FqParams>(r.c1.l, r.c1.l, r.c1.l);
+        add_lazy_limbs<FqParams>(u, a.c0.l, a.c1.l);
+        sub_raw_limbs<FqParams>(v, a.c0.l, a.c1.l);
         mul_wide(T, u, v);
         mont_reduce_wide_lazy<FqParams>(r.c0.l, T);
         cond_sub_2p<FqParams>(r.c0.l);
@@ -689,6 +778,16 @@ OG_HD Fq2 fq2_sqr_lazy(const Fq2& a) { return fq2_sqr_lazy_call(a); }
 #else
 OG_HD Fq2 fq2_mul_lazy(const Fq2& a, const Fq2& b) { return Fq2::mul_lazy_inl(a, b); }
 OG_HD Fq2 fq2_sqr_lazy(const Fq2& a) { return Fq2::sqr_lazy_inl(a); }
+#endif
+
+// The lazy Fq squaring of the G1 group law.  Units built with OG_FQ_SQR_CALL (the G1 MSM unit) keep ONE out-of-line copy of it
+// (8 registers in, 8 out): the G1 bucket kernel with the squarer inlined twice next to eight inlined products outgrows the
+// instruction cache (warps waiting for instructions).
+#if defined(__CUDA_ARCH__) && defined(OG_FQ_SQR_CALL)
+static __device__ __noinline__ Fq fq_sqr_lazy_call(Fq a) { return a.sqr_lazy(); }
+OG_HD Fq fq_sqr_lazy(const Fq& a) { return fq_sqr_lazy_call(a); }
+#else
+OG_HD Fq fq_sqr_lazy(const Fq& a) { return a.sqr_lazy(); }
 #endif
 
 }  // namespace og

@@ -13,6 +13,9 @@
 //   6. k_group_total / k_horner
 // All arithmetic is 8x32-bit Montgomery limbs in registers (fp.cuh); the kernels are bound by the
 // integer multiply-add pipe, not HBM: a G1 mixed add moves 64 B + 4 B and costs ~3.5k instructions.
+#ifdef OG_MSM_G1
+#define OG_FQ_SQR_CALL      // the G1 bucket accumulation squares through one out-of-line copy of the lazy squarer (fp.cuh)
+#endif
 #include "msm.cuh"
 #include "glv.cuh"
 #include <stdlib.h>
@@ -490,24 +493,9 @@ struct SmAcc1 {
 };
 
 // 8 CTAs of 128 threads per SM (64 registers); only the next 4-byte ENTRY is read ahead, the 64-byte gather is
-// covered by the other warps (compared against 6/7 CTAs and against a prefetched point)
-// the two squarings of a mixed addition through ONE out-of-line copy of the wide squarer (8 registers in, 8 out): with the squarer
-// inlined twice next to eight inlined products the kernel outgrows the instruction cache (ncu: warps waiting for instructions)
-#ifndef OG_SQR_CALL
-#define OG_SQR_CALL 1
-#endif
-#if OG_SQR_CALL
-static __device__ __noinline__ Fq fq_sqr_call(Fq a) { return a.sqr(); }
-#define OG_ACC_SQR(x) fq_sqr_call(x)
-#else
-#define OG_ACC_SQR(x) (x).sqr()
-#endif
-#if defined(OG_MUL_CALL) && OG_MUL_CALL      // A/B: the eight products out of line as well
-static __device__ __noinline__ Fq fq_mul_call(Fq a, Fq b) { return a * b; }
-#define OG_ACC_MUL(x, y) fq_mul_call((x), (y))
-#else
-#define OG_ACC_MUL(x, y) ((x) * (y))
-#endif
+// covered by the other warps (compared against 6/7 CTAs and against a prefetched point).  The mixed addition is g1_madd_lazy
+// (ec.cuh): lazily reduced Fq with the eight products inlined and the two squarings through one out-of-line copy of the lazy
+// squarer (fq_sqr_lazy_call); the accumulator stays in [0, 2p) and is made canonical when the bucket is stored.
 #ifndef OG_ACC1_MINB
 #define OG_ACC1_MINB 8
 #endif
@@ -535,36 +523,38 @@ __global__ void __launch_bounds__(128, OG_ACC1_MINB) k_bucket_acc_sm1(const Affi
         e = en;
         if (q.is_inf()) continue;
         if (inf) { A.st(0, q.x); A.st(1, q.y); A.st(2, Fq::one()); A.st(3, Fq::one()); inf = false; continue; }
-        Fq p = OG_ACC_MUL(q.x, A.ld(2)) - A.ld(0);
-        Fq r = OG_ACC_MUL(q.y, A.ld(3)) - A.ld(1);
-        if (p.is_zero()) {
-            if (r.is_zero()) { XYZZ<Fq> d = XYZZ<Fq>::dbl_affine(q); A.st(0, d.x); A.st(1, d.y); A.st(2, d.zz); A.st(3, d.zzz); }
-            else inf = true;
-            continue;
-        }
-        // ordered so that few temporaries are live at a time: zz and zzz are updated as soon as pp / ppp exist
-        Fq pp = OG_ACC_SQR(p);
-        A.st(2, OG_ACC_MUL(A.ld(2), pp));
-        Fq ppp = OG_ACC_MUL(p, pp);
-        A.st(3, OG_ACC_MUL(A.ld(3), ppp));
-        Fq q1 = OG_ACC_MUL(A.ld(0), pp);
-        Fq x3 = OG_ACC_SQR(r) - ppp - q1.dbl();
-        A.st(0, x3);
-        A.st(1, OG_ACC_MUL(r, q1 - x3) - OG_ACC_MUL(A.ld(1), ppp));
+        if (!g1_madd_lazy(A, q)) inf = true;          // the accumulator stays lazy ([0, 2p)) until the bucket is stored
     }
-    buckets[key] = inf ? XYZZ<Fq>::inf() : XYZZ<Fq>{A.ld(0), A.ld(1), A.ld(2), A.ld(3)};
+    buckets[key] = inf ? XYZZ<Fq>::inf() : XYZZ<Fq>{A.ld(0).canonical(), A.ld(1).canonical(), A.ld(2).canonical(), A.ld(3).canonical()};
 }
 
-// Test/debug probe (og_field_probe_raw, unit 0): raw Montgomery limbs in and out, no conversion and no range check, through the
-// product and the squarer (fq_sqr_call) of k_bucket_acc_sm1, with its launch bounds.  In this whole-program build ptxas compiles a
-// copy of every __noinline__ callee into each kernel that calls it, so the probe runs its own copy of fq_sqr_call: the same PTX, but
-// not necessarily the bucket kernel's register allocation.  op 0: a * b, 1: sqr(a), 2: a - b, 3: a.dbl()
+// Test/debug probe (og_field_probe_raw, unit 0): raw Montgomery limbs in and out, no conversion and no range check, with
+// k_bucket_acc_sm1's launch bounds.  ops 0-3 are the canonical forms: 0: a * b, 1: a.sqr(), 2: a - b, 3: a.dbl().  ops 8-14 are the
+// lazy forms g1_madd_lazy runs: 8: mul_lazy, 9: fq_sqr_lazy (the out-of-line squarer), 10: add_lazy, 11: sub_lazy, 12: canonical(a),
+// 13: is_zero_lazy(a) (1 or 0 in limb 0, every other limb 0), 14: mul_sum_lazy(a, a, b.neg_raw(), b.neg_raw()) = a^2 + (2p - b)^2,
+// which reaches the 8p^2 bound of the one-reduction Y3 with a near 2p and b near 0.  In this whole-program build ptxas compiles a copy of every
+// __noinline__ callee into each kernel that calls it, so the probe runs its own copy of fq_sqr_lazy_call: the same PTX, but not
+// necessarily the bucket kernel's register allocation.
 __global__ void __launch_bounds__(128, OG_ACC1_MINB) k_field_probe_g1(int32_t op, const Fq* __restrict__ a, const Fq* __restrict__ b, uint64_t n,
                                                         Fq* __restrict__ out) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const Fq x = a[i], y = b[i];
-    out[i] = op == 0 ? OG_ACC_MUL(x, y) : op == 1 ? OG_ACC_SQR(x) : op == 2 ? x - y : x.dbl();
+    Fq z;
+    switch (op) {
+        case 0: z = x * y; break;
+        case 1: z = x.sqr(); break;
+        case 2: z = x - y; break;
+        case 3: z = x.dbl(); break;
+        case 8: z = Fq::mul_lazy(x, y); break;
+        case 9: z = fq_sqr_lazy(x); break;
+        case 10: z = Fq::add_lazy(x, y); break;
+        case 11: z = Fq::sub_lazy(x, y); break;
+        case 12: z = x.canonical(); break;
+        case 13: z = Fq::zero(); z.l[0] = x.is_zero_lazy() ? 1u : 0u; break;
+        default: { const Fq v = y.neg_raw(); z = Fq::mul_sum_lazy(x, x, v, v); break; }
+    }
+    out[i] = z;
 }
 #endif
 

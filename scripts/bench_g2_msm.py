@@ -1,14 +1,20 @@
-"""The prover's G2 MSM inside the headline workload: 1024 depth-32 withdraw proofs per step (bench.py's step), per-kernel
-CUDA-event times from og_profile for the G2 bucket accumulation, the G2 reduction and heavy buckets, and the whole step.
+"""The prover's G2 and G1 MSMs inside the headline workload: 1024 depth-32 withdraw proofs per step (bench.py's step), per-kernel
+CUDA-event times from og_profile for the G2 and G1 bucket accumulations, their reductions and heavy buckets, and the whole step.
 
 The G2 accumulation's share of the carry-chain peak is computed from static counts: one mixed addition per (point, window)
 of the B MSM and WIDE_PER_MADD 32x32->64 multiply-adds per addition (8 lazy Fq2 products of 3 wide products + 2 reductions =
 320, 2 lazy Fq2 squarings of 2 wide products + 2 reductions = 256: fp.cuh), against og_int_pipe_peaks measured in the same
-run.  The card's name, power limit and SM clock are read with read-only nvidia-smi queries in the same call.
+run.  The G1 accumulation's share is computed over the A and C' MSMs from the expected number of mixed additions under uniform
+digits -- per (proof, window) the nonzero digits minus the occupied buckets, since the first point of a bucket is stored, not
+added; about 0.56 of bench.py's one addition per (point, window) -- with G1_WIDE_PER_MADD multiply-adds per addition: 6 lazy
+products of 128 (interleaved Montgomery), the one-reduction Y3 of 192 (two products and one reduction, mont_mul_sum_lazy) and
+2 lazy squarings of 36 + 64, 1160 in all (fp.cuh).  Builds before the lazy G1 accumulation spent 1224 (8 x 128 + 2 x 100);
+--g1-wide-per-madd 1224 reports an older library's share.  The card's name, power limit and SM clock are read with read-only
+nvidia-smi queries in the same call.
 
 OWSHEN_B200_LIB=<path> runs another build of the library, so that two builds can be alternated in one session:
     for i in 1 2 3; do OWSHEN_B200_LIB=old.so python scripts/bench_g2_msm.py; python scripts/bench_g2_msm.py; done
-Usage: python scripts/bench_g2_msm.py [--steps 3] [--warmup 2] [--batch 1024]"""
+Usage: python scripts/bench_g2_msm.py [--steps 3] [--warmup 2] [--batch 1024] [--g1-wide-per-madd 1160]"""
 import argparse
 import json
 import os
@@ -20,6 +26,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 WIDE_PER_MADD = 8 * 320 + 2 * 256
+G1_WIDE_PER_MADD = 6 * 128 + 192 + 2 * (36 + 64)
 KERNELS = ("k_bucket_acc_g2", "k_reduce_level_g2", "k_bucket_heavy_g2", "k_bucket_acc_g1", "k_reduce_level_g1")
 
 
@@ -39,6 +46,7 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--batch", type=int, default=1024)
+    ap.add_argument("--g1-wide-per-madd", type=int, default=G1_WIDE_PER_MADD)
     args = ap.parse_args()
 
     import torch
@@ -92,6 +100,19 @@ def main():
     floor_ms = 1e3 * madds * WIDE_PER_MADD / peak
     per_step = {k: prof[k][1] / args.steps for k in KERNELS if k in prof}
     acc = per_step.get("k_bucket_acc_g2")
+    # G1: one mixed addition per (point, window) of the A and C' MSMs, as bench.py counts them
+    info = api.r1cs_info(bench.DEPTH)
+    m = 1 << info["log_m"]
+    n_supp = len(set(api.r1cs_export(bench.DEPTH, "B")[1]))
+    n_priv = info["n_vars"] - info["n_pub"] - 1
+    win = lambda c: (255 + c - 1) // c
+    c_a, c_c = PK.window_bits[0], PK.window_bits[2]
+    def adds(n, c):                         # expected mixed additions of one (proof, window) group: entries - occupied buckets
+        nb, k = 1 << (c - 1), n * (1 - 2.0 ** -c)
+        return k - nb * (1 - (1 - 1 / nb) ** k)
+    g1_madds = args.batch * (adds(info["n_vars"] + 2, c_a) * win(c_a) + adds(n_priv + n_supp + m + 1, c_c) * win(c_c))
+    g1_floor_ms = 1e3 * g1_madds * args.g1_wide_per_madd / peak
+    acc1 = per_step.get("k_bucket_acc_g1")
     out = {
         "lib": os.environ.get("OWSHEN_B200_LIB") or "in-tree",
         "gpu": gpu_info(), "sm_clock_timed": clocks,
@@ -100,6 +121,8 @@ def main():
         "g2_madds_per_step": madds, "wide_madds_per_g2_madd": WIDE_PER_MADD,
         "carry_chain_peak_per_s": peak, "g2_acc_ms_at_peak": round(floor_ms, 1),
         "g2_acc_share_of_peak": round(floor_ms / acc, 3) if acc else None,
+        "g1_madds_per_step": round(g1_madds), "wide_madds_per_g1_madd": args.g1_wide_per_madd, "g1_acc_ms_at_peak": round(g1_floor_ms, 1),
+        "g1_acc_share_of_peak": round(g1_floor_ms / acc1, 3) if acc1 else None,
     }
     print(json.dumps(out))
     PK.close()
