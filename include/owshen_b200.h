@@ -256,6 +256,37 @@ int32_t og_exclusion_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifi
                              const uint64_t* excl_low, const uint64_t* excl_next, const uint8_t* excl_siblings,
                              const uint32_t* excl_path_bits, uint32_t batch, uint8_t* witnesses);
 
+/* ---- labeled notes and the labeled withdraw statement (DESIGN.md section 3): partial withdrawals with change, checked
+ * against a deposit blocklist ---- */
+/* A labeled note is (nullifier, secret, token, amount < 2^64, label < 2^32); precommitment = MultiMiMC7([nullifier, secret], 2),
+ * leaf = MultiMiMC7([precommitment, token, amount, label], 2).  The label is the pool leaf index at which the node appended
+ * the deposit.  Wallet: precommitments of n notes (32 B each in and out). */
+int32_t og_labeled_precommitments(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, uint64_t n, uint8_t* out);
+/* Node: leaves of n deposits from precommitments and tokens (32 B each), amounts (uint64) and labels (uint32). */
+int32_t og_labeled_leaves(og_ctx* ctx, const uint8_t* precommitments, const uint8_t* tokens, const uint64_t* amounts,
+                          const uint32_t* labels, uint64_t n, uint8_t* out);
+/* Public inputs (root, nullifier_hash, recipient, exclusion_root, token, withdrawn, change_commitment).  The note's leaf
+ * reaches root along the pool path; amount, withdrawn and change = amount - withdrawn are range-checked to 64 bits and the
+ * label to 32; change_commitment is the leaf of the change note (change_nullifier, change_secret, token, change, label);
+ * x = label + 1 satisfies excl_low < x < excl_next (33-bit range checks) and the blocklist leaf of (excl_low, excl_next)
+ * reaches exclusion_root (the exclusion statement's tree, same depth as the pool's, 1..32).  At depth 32: 52 685 variables,
+ * 52 617 constraints, domain 2^16. */
+int32_t og_labeled_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_labeled_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                               uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: token, recipient 32 B each; withdrawn (uint64);
+ * nullifier, secret 32 B each; amount (uint64); label (uint32); siblings depth * 32 B and path_bits one word (the note's
+ * pool path); change_nullifier, change_secret 32 B each; excl_low, excl_next (uint64); excl_siblings depth * 32 B and
+ * excl_path_bits one word (the blocklist path).  Path words: bit l set when the level-l node is a right child, only the low
+ * depth bits count.  Both roots, the nullifier hash and change_commitment are derived; an overdraw, a flagged label or a
+ * blocklist leaf that does not bracket it gives a witness that does not satisfy the R1CS. */
+int32_t og_labeled_witness(og_ctx* ctx, uint32_t depth, const uint8_t* tokens, const uint8_t* recipients, const uint64_t* withdrawn,
+                           const uint8_t* nullifiers, const uint8_t* secrets, const uint64_t* amounts, const uint32_t* labels,
+                           const uint8_t* siblings, const uint32_t* path_bits, const uint8_t* change_nullifiers,
+                           const uint8_t* change_secrets, const uint64_t* excl_low, const uint64_t* excl_next,
+                           const uint8_t* excl_siblings, const uint32_t* excl_path_bits, uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -345,6 +376,23 @@ int32_t og_groth16_prove_exclusion_dev(og_ctx* ctx, const og_pk* pk, const uint8
                                        const uint64_t* d_excl_low, const uint64_t* d_excl_next, const uint8_t* d_excl_siblings,
                                        const uint32_t* d_excl_path_bits, uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs,
                                        uint8_t* d_public_out);
+/* batch of labeled withdraw proofs, witness generation on the GPU; inputs as in og_labeled_witness.  OG_E_INVALID unless
+ * the key has a labeled statement's shape (the depth is recognised from it).  public_out (optional): batch * 7 * 32 B =
+ * root, nullifier_hash, recipient, exclusion_root, token, withdrawn, change_commitment. */
+int32_t og_groth16_prove_labeled(og_ctx* ctx, const og_pk* pk, const uint8_t* tokens, const uint8_t* recipients,
+                                 const uint64_t* withdrawn, const uint8_t* nullifiers, const uint8_t* secrets, const uint64_t* amounts,
+                                 const uint32_t* labels, const uint8_t* siblings, const uint32_t* path_bits,
+                                 const uint8_t* change_nullifiers, const uint8_t* change_secrets, const uint64_t* excl_low,
+                                 const uint64_t* excl_next, const uint8_t* excl_siblings, const uint32_t* excl_path_bits,
+                                 uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out);
+/* same with every buffer already in HBM; no synchronisation */
+int32_t og_groth16_prove_labeled_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_tokens, const uint8_t* d_recipients,
+                                     const uint64_t* d_withdrawn, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                     const uint64_t* d_amounts, const uint32_t* d_labels, const uint8_t* d_siblings,
+                                     const uint32_t* d_path_bits, const uint8_t* d_change_nullifiers,
+                                     const uint8_t* d_change_secrets, const uint64_t* d_excl_low, const uint64_t* d_excl_next,
+                                     const uint8_t* d_excl_siblings, const uint32_t* d_excl_path_bits, uint32_t batch,
+                                     const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

@@ -1,5 +1,5 @@
 """owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool deposit, withdraw, transfer, association-set
-withdraw and exclusion withdraw proofs over BN254, with encrypted delivery of the notes they create.
+withdraw, exclusion withdraw and labeled withdraw proofs over BN254, with encrypted delivery of the notes they create.
 
 Python is the host language here because the reference's (Rust) toolchain is absent from this image;
 everything below is a thin ctypes veneer over the C ABI in include/owshen_b200.h, which is the real
@@ -12,6 +12,7 @@ from .api import (Context, ProvingKey, MerkleTree, OwshenB200Error, lib, build_l
                   setup_transfer, transfer_r1cs_info, transfer_r1cs_export, FR_MODULUS, PROOF_BYTES,
                   setup_association, association_r1cs_info, association_r1cs_export, ptau_prepare_association,
                   ExclusionSet, setup_exclusion, exclusion_r1cs_info, exclusion_r1cs_export, ptau_prepare_exclusion,
+                  deposit_labeled, setup_labeled, labeled_r1cs_info, labeled_r1cs_export, ptau_prepare_labeled,
                   ptau_new, ptau_contribute, ptau_verify, ptau_prepare, ptau_prepare_withdraw, ptau_prepare_deposit,
                   ptau_prepare_transfer, phase2_contribute, phase2_verify, NOTE_SUBGROUP_ORDER, NOTE_NOT_OWNED, NOTE_MALFORMED)
 
@@ -22,4 +23,5 @@ __all__ = ["Context", "ProvingKey", "MerkleTree", "OwshenB200Error", "lib", "bui
            "ptau_prepare_transfer", "phase2_contribute", "phase2_verify",
            "setup_association", "association_r1cs_info", "association_r1cs_export", "ptau_prepare_association",
            "ExclusionSet", "setup_exclusion", "exclusion_r1cs_info", "exclusion_r1cs_export", "ptau_prepare_exclusion",
+           "deposit_labeled", "setup_labeled", "labeled_r1cs_info", "labeled_r1cs_export", "ptau_prepare_labeled",
            "NOTE_SUBGROUP_ORDER", "NOTE_NOT_OWNED", "NOTE_MALFORMED"]

@@ -106,6 +106,11 @@ _SIGS = {
     "og_exclusion_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_exclusion_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_exclusion_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p]),
+    "og_labeled_precommitments": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
+    "og_labeled_leaves": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 4 + [C.c_uint64, C.c_void_p]),
+    "og_labeled_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_labeled_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_labeled_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -124,6 +129,8 @@ _SIGS = {
     "og_groth16_prove_association_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_exclusion": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_exclusion_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_labeled": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_labeled_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -227,6 +234,15 @@ def _u32_array(xs):
     return xs if _blen(xs) is not None or isinstance(xs, int) else _bits_array(xs)
 
 
+def _label_array(xs):
+    """Labels as a buffer of little-endian uint32: bytes-like, a uint32 array / tensor, or a sequence of ints < 2^32."""
+    if _blen(xs) is not None or isinstance(xs, int):
+        return xs
+    vals = [int(x) for x in xs]
+    _need(all(0 <= x < 1 << 32 for x in vals), "labels must be integers in [0, 2^32)")
+    return (C.c_uint32 * len(vals))(*vals)
+
+
 # The statements' boundary, mirroring the statement table of csrc/mimc.cuh: statement -> (takes a depth, input arrays in C ABI
 # order as (name, bytes per proof, bytes per proof and tree level, conversion of a sequence of ints)).  The C entry points are
 # og_<statement>_r1cs_info / _r1cs_export / _witness and og_groth16_prove_<statement>(_dev).
@@ -243,6 +259,11 @@ _STATEMENTS = {
     "exclusion": (True, (("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("recipients", 32, 0, None), ("siblings", 0, 32, None),
                          ("path_bits", 4, 0, _u32_array), ("excl_low", 8, 0, _u64_array), ("excl_next", 8, 0, _u64_array),
                          ("excl_siblings", 0, 32, None), ("excl_path_bits", 4, 0, _u32_array))),
+    "labeled": (True, (("tokens", 32, 0, None), ("recipients", 32, 0, None), ("withdrawn", 8, 0, _u64_array), ("nullifiers", 32, 0, None),
+                       ("secrets", 32, 0, None), ("amounts", 8, 0, _u64_array), ("labels", 4, 0, _label_array), ("siblings", 0, 32, None),
+                       ("path_bits", 4, 0, _u32_array), ("change_nullifiers", 32, 0, None), ("change_secrets", 32, 0, None),
+                       ("excl_low", 8, 0, _u64_array), ("excl_next", 8, 0, _u64_array), ("excl_siblings", 0, 32, None),
+                       ("excl_path_bits", 4, 0, _u32_array))),
 }
 
 
@@ -598,6 +619,40 @@ class Context:
         return self._statement_witness("exclusion", depth, (nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next,
                                                             excl_siblings, excl_path_bits))
 
+    # ---- labeled notes (DESIGN.md section 3, "Labeled withdrawals") --------------------------------------------------
+    def labeled_precommitments(self, nullifiers: bytes, secrets: bytes) -> bytes:
+        """MultiMiMC7([nullifier, secret], 2) of each note (32 bytes each in and out): what a depositor sends the node."""
+        _need(len(nullifiers) % 32 == 0 and len(secrets) == len(nullifiers),
+              "labeled_precommitments: nullifiers and secrets must be equally long multiples of 32 bytes")
+        n = len(nullifiers) // 32
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_labeled_precommitments(self._h, nullifiers, secrets, n, out), self)
+        return out.raw
+
+    def labeled_leaves(self, precommitments: bytes, tokens: bytes, amounts, labels) -> bytes:
+        """MultiMiMC7([precommitment, token, amount, label], 2) of each deposit: precommitments and tokens 32 bytes each,
+        amounts uint64 and labels uint32 (little-endian buffers, arrays or sequences of ints)."""
+        _need(len(precommitments) % 32 == 0 and len(tokens) == len(precommitments),
+              "labeled_leaves: precommitments and tokens must be equally long multiples of 32 bytes")
+        n = len(precommitments) // 32
+        am, la = _u64_array(amounts), _label_array(labels)
+        for name, buf, size in (("amounts", am, 8), ("labels", la, 4)):
+            _need((C.sizeof(buf) if isinstance(buf, C.Array) else _blen(buf)) == size * n, f"labeled_leaves: expected one {name[:-1]} per deposit")
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_labeled_leaves(self._h, precommitments, tokens, _ptr(am), _ptr(la), n, out), self)
+        return out.raw
+
+    def labeled_witness(self, depth, tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+                        change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits) -> bytes:
+        """Full assignments of the depth-`depth` labeled withdraw statement, n_vars * 32 bytes per proof, computed on the GPU.
+        Per proof: token, recipient, nullifier, secret, change_nullifier, change_secret 32 bytes each; withdrawn, amount,
+        excl_low and excl_next one uint64 each and the label one uint32 (little-endian buffers, arrays or ints); siblings
+        and excl_siblings depth elements each (the note's pool path and the blocklist-tree path of its label,
+        ExclusionSet.witness), path_bits and excl_path_bits one word each."""
+        return self._statement_witness("labeled", depth, (tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings,
+                                                          path_bits, change_nullifiers, change_secrets, excl_low, excl_next,
+                                                          excl_siblings, excl_path_bits))
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -670,6 +725,15 @@ def exclusion_r1cs_export(depth: int, which: str):
     return _statement_r1cs_export("exclusion", depth, which)
 
 
+def labeled_r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("labeled", depth)
+
+
+def labeled_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` labeled withdraw R1CS."""
+    return _statement_r1cs_export("labeled", depth, which)
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -729,6 +793,12 @@ def setup_exclusion(ctx: Context, depth: int, tau: int, alpha: int, beta: int, g
     """Development setup of the depth-`depth` exclusion withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS through
     setup_r1cs.  The key records depth 0; the prover recognises it as an exclusion key by its shape."""
     return _setup_statement(ctx, "exclusion", depth, (tau, alpha, beta, gamma, delta))
+
+
+def setup_labeled(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` labeled withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS through
+    setup_r1cs.  The key records depth 0; the prover recognises it as a labeled key by its shape."""
+    return _setup_statement(ctx, "labeled", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -813,6 +883,10 @@ def ptau_prepare_association(ctx: Context, acc: bytes, depth: int):
 
 def ptau_prepare_exclusion(ctx: Context, acc: bytes, depth: int):
     return _ptau_prepare_statement(ctx, acc, "exclusion", depth)
+
+
+def ptau_prepare_labeled(ctx: Context, acc: bytes, depth: int):
+    return _ptau_prepare_statement(ctx, acc, "labeled", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -951,6 +1025,21 @@ class ProvingKey:
         return self._prove_statement("exclusion", self.exclusion_depth,
                                      (nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings,
                                       excl_path_bits), rs, want_public)
+
+    @property
+    def labeled_depth(self):
+        """The depth d whose labeled statement has this key's shape (labeled_r1cs_info), or None."""
+        return self._shape_depth("labeled")
+
+    def prove_labeled(self, tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits, change_nullifiers,
+                      change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits, rs, want_public=True):
+        """Batch of labeled withdraw proofs from the notes (witness generation on the GPU).  Inputs as in
+        Context.labeled_witness; returns (proofs, public_inputs) with public inputs (root, nullifier_hash, recipient,
+        exclusion_root, token, withdrawn, change_commitment) per proof."""
+        return self._prove_statement("labeled", self.labeled_depth,
+                                     (tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+                                      change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits), rs,
+                                     want_public)
 
     def prover_plan(self, batch: int) -> dict:
         """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and
@@ -1130,6 +1219,22 @@ class MerkleTree:
         len(indices) x depth x 32 bytes, proof-major, and one path_bits word per leaf."""
         got = [self.path(i) for i in indices]
         return b"".join(s for s, _ in got), [b for _, b in got]
+
+
+def deposit_labeled(tree: MerkleTree, precommitments: bytes, tokens: bytes, amounts):
+    """Append labeled deposits to the pool tree -> their labels.  The node assigns each deposit the next pool leaf index as
+    its label, computes the leaf MultiMiMC7([precommitment, token, amount, label], 2) on the GPU from what the depositor sent
+    (precommitments and tokens 32 bytes each, amounts uint64), and inserts the leaves in one insert_batch.  It never takes a
+    leaf from the depositor: a label it did not assign cannot enter the pool."""
+    _need(len(precommitments) % 32 == 0 and len(tokens) == len(precommitments),
+          "deposit_labeled: precommitments and tokens must be equally long multiples of 32 bytes")
+    n, start = len(precommitments) // 32, tree.n_leaves
+    if start + n > (1 << tree.depth):
+        raise OverflowError(f"tree of depth {tree.depth} holds {1 << tree.depth} leaves; {start} present, {n} more requested")
+    labels = list(range(start, start + n))
+    leaves = tree.ctx.labeled_leaves(precommitments, tokens, amounts, labels)
+    tree.insert_batch([leaves[32 * k:32 * k + 32] for k in range(n)])
+    return labels
 
 
 EXCLUSION_KEY_MAX = (1 << 32) + 1        # the blocklist tree's last key: above every note key (leaf index + 1 <= 2^32)

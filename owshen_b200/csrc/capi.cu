@@ -990,6 +990,52 @@ int32_t og_exclusion_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifi
                                                         excl_siblings, excl_path_bits}, batch, witnesses);
 }
 
+// ---- labeled notes and the labeled withdraw statement --------------------------------------------------------------
+int32_t og_labeled_precommitments(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !nullifiers || !secrets || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, ds, uint8_t, S_IO_B, 32 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_C, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dn, nullifiers, 32 * n); H2D(ctx, ds, secrets, 32 * n);
+    OG_TRY(labeled_precommitments_dev(ctx, dn, ds, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_labeled_leaves(og_ctx* ctx, const uint8_t* precommitments, const uint8_t* tokens, const uint64_t* amounts, const uint32_t* labels,
+                          uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !precommitments || !tokens || !amounts || !labels || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dp, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, dt, uint8_t, S_IO_B, 32 * n);
+    OG_SLOT(ctx, da, uint64_t, S_IO_C, 8 * n);
+    OG_SLOT(ctx, dl, uint32_t, S_IO_D, 4 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_E, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dp, precommitments, 32 * n); H2D(ctx, dt, tokens, 32 * n); H2D(ctx, da, amounts, 8 * n); H2D(ctx, dl, labels, 4 * n);
+    OG_TRY(labeled_leaves_dev(ctx, dp, dt, da, dl, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_labeled_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_LABELED, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_labeled_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    return statement_r1cs_export(ST_LABELED, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
+int32_t og_labeled_witness(og_ctx* ctx, uint32_t depth, const uint8_t* tokens, const uint8_t* recipients, const uint64_t* withdrawn,
+                           const uint8_t* nullifiers, const uint8_t* secrets, const uint64_t* amounts, const uint32_t* labels,
+                           const uint8_t* siblings, const uint32_t* path_bits, const uint8_t* change_nullifiers, const uint8_t* change_secrets,
+                           const uint64_t* excl_low, const uint64_t* excl_next, const uint8_t* excl_siblings, const uint32_t* excl_path_bits,
+                           uint32_t batch, uint8_t* witnesses) {
+    return statement_witness(ctx, ST_LABELED, depth, {tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+                                                      change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits},
+                             batch, witnesses);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1122,6 +1168,27 @@ int32_t og_groth16_prove_exclusion(og_ctx* ctx, const og_pk* pk, const uint8_t* 
                                    const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
     return statement_prove(ctx, pk, ST_EXCLUSION, {nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings,
                                                    excl_path_bits}, batch, rs, proofs, public_out);
+}
+
+int32_t og_groth16_prove_labeled_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_tokens, const uint8_t* d_recipients,
+                                     const uint64_t* d_withdrawn, const uint8_t* d_nullifiers, const uint8_t* d_secrets, const uint64_t* d_amounts,
+                                     const uint32_t* d_labels, const uint8_t* d_siblings, const uint32_t* d_path_bits,
+                                     const uint8_t* d_change_nullifiers, const uint8_t* d_change_secrets, const uint64_t* d_excl_low,
+                                     const uint64_t* d_excl_next, const uint8_t* d_excl_siblings, const uint32_t* d_excl_path_bits, uint32_t batch,
+                                     const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    return statement_prove_dev(ctx, pk, ST_LABELED, {d_tokens, d_recipients, d_withdrawn, d_nullifiers, d_secrets, d_amounts, d_labels, d_siblings,
+                                                     d_path_bits, d_change_nullifiers, d_change_secrets, d_excl_low, d_excl_next, d_excl_siblings,
+                                                     d_excl_path_bits}, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_labeled(og_ctx* ctx, const og_pk* pk, const uint8_t* tokens, const uint8_t* recipients, const uint64_t* withdrawn,
+                                 const uint8_t* nullifiers, const uint8_t* secrets, const uint64_t* amounts, const uint32_t* labels,
+                                 const uint8_t* siblings, const uint32_t* path_bits, const uint8_t* change_nullifiers,
+                                 const uint8_t* change_secrets, const uint64_t* excl_low, const uint64_t* excl_next, const uint8_t* excl_siblings,
+                                 const uint32_t* excl_path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
+    return statement_prove(ctx, pk, ST_LABELED, {tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+                                                 change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits},
+                           batch, rs, proofs, public_out);
 }
 
 int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {

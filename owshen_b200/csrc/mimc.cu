@@ -1,6 +1,7 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
-// paths (BASELINE config 2), level-by-level tree build, and the witness generators of the withdraw,
-// deposit, transfer, association and exclusion statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
+// paths (BASELINE config 2), level-by-level tree build, the labeled-note hashes, and the witness generators of the withdraw,
+// deposit, transfer, association, exclusion and labeled withdraw statements (every t^2, t^4, t^6, t^7 of every round is a
+// circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -289,18 +290,24 @@ __global__ void __launch_bounds__(64) k_association_witness(AssociationLayout L,
     }
 }
 
+constexpr uint64_t R_LO64 = 0x43e1f593f0000001ull;   // r mod 2^64
+
 // the 33 low bits of the canonical representative of (a - b - 1) mod r, for a, b < 2^64: when a <= b the difference is
 // r - (b + 1 - a), whose low 64 bits are r's low 64 bits minus (b + 1 - a), all mod 2^64
 __device__ __forceinline__ uint64_t gap_bits(uint64_t a, uint64_t b) {
-    constexpr uint64_t R_LO64 = 0x43e1f593f0000001ull;
     return a - b - 1 + (a > b ? 0 : R_LO64);
 }
 
-// the EXCLUSION_RANGE_BITS low bits of v as field elements 0 / 1, LSB first
-__device__ __forceinline__ void store_range_bits(Fr* out, uint64_t v) {
+// likewise the 64 low bits of the canonical (a - b) mod r
+__device__ __forceinline__ uint64_t diff_bits(uint64_t a, uint64_t b) {
+    return a - b + (a >= b ? 0 : R_LO64);
+}
+
+// the n_bits low bits of v as field elements 0 / 1, LSB first
+__device__ __forceinline__ void store_range_bits(Fr* out, uint64_t v, uint32_t n_bits = EXCLUSION_RANGE_BITS) {
     const Fr one = Fr::one(), zero = Fr::zero();
 #pragma unroll 1
-    for (uint32_t k = 0; k < EXCLUSION_RANGE_BITS; k++) out[k] = ((v >> k) & 1) ? one : zero;
+    for (uint32_t k = 0; k < n_bits; k++) out[k] = ((v >> k) & 1) ? one : zero;
 }
 
 // Witness of the exclusion withdraw statement, layout of DESIGN.md section 3 (== oracle/exclusion_circuit.py); row p starts
@@ -341,6 +348,113 @@ __global__ void __launch_bounds__(64) k_exclusion_witness(ExclusionLayout L, uin
     }
 }
 
+__device__ __forceinline__ Fr fr_from_u64(uint64_t v) {
+    const uint32_t c[8] = {(uint32_t)v, (uint32_t)(v >> 32), 0, 0, 0, 0, 0, 0};
+    return Fr::from_canonical(c);
+}
+
+// MultiMiMC7(xs, key): r = key; r = r + x + hash(x, r) per input.  The plain form runs the lazy chain of mimc_core.cuh; the
+// TRACE form stores every round value of the k-th permutation from trace + k * perm on.
+template <bool TRACE, int N>
+__device__ __forceinline__ Fr mimc7_multi_hash(const Fr (&xs)[N], const Fr& key, Fr* trace, uint32_t perm) {
+    Fr r = key;
+#pragma unroll
+    for (int k = 0; k < N; k++) {
+        const Fr h = TRACE ? mimc7_hash<true>(xs[k], r, trace + k * perm) : mimc7_perm_lazy<false>(xs[k], r, [](int i) { return mimc_c(i); });
+        r = r + xs[k] + h;
+    }
+    return r;
+}
+
+// Labeled notes (oracle/labeled_circuit.py), one thread per note: precommitment = MultiMiMC7([nullifier, secret], 2) for the
+// wallet, leaf = MultiMiMC7([precommitment, token, amount, label], 2) for the node
+__global__ void __launch_bounds__(64) k_labeled_precommitments(const uint8_t* __restrict__ nullifiers, const uint8_t* __restrict__ secrets,
+                                                               uint64_t n, uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[2] = {load_canonical<Fr>(nullifiers + 32 * i, flag), load_canonical<Fr>(secrets + 32 * i, flag)};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(LABELED_KEY), nullptr, 0));
+}
+
+__global__ void __launch_bounds__(64) k_labeled_leaves(const uint8_t* __restrict__ pre, const uint8_t* __restrict__ tokens,
+                                                       const uint64_t* __restrict__ amounts, const uint32_t* __restrict__ labels, uint64_t n,
+                                                       uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[4] = {load_canonical<Fr>(pre + 32 * i, flag), load_canonical<Fr>(tokens + 32 * i, flag), fr_from_u64(amounts[i]),
+                      Fr::from_u32(labels[i])};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(LABELED_KEY), nullptr, 0));
+}
+
+// Witness of the labeled withdraw statement, layout of DESIGN.md section 3 (== oracle/labeled_circuit.py); row p starts at
+// W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with three warps, one per independent chain of a proof, so no
+// warp diverges and a proof's critical path stays at about one withdraw path:
+//   warp 0   nullifier, secret, the precommitment and the leaf with their round values, the pool path, root: 70
+//            permutations at depth 32
+//   warp 1   low and next, the blocklist leaf MultiMiMC7([low, next], 0) with its round values, the exclusion path,
+//            exclusion_root: 66 permutations
+//   warp 2   the public and scalar inputs, the nullifier hash, the change precommitment and change_commitment with their
+//            round values (7 permutations), then every range bit from integer arithmetic
+// The warps write disjoint variables, so no barrier is needed.
+__global__ void __launch_bounds__(96) k_labeled_witness(LabeledLayout L, uint32_t w_stride, LabeledInputs in, uint32_t batch,
+                                                        Fr* __restrict__ W, int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    if (p >= batch) return;
+    Fr* w = W + (uint64_t)p * w_stride;
+    const Fr key = Fr::from_u32(LABELED_KEY);
+    if (role == 0) {
+        const Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
+        const Fr se = load_canonical<Fr>(in.secrets + 32ull * p, flag);
+        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+        w[8] = nu; w[9] = se;
+        const Fr note[2] = {nu, se};
+        const Fr pre = mimc7_multi_hash<true>(note, key, w + L.pre_base, L.perm);
+        w[L.pre_out] = pre;
+        const Fr leaf_in[4] = {pre, token, fr_from_u64(in.amounts[p]), Fr::from_u32(in.labels[p])};
+        const Fr leaf = mimc7_multi_hash<true>(leaf_in, key, w + L.leaf_base, L.perm);
+        w[L.leaf_out] = leaf;
+        w[1] = witness_path(leaf, w + L.pool_base, L.depth, L.lvl_size, L.perm, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
+    } else if (role == 1) {
+        const Fr lo = fr_from_u64(in.low[p]), nx = fr_from_u64(in.next[p]);
+        w[15] = lo; w[16] = nx;
+        const Fr leaf = mimc7_hash2<true>(lo, nx, w + L.xleaf_base, w + L.xleaf_base + L.perm);
+        w[L.xleaf_out] = leaf;
+        w[4] = witness_path(leaf, w + L.excl_base, L.depth, L.lvl_size, L.perm, in.excl_siblings + 32ull * L.depth * p,
+                            in.excl_path_bits[p], flag);
+    } else {
+        const Fr one = Fr::one();
+        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+        const Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+        const Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
+        const Fr cnu = load_canonical<Fr>(in.change_nullifiers + 32ull * p, flag);
+        const Fr cse = load_canonical<Fr>(in.change_secrets + 32ull * p, flag);
+        const uint64_t amount = in.amounts[p], wd = in.withdrawn[p], lo = in.low[p], nx = in.next[p];
+        const uint32_t label = in.labels[p];
+        const Fr am = fr_from_u64(amount), fwd = fr_from_u64(wd), la = Fr::from_u32(label), change = am - fwd;
+        w[0] = one; w[3] = re; w[5] = token; w[6] = fwd;
+        w[10] = re.sqr();
+        w[11] = am; w[12] = la; w[13] = cnu; w[14] = cse;
+        // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
+        w[2] = one + nu + mimc7_hash<true>(nu, one, w + 17);
+        const Fr cnote[2] = {cnu, cse};
+        const Fr cpre = mimc7_multi_hash<true>(cnote, key, w + L.cpre_base, L.perm);
+        w[L.cpre_out] = cpre;
+        const Fr ccm_in[4] = {cpre, token, change, la};
+        w[7] = mimc7_multi_hash<true>(ccm_in, key, w + L.ccm_base, L.perm);
+        // the range bits; x = label + 1 <= 2^32
+        const uint64_t x = (uint64_t)label + 1;
+        store_range_bits(w + L.amount_bits, amount, LABELED_AMOUNT_BITS);
+        store_range_bits(w + L.withdrawn_bits, wd, LABELED_AMOUNT_BITS);
+        store_range_bits(w + L.change_bits, diff_bits(amount, wd), LABELED_AMOUNT_BITS);
+        store_range_bits(w + L.label_bits, label, LABELED_LABEL_BITS);
+        store_range_bits(w + L.low_bits, lo);
+        store_range_bits(w + L.next_bits, nx);
+        store_range_bits(w + L.gap_lo_bits, gap_bits(x, lo));
+        store_range_bits(w + L.gap_hi_bits, gap_bits(nx, x));
+    }
+}
+
 // ---- host side ------------------------------------------------------------------------------------
 void mimc_constants_host(Fr* out91) { mimc7_round_constants(out91); }
 
@@ -375,6 +489,19 @@ int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_o
     return OG_OK;
 }
 
+int32_t labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_nullifiers, const uint8_t* d_secrets, uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_labeled_precommitments, (unsigned)((n + 63) / 64), 64, 0, d_nullifiers, d_secrets, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint32_t* d_labels,
+                           uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_labeled_leaves, (unsigned)((n + 63) / 64), 64, 0, d_pre, d_tokens, d_amounts, d_labels, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
 // levels: Montgomery-form buffer holding n + n/2 + ... + 1 elements, level 0 already filled
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves) {
     Fr* in = d_levels;
@@ -400,8 +527,8 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
     return OG_OK;
 }
 
-// One CTA covers 32 proofs in every statement's kernel; the transfer, association and exclusion kernels give a proof more than
-// one warp.
+// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion and labeled kernels give a proof
+// more than one warp.
 int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
                               Fr* d_W) {
     if (batch == 0) return OG_OK;
@@ -431,6 +558,13 @@ int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t
         const ExclusionInputs t{a[0], a[1], a[2], a[3], (const uint32_t*)a[4], (const uint64_t*)a[5], (const uint64_t*)a[6], a[7],
                                 (const uint32_t*)a[8]};
         OG_LAUNCH(ctx, k_exclusion_witness, grid, 64, 0, ExclusionLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
+        break;
+    }
+    case ST_LABELED: {
+        const LabeledInputs t{a[0], a[1], (const uint64_t*)a[2], a[3], a[4], (const uint64_t*)a[5], (const uint32_t*)a[6], a[7],
+                              (const uint32_t*)a[8], a[9], a[10], (const uint64_t*)a[11], (const uint64_t*)a[12], a[13],
+                              (const uint32_t*)a[14]};
+        OG_LAUNCH(ctx, k_labeled_witness, grid, 96, 0, LabeledLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
         break;
     }
     }

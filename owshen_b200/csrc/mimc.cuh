@@ -1,7 +1,7 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit, transfer, association and exclusion statements (DESIGN.md section 3; must equal
+// withdraw, deposit, transfer, association, exclusion and labeled withdraw statements (DESIGN.md section 3; must equal
 // oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout,
-// oracle/association_circuit.py: Layout and oracle/exclusion_circuit.py: Layout).
+// oracle/association_circuit.py: Layout, oracle/exclusion_circuit.py: Layout and oracle/labeled_circuit.py: Layout).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -159,12 +159,75 @@ struct ExclusionInputs {
     const uint32_t* excl_path_bits;
 };
 
+constexpr uint32_t LABELED_N_PUB = 7;
+constexpr uint32_t LABELED_KEY = 2;            // MultiMiMC7 key of labeled precommitments and leaves (0: commitments, nodes; 1: nullifiers)
+constexpr uint32_t LABELED_AMOUNT_BITS = 64, LABELED_LABEL_BITS = 32;
+
+// 0 ONE | 1 root | 2 nullifier_hash | 3 recipient | 4 exclusion_root | 5 token | 6 withdrawn | 7 change_commitment
+// | 8 nullifier | 9 secret | 10 recipient_sq | 11 amount | 12 label | 13 change_nullifier | 14 change_secret | 15 low | 16 next
+// | 17.. nullifier-hash permutation | precommitment perm1, perm2, out | leaf perm[4], out | depth pool levels
+// | amount, withdrawn, change bits (64 each), label bits (32), low, next, gap_lo, gap_hi bits (33 each; all LSB first)
+// | change precommitment perm1, perm2, out | change commitment perm[4] | blocklist leaf perm1, perm2, out | depth exclusion
+// levels (oracle/labeled_circuit.py); a level block is the withdraw statement's.
+struct LabeledLayout {
+    uint32_t depth, perm, pre_base, pre_out, leaf_base, leaf_out, pool_base, amount_bits, withdrawn_bits, change_bits, label_bits,
+        low_bits, next_bits, gap_lo_bits, gap_hi_bits, cpre_base, cpre_out, ccm_base, xleaf_base, xleaf_out, excl_base, lvl_size,
+        n_vars, n_constraints;
+    static LabeledLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        LabeledLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        const uint32_t P = L.perm;
+        L.lvl_size = 2 * P + 4;
+        L.pre_base = 17 + P;
+        L.pre_out = L.pre_base + 2 * P;
+        L.leaf_base = L.pre_out + 1;
+        L.leaf_out = L.leaf_base + 4 * P;
+        L.pool_base = L.leaf_out + 1;
+        L.amount_bits = L.pool_base + depth * L.lvl_size;
+        L.withdrawn_bits = L.amount_bits + LABELED_AMOUNT_BITS;
+        L.change_bits = L.withdrawn_bits + LABELED_AMOUNT_BITS;
+        L.label_bits = L.change_bits + LABELED_AMOUNT_BITS;
+        L.low_bits = L.label_bits + LABELED_LABEL_BITS;
+        L.next_bits = L.low_bits + EXCLUSION_RANGE_BITS;
+        L.gap_lo_bits = L.next_bits + EXCLUSION_RANGE_BITS;
+        L.gap_hi_bits = L.gap_lo_bits + EXCLUSION_RANGE_BITS;
+        L.cpre_base = L.gap_hi_bits + EXCLUSION_RANGE_BITS;
+        L.cpre_out = L.cpre_base + 2 * P;
+        L.ccm_base = L.cpre_out + 1;
+        L.xleaf_base = L.ccm_base + 4 * P;
+        L.xleaf_out = L.xleaf_base + 2 * P;
+        L.excl_base = L.xleaf_out + 1;
+        L.n_vars = L.excl_base + depth * L.lvl_size;
+        L.n_constraints = 373 + 15 * P + depth * (4 * P + 6);
+        return L;
+    }
+};
+
+// the caller's inputs of a batch of labeled withdrawals (k_labeled_witness's argument), in C ABI order; per proof: token and
+// recipient 32 B each, withdrawn (u64), nullifier and secret 32 B each, amount (u64), label (u32), depth pool siblings and a
+// path-bits word, change nullifier and change secret 32 B each, the blocklist leaf's keys low and next (u64), depth
+// blocklist-tree siblings and a path-bits word
+struct LabeledInputs {
+    const uint8_t *tokens, *recipients;
+    const uint64_t* withdrawn;
+    const uint8_t *nullifiers, *secrets;
+    const uint64_t* amounts;
+    const uint32_t* labels;
+    const uint8_t* siblings;
+    const uint32_t* path_bits;
+    const uint8_t *change_nullifiers, *change_secrets;
+    const uint64_t *low, *next;
+    const uint8_t* excl_siblings;
+    const uint32_t* excl_path_bits;
+};
+
 // ---- the statement table ------------------------------------------------------------------------------------------------
 // What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
 // statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
 // statement_witness_dev) and its og_* forwarders (capi.cu).
-enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION };
-constexpr uint32_t STATEMENT_MAX_INPUTS = 11;
+enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED };
+constexpr uint32_t STATEMENT_MAX_INPUTS = 15;
 
 struct StatementShape { uint32_t n_vars, n_constraints; };
 template <class Layout> StatementShape layout_shape(uint32_t depth) { const Layout L = Layout::make(depth); return {L.n_vars, L.n_constraints}; }
@@ -192,6 +255,10 @@ constexpr StatementDesc STATEMENTS[] = {
     {ASSOCIATION_N_PUB, layout_shape<AssociationLayout>, true, 7, {32, 32, 32, 0, 4, 0, 4}, {0, 0, 0, 32, 0, 32, 0}},
     // exclusion: nullifiers, secrets, recipients, siblings, path_bits, excl_low, excl_next, excl_siblings, excl_path_bits
     {EXCLUSION_N_PUB, layout_shape<ExclusionLayout>, true, 9, {32, 32, 32, 0, 4, 8, 8, 0, 4}, {0, 0, 0, 32, 0, 0, 0, 32, 0}},
+    // labeled: tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits, change_nullifiers,
+    // change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits
+    {LABELED_N_PUB, layout_shape<LabeledLayout>, true, 15, {32, 32, 8, 32, 32, 8, 4, 0, 4, 32, 32, 8, 8, 0, 4},
+     {0, 0, 0, 0, 0, 0, 0, 32, 0, 0, 0, 0, 0, 32, 0}},
 };
 
 // the input arrays of a batch in the statement's C ABI order (host or device pointers)
@@ -213,6 +280,10 @@ struct StatementInputs {
 int32_t mimc_hash2_dev(og_ctx* ctx, const uint8_t* d_l, const uint8_t* d_r, uint64_t n, uint8_t* d_out);
 int32_t mimc_merkle_paths_dev(og_ctx* ctx, const uint8_t* d_leaves, const uint8_t* d_siblings, const uint32_t* d_bits,
                               uint32_t n_paths, uint32_t depth, uint8_t* d_out);
+// labeled notes (oracle/labeled_circuit.py): MultiMiMC7([nullifier, secret], 2) and MultiMiMC7([pre, token, amount, label], 2)
+int32_t labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_nullifiers, const uint8_t* d_secrets, uint64_t n, uint8_t* d_out);
+int32_t labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint32_t* d_labels,
+                           uint64_t n, uint8_t* d_out);
 int32_t mimc_to_mont_dev(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Fr* d_out);
 int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_out);
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves);
