@@ -287,6 +287,29 @@ int32_t og_labeled_witness(og_ctx* ctx, uint32_t depth, const uint8_t* tokens, c
                            const uint8_t* change_secrets, const uint64_t* excl_low, const uint64_t* excl_next,
                            const uint8_t* excl_siblings, const uint32_t* excl_path_bits, uint32_t batch, uint8_t* witnesses);
 
+/* ---- the labeled association withdraw statement (DESIGN.md section 3): partial withdrawals of labeled notes whose deposit
+ * is on a provider's approved list ---- */
+/* Public inputs (root, nullifier_hash, recipient, association_root, token, withdrawn, change_commitment).  The labeled
+ * statement's note part (leaf under root, 64-bit ranges on amount, withdrawn and change, 32-bit range on the label, the
+ * change note's commitment under the same label); then assoc_leaf = label + 1 reaches association_root in the provider's
+ * tree of approved labels (leaf L + 1 per approved label L, every other leaf 0; same depth as the pool's, 1..32).  At depth
+ * 32: 51 823 variables, 51 753 constraints, domain 2^16. */
+int32_t og_labeled_association_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_labeled_association_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                           uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: token, recipient 32 B each; withdrawn (uint64);
+ * nullifier, secret 32 B each; amount (uint64); label (uint32); siblings depth * 32 B and path_bits one word (the note's
+ * pool path); change_nullifier, change_secret 32 B each; assoc_siblings depth * 32 B and assoc_path_bits one word (the path
+ * of the label's leaf in the approved-label tree).  Path words: bit l set when the level-l node is a right child, only the
+ * low depth bits count.  Both roots, the nullifier hash, assoc_leaf and change_commitment are derived; an overdraw or an
+ * unapproved label gives a witness that does not satisfy the R1CS. */
+int32_t og_labeled_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* tokens, const uint8_t* recipients,
+                                       const uint64_t* withdrawn, const uint8_t* nullifiers, const uint8_t* secrets,
+                                       const uint64_t* amounts, const uint32_t* labels, const uint8_t* siblings, const uint32_t* path_bits,
+                                       const uint8_t* change_nullifiers, const uint8_t* change_secrets, const uint8_t* assoc_siblings,
+                                       const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -393,6 +416,23 @@ int32_t og_groth16_prove_labeled_dev(og_ctx* ctx, const og_pk* pk, const uint8_t
                                      const uint8_t* d_change_secrets, const uint64_t* d_excl_low, const uint64_t* d_excl_next,
                                      const uint8_t* d_excl_siblings, const uint32_t* d_excl_path_bits, uint32_t batch,
                                      const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of labeled association withdraw proofs, witness generation on the GPU; inputs as in og_labeled_association_witness.
+ * OG_E_INVALID unless the key has a labeled association statement's shape (the depth is recognised from it).  public_out
+ * (optional): batch * 7 * 32 B = root, nullifier_hash, recipient, association_root, token, withdrawn, change_commitment. */
+int32_t og_groth16_prove_labeled_association(og_ctx* ctx, const og_pk* pk, const uint8_t* tokens, const uint8_t* recipients,
+                                             const uint64_t* withdrawn, const uint8_t* nullifiers, const uint8_t* secrets,
+                                             const uint64_t* amounts, const uint32_t* labels, const uint8_t* siblings,
+                                             const uint32_t* path_bits, const uint8_t* change_nullifiers, const uint8_t* change_secrets,
+                                             const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch,
+                                             const uint8_t* rs, uint8_t* proofs, uint8_t* public_out);
+/* same with every buffer already in HBM; no synchronisation */
+int32_t og_groth16_prove_labeled_association_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_tokens, const uint8_t* d_recipients,
+                                                 const uint64_t* d_withdrawn, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                                 const uint64_t* d_amounts, const uint32_t* d_labels, const uint8_t* d_siblings,
+                                                 const uint32_t* d_path_bits, const uint8_t* d_change_nullifiers,
+                                                 const uint8_t* d_change_secrets, const uint8_t* d_assoc_siblings,
+                                                 const uint32_t* d_assoc_path_bits, uint32_t batch, const uint8_t* d_rs,
+                                                 uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

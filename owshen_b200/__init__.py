@@ -1,5 +1,6 @@
 """owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool deposit, withdraw, transfer, association-set
-withdraw, exclusion withdraw and labeled withdraw proofs over BN254, with encrypted delivery of the notes they create.
+withdraw, exclusion withdraw, labeled withdraw and labeled association withdraw proofs over BN254, with encrypted delivery
+of the notes they create.
 
 Python is the host language here because the reference's (Rust) toolchain is absent from this image;
 everything below is a thin ctypes veneer over the C ABI in include/owshen_b200.h, which is the real
@@ -13,6 +14,8 @@ from .api import (Context, ProvingKey, MerkleTree, OwshenB200Error, lib, build_l
                   setup_association, association_r1cs_info, association_r1cs_export, ptau_prepare_association,
                   ExclusionSet, setup_exclusion, exclusion_r1cs_info, exclusion_r1cs_export, ptau_prepare_exclusion,
                   deposit_labeled, setup_labeled, labeled_r1cs_info, labeled_r1cs_export, ptau_prepare_labeled,
+                  ApprovedLabels, setup_labeled_association, labeled_association_r1cs_info, labeled_association_r1cs_export,
+                  ptau_prepare_labeled_association,
                   ptau_new, ptau_contribute, ptau_verify, ptau_prepare, ptau_prepare_withdraw, ptau_prepare_deposit,
                   ptau_prepare_transfer, phase2_contribute, phase2_verify, NOTE_SUBGROUP_ORDER, NOTE_NOT_OWNED, NOTE_MALFORMED)
 
@@ -24,4 +27,6 @@ __all__ = ["Context", "ProvingKey", "MerkleTree", "OwshenB200Error", "lib", "bui
            "setup_association", "association_r1cs_info", "association_r1cs_export", "ptau_prepare_association",
            "ExclusionSet", "setup_exclusion", "exclusion_r1cs_info", "exclusion_r1cs_export", "ptau_prepare_exclusion",
            "deposit_labeled", "setup_labeled", "labeled_r1cs_info", "labeled_r1cs_export", "ptau_prepare_labeled",
+           "ApprovedLabels", "setup_labeled_association", "labeled_association_r1cs_info", "labeled_association_r1cs_export",
+           "ptau_prepare_labeled_association",
            "NOTE_SUBGROUP_ORDER", "NOTE_NOT_OWNED", "NOTE_MALFORMED"]

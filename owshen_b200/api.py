@@ -111,6 +111,9 @@ _SIGS = {
     "og_labeled_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_labeled_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_labeled_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p]),
+    "og_labeled_association_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_labeled_association_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_labeled_association_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 13 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -131,6 +134,9 @@ _SIGS = {
     "og_groth16_prove_exclusion_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_labeled": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_labeled_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_labeled_association": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 13 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_labeled_association_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 13
+                                                 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -264,6 +270,11 @@ _STATEMENTS = {
                        ("path_bits", 4, 0, _u32_array), ("change_nullifiers", 32, 0, None), ("change_secrets", 32, 0, None),
                        ("excl_low", 8, 0, _u64_array), ("excl_next", 8, 0, _u64_array), ("excl_siblings", 0, 32, None),
                        ("excl_path_bits", 4, 0, _u32_array))),
+    "labeled_association": (True, (("tokens", 32, 0, None), ("recipients", 32, 0, None), ("withdrawn", 8, 0, _u64_array),
+                                   ("nullifiers", 32, 0, None), ("secrets", 32, 0, None), ("amounts", 8, 0, _u64_array),
+                                   ("labels", 4, 0, _label_array), ("siblings", 0, 32, None), ("path_bits", 4, 0, _u32_array),
+                                   ("change_nullifiers", 32, 0, None), ("change_secrets", 32, 0, None), ("assoc_siblings", 0, 32, None),
+                                   ("assoc_path_bits", 4, 0, _u32_array))),
 }
 
 
@@ -653,6 +664,15 @@ class Context:
                                                           path_bits, change_nullifiers, change_secrets, excl_low, excl_next,
                                                           excl_siblings, excl_path_bits))
 
+    def labeled_association_witness(self, depth, tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings,
+                                    path_bits, change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits) -> bytes:
+        """Full assignments of the depth-`depth` labeled association withdraw statement, n_vars * 32 bytes per proof, computed
+        on the GPU.  The first eleven inputs as in labeled_witness; assoc_siblings depth elements and assoc_path_bits one word
+        per proof (the path of the label's leaf in the provider's tree, ApprovedLabels.witness)."""
+        return self._statement_witness("labeled_association", depth, (tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels,
+                                                                      siblings, path_bits, change_nullifiers, change_secrets,
+                                                                      assoc_siblings, assoc_path_bits))
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -734,6 +754,15 @@ def labeled_r1cs_export(depth: int, which: str):
     return _statement_r1cs_export("labeled", depth, which)
 
 
+def labeled_association_r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("labeled_association", depth)
+
+
+def labeled_association_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` labeled association R1CS."""
+    return _statement_r1cs_export("labeled_association", depth, which)
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -799,6 +828,12 @@ def setup_labeled(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gam
     """Development setup of the depth-`depth` labeled withdraw statement -> (pk_bytes, vk_bytes): its exported R1CS through
     setup_r1cs.  The key records depth 0; the prover recognises it as a labeled key by its shape."""
     return _setup_statement(ctx, "labeled", depth, (tau, alpha, beta, gamma, delta))
+
+
+def setup_labeled_association(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` labeled association withdraw statement -> (pk_bytes, vk_bytes): its exported
+    R1CS through setup_r1cs.  The key records depth 0; the prover recognises it as a labeled association key by its shape."""
+    return _setup_statement(ctx, "labeled_association", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -887,6 +922,10 @@ def ptau_prepare_exclusion(ctx: Context, acc: bytes, depth: int):
 
 def ptau_prepare_labeled(ctx: Context, acc: bytes, depth: int):
     return _ptau_prepare_statement(ctx, acc, "labeled", depth)
+
+
+def ptau_prepare_labeled_association(ctx: Context, acc: bytes, depth: int):
+    return _ptau_prepare_statement(ctx, acc, "labeled_association", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -1040,6 +1079,20 @@ class ProvingKey:
                                      (tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
                                       change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits), rs,
                                      want_public)
+
+    @property
+    def labeled_association_depth(self):
+        """The depth d whose labeled association statement has this key's shape (labeled_association_r1cs_info), or None."""
+        return self._shape_depth("labeled_association")
+
+    def prove_labeled_association(self, tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+                                  change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits, rs, want_public=True):
+        """Batch of labeled association withdraw proofs from the notes (witness generation on the GPU).  Inputs as in
+        Context.labeled_association_witness; returns (proofs, public_inputs) with public inputs (root, nullifier_hash,
+        recipient, association_root, token, withdrawn, change_commitment) per proof."""
+        return self._prove_statement("labeled_association", self.labeled_association_depth,
+                                     (tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+                                      change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits), rs, want_public)
 
     def prover_plan(self, batch: int) -> dict:
         """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and
@@ -1283,3 +1336,50 @@ class ExclusionSet:
         js = [bisect.bisect_left(self.keys, i + 1) - 1 for i in indices]
         sibs, bits = self.tree.paths(js)
         return [self.keys[j] for j in js], [self.keys[j + 1] for j in js], sibs, bits
+
+
+class ApprovedLabels:
+    """A compliance provider's approved deposits as the labeled association statement's tree (DESIGN.md section 3).
+
+    The approved labels (pool leaf indices, validated into [0, 2^depth), deduplicated and sorted) give the leaves label + 1,
+    32 bytes little-endian, appended by one MerkleTree.insert_batch of the pool's depth, so the tree is hashed on the GPU;
+    every other leaf is 0.  approve(labels) appends the labels not yet approved in one more insert_batch: a provider clears
+    deposits as they arrive, and only the new leaves' ancestors are hashed.  witness(labels) gives what
+    prove_labeled_association takes for approved labels."""
+
+    def __init__(self, ctx: Context, depth: int, labels, store=None):
+        _need(1 <= depth <= 32, "ApprovedLabels: depth must be in 1..32")
+        self.depth = depth
+        self.labels = []                                  # in leaf order
+        self._leaf = {}                                   # label -> its leaf index
+        self.tree = MerkleTree(ctx, depth, store, prefix=b"al/")
+        _need(self.tree.n_leaves == 0, "ApprovedLabels: the store already holds an approved-label tree")
+        self.approve(labels)
+
+    def approve(self, labels):
+        """Append the labels not yet approved (sorted) -> them."""
+        labels = [int(x) for x in labels]
+        _need(all(0 <= x < 1 << self.depth for x in labels), f"ApprovedLabels: labels are pool leaf indices in [0, 2^{self.depth})")
+        new = sorted(set(x for x in labels if x not in self._leaf))
+        self.tree.insert_batch([(x + 1).to_bytes(32, "little") for x in new])
+        for x in new:
+            self._leaf[x] = len(self.labels)
+            self.labels.append(x)
+        return new
+
+    def root(self) -> bytes:
+        return self.tree.root()
+
+    def __contains__(self, label) -> bool:
+        return label in self._leaf
+
+    def __len__(self) -> int:
+        return len(self.labels)
+
+    def witness(self, labels):
+        """(assoc_siblings, assoc_path_bits) for notes of `labels`: the paths of their leaves (len(labels) x depth x 32 bytes)
+        and path words.  ValueError names every label that is not approved."""
+        labels = [int(x) for x in labels]
+        bad = sorted(set(x for x in labels if x not in self._leaf))
+        _need(not bad, f"ApprovedLabels.witness: labels {bad} are not approved")
+        return self.tree.paths([self._leaf[x] for x in labels])

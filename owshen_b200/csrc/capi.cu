@@ -1036,6 +1036,24 @@ int32_t og_labeled_witness(og_ctx* ctx, uint32_t depth, const uint8_t* tokens, c
                              batch, witnesses);
 }
 
+// ---- labeled association withdraw statement -------------------------------------------------------------------------
+int32_t og_labeled_association_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_LABELED_ASSOCIATION, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_labeled_association_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                           uint64_t* nnz) {
+    return statement_r1cs_export(ST_LABELED_ASSOCIATION, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
+int32_t og_labeled_association_witness(og_ctx* ctx, uint32_t depth, const uint8_t* tokens, const uint8_t* recipients,
+                                       const uint64_t* withdrawn, const uint8_t* nullifiers, const uint8_t* secrets,
+                                       const uint64_t* amounts, const uint32_t* labels, const uint8_t* siblings, const uint32_t* path_bits,
+                                       const uint8_t* change_nullifiers, const uint8_t* change_secrets, const uint8_t* assoc_siblings,
+                                       const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses) {
+    return statement_witness(ctx, ST_LABELED_ASSOCIATION, depth, {tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels,
+                                                                  siblings, path_bits, change_nullifiers, change_secrets, assoc_siblings,
+                                                                  assoc_path_bits}, batch, witnesses);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1188,6 +1206,29 @@ int32_t og_groth16_prove_labeled(og_ctx* ctx, const og_pk* pk, const uint8_t* to
                                  const uint32_t* excl_path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
     return statement_prove(ctx, pk, ST_LABELED, {tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
                                                  change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits},
+                           batch, rs, proofs, public_out);
+}
+
+int32_t og_groth16_prove_labeled_association_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_tokens, const uint8_t* d_recipients,
+                                                 const uint64_t* d_withdrawn, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                                                 const uint64_t* d_amounts, const uint32_t* d_labels, const uint8_t* d_siblings,
+                                                 const uint32_t* d_path_bits, const uint8_t* d_change_nullifiers,
+                                                 const uint8_t* d_change_secrets, const uint8_t* d_assoc_siblings,
+                                                 const uint32_t* d_assoc_path_bits, uint32_t batch, const uint8_t* d_rs,
+                                                 uint8_t* d_proofs, uint8_t* d_public_out) {
+    return statement_prove_dev(ctx, pk, ST_LABELED_ASSOCIATION, {d_tokens, d_recipients, d_withdrawn, d_nullifiers, d_secrets, d_amounts,
+                                                                 d_labels, d_siblings, d_path_bits, d_change_nullifiers, d_change_secrets,
+                                                                 d_assoc_siblings, d_assoc_path_bits}, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_labeled_association(og_ctx* ctx, const og_pk* pk, const uint8_t* tokens, const uint8_t* recipients,
+                                             const uint64_t* withdrawn, const uint8_t* nullifiers, const uint8_t* secrets,
+                                             const uint64_t* amounts, const uint32_t* labels, const uint8_t* siblings,
+                                             const uint32_t* path_bits, const uint8_t* change_nullifiers, const uint8_t* change_secrets,
+                                             const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits, uint32_t batch,
+                                             const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
+    return statement_prove(ctx, pk, ST_LABELED_ASSOCIATION, {tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings,
+                                                             path_bits, change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits},
                            batch, rs, proofs, public_out);
 }
 

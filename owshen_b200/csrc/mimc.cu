@@ -1,7 +1,7 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
 // paths (BASELINE config 2), level-by-level tree build, the labeled-note hashes, and the witness generators of the withdraw,
-// deposit, transfer, association, exclusion and labeled withdraw statements (every t^2, t^4, t^6, t^7 of every round is a
-// circuit variable).
+// deposit, transfer, association, exclusion, labeled and labeled association withdraw statements (every t^2, t^4, t^6, t^7 of
+// every round is a circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -386,15 +386,62 @@ __global__ void __launch_bounds__(64) k_labeled_leaves(const uint8_t* __restrict
     store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(LABELED_KEY), nullptr, 0));
 }
 
+// The labeled note's part of the labeled and labeled association witnesses, whose layouts and inputs share the names it
+// reads.  labeled_note_witness: nullifier, secret, the precommitment and the leaf with their round values, the pool path,
+// root (70 permutations at depth 32).  labeled_change_witness: the public and scalar inputs but variable 4 (the exclusion or
+// association root) and variables 15 on, the nullifier hash, the change precommitment and change_commitment with their round
+// values (7 permutations), then the amount, withdrawn, change and label bits from integer arithmetic.
+template <class Layout, class Inputs>
+__device__ __forceinline__ void labeled_note_witness(const Layout& L, Fr* w, const Inputs& in, uint32_t p, int* flag) {
+    const Fr key = Fr::from_u32(LABELED_KEY);
+    const Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
+    const Fr se = load_canonical<Fr>(in.secrets + 32ull * p, flag);
+    const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+    w[8] = nu; w[9] = se;
+    const Fr note[2] = {nu, se};
+    const Fr pre = mimc7_multi_hash<true>(note, key, w + L.pre_base, L.perm);
+    w[L.pre_out] = pre;
+    const Fr leaf_in[4] = {pre, token, fr_from_u64(in.amounts[p]), Fr::from_u32(in.labels[p])};
+    const Fr leaf = mimc7_multi_hash<true>(leaf_in, key, w + L.leaf_base, L.perm);
+    w[L.leaf_out] = leaf;
+    w[1] = witness_path(leaf, w + L.pool_base, L.depth, L.lvl_size, L.perm, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
+}
+
+template <class Layout, class Inputs>
+__device__ __forceinline__ void labeled_change_witness(const Layout& L, Fr* w, const Inputs& in, uint32_t p, int* flag) {
+    const Fr key = Fr::from_u32(LABELED_KEY);
+    const Fr one = Fr::one();
+    const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+    const Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+    const Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
+    const Fr cnu = load_canonical<Fr>(in.change_nullifiers + 32ull * p, flag);
+    const Fr cse = load_canonical<Fr>(in.change_secrets + 32ull * p, flag);
+    const uint64_t amount = in.amounts[p], wd = in.withdrawn[p];
+    const uint32_t label = in.labels[p];
+    const Fr am = fr_from_u64(amount), fwd = fr_from_u64(wd), la = Fr::from_u32(label), change = am - fwd;
+    w[0] = one; w[3] = re; w[5] = token; w[6] = fwd;
+    w[10] = re.sqr();
+    w[11] = am; w[12] = la; w[13] = cnu; w[14] = cse;
+    // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
+    w[2] = one + nu + mimc7_hash<true>(nu, one, w + L.pre_base - L.perm);
+    const Fr cnote[2] = {cnu, cse};
+    const Fr cpre = mimc7_multi_hash<true>(cnote, key, w + L.cpre_base, L.perm);
+    w[L.cpre_out] = cpre;
+    const Fr ccm_in[4] = {cpre, token, change, la};
+    w[7] = mimc7_multi_hash<true>(ccm_in, key, w + L.ccm_base, L.perm);
+    store_range_bits(w + L.amount_bits, amount, LABELED_AMOUNT_BITS);
+    store_range_bits(w + L.withdrawn_bits, wd, LABELED_AMOUNT_BITS);
+    store_range_bits(w + L.change_bits, diff_bits(amount, wd), LABELED_AMOUNT_BITS);
+    store_range_bits(w + L.label_bits, label, LABELED_LABEL_BITS);
+}
+
 // Witness of the labeled withdraw statement, layout of DESIGN.md section 3 (== oracle/labeled_circuit.py); row p starts at
 // W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with three warps, one per independent chain of a proof, so no
 // warp diverges and a proof's critical path stays at about one withdraw path:
-//   warp 0   nullifier, secret, the precommitment and the leaf with their round values, the pool path, root: 70
-//            permutations at depth 32
+//   warp 0   labeled_note_witness: 70 permutations at depth 32
 //   warp 1   low and next, the blocklist leaf MultiMiMC7([low, next], 0) with its round values, the exclusion path,
 //            exclusion_root: 66 permutations
-//   warp 2   the public and scalar inputs, the nullifier hash, the change precommitment and change_commitment with their
-//            round values (7 permutations), then every range bit from integer arithmetic
+//   warp 2   the low, next, gap_lo and gap_hi bits, then labeled_change_witness (7 permutations)
 // The warps write disjoint variables, so no barrier is needed.
 __global__ void __launch_bounds__(96) k_labeled_witness(LabeledLayout L, uint32_t w_stride, LabeledInputs in, uint32_t batch,
                                                         Fr* __restrict__ W, int* flag) {
@@ -402,19 +449,8 @@ __global__ void __launch_bounds__(96) k_labeled_witness(LabeledLayout L, uint32_
     const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
     if (p >= batch) return;
     Fr* w = W + (uint64_t)p * w_stride;
-    const Fr key = Fr::from_u32(LABELED_KEY);
     if (role == 0) {
-        const Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
-        const Fr se = load_canonical<Fr>(in.secrets + 32ull * p, flag);
-        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
-        w[8] = nu; w[9] = se;
-        const Fr note[2] = {nu, se};
-        const Fr pre = mimc7_multi_hash<true>(note, key, w + L.pre_base, L.perm);
-        w[L.pre_out] = pre;
-        const Fr leaf_in[4] = {pre, token, fr_from_u64(in.amounts[p]), Fr::from_u32(in.labels[p])};
-        const Fr leaf = mimc7_multi_hash<true>(leaf_in, key, w + L.leaf_base, L.perm);
-        w[L.leaf_out] = leaf;
-        w[1] = witness_path(leaf, w + L.pool_base, L.depth, L.lvl_size, L.perm, in.siblings + 32ull * L.depth * p, in.path_bits[p], flag);
+        labeled_note_witness(L, w, in, p, flag);
     } else if (role == 1) {
         const Fr lo = fr_from_u64(in.low[p]), nx = fr_from_u64(in.next[p]);
         w[15] = lo; w[16] = nx;
@@ -423,35 +459,37 @@ __global__ void __launch_bounds__(96) k_labeled_witness(LabeledLayout L, uint32_
         w[4] = witness_path(leaf, w + L.excl_base, L.depth, L.lvl_size, L.perm, in.excl_siblings + 32ull * L.depth * p,
                             in.excl_path_bits[p], flag);
     } else {
-        const Fr one = Fr::one();
-        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
-        const Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
-        const Fr nu = load_canonical<Fr>(in.nullifiers + 32ull * p, flag);
-        const Fr cnu = load_canonical<Fr>(in.change_nullifiers + 32ull * p, flag);
-        const Fr cse = load_canonical<Fr>(in.change_secrets + 32ull * p, flag);
-        const uint64_t amount = in.amounts[p], wd = in.withdrawn[p], lo = in.low[p], nx = in.next[p];
-        const uint32_t label = in.labels[p];
-        const Fr am = fr_from_u64(amount), fwd = fr_from_u64(wd), la = Fr::from_u32(label), change = am - fwd;
-        w[0] = one; w[3] = re; w[5] = token; w[6] = fwd;
-        w[10] = re.sqr();
-        w[11] = am; w[12] = la; w[13] = cnu; w[14] = cse;
-        // nullifier_hash = MultiMiMC7([nullifier], key 1) = 1 + nullifier + hash(nullifier, 1), as in withdraw
-        w[2] = one + nu + mimc7_hash<true>(nu, one, w + 17);
-        const Fr cnote[2] = {cnu, cse};
-        const Fr cpre = mimc7_multi_hash<true>(cnote, key, w + L.cpre_base, L.perm);
-        w[L.cpre_out] = cpre;
-        const Fr ccm_in[4] = {cpre, token, change, la};
-        w[7] = mimc7_multi_hash<true>(ccm_in, key, w + L.ccm_base, L.perm);
-        // the range bits; x = label + 1 <= 2^32
-        const uint64_t x = (uint64_t)label + 1;
-        store_range_bits(w + L.amount_bits, amount, LABELED_AMOUNT_BITS);
-        store_range_bits(w + L.withdrawn_bits, wd, LABELED_AMOUNT_BITS);
-        store_range_bits(w + L.change_bits, diff_bits(amount, wd), LABELED_AMOUNT_BITS);
-        store_range_bits(w + L.label_bits, label, LABELED_LABEL_BITS);
+        // x = label + 1 <= 2^32
+        const uint64_t lo = in.low[p], nx = in.next[p], x = (uint64_t)in.labels[p] + 1;
         store_range_bits(w + L.low_bits, lo);
         store_range_bits(w + L.next_bits, nx);
         store_range_bits(w + L.gap_lo_bits, gap_bits(x, lo));
         store_range_bits(w + L.gap_hi_bits, gap_bits(nx, x));
+        labeled_change_witness(L, w, in, p, flag);
+    }
+}
+
+// Witness of the labeled association withdraw statement, layout of DESIGN.md section 3
+// (== oracle/labeled_association_circuit.py); row p starts at W + p * w_stride, Montgomery form.  The labeled kernel's shape:
+// a CTA covers 32 proofs with three warps, one per independent chain of a proof, writing disjoint variables without a barrier:
+//   warp 0   labeled_note_witness: 70 permutations at depth 32, the critical path
+//   warp 1   assoc_leaf = label + 1, the association path from it, association_root: 64 permutations
+//   warp 2   labeled_change_witness: 7 permutations and the range bits
+__global__ void __launch_bounds__(96) k_labeled_association_witness(LabeledAssociationLayout L, uint32_t w_stride, LabeledAssociationInputs in,
+                                                                    uint32_t batch, Fr* __restrict__ W, int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    if (p >= batch) return;
+    Fr* w = W + (uint64_t)p * w_stride;
+    if (role == 0) {
+        labeled_note_witness(L, w, in, p, flag);
+    } else if (role == 1) {
+        const Fr leaf = fr_from_u64((uint64_t)in.labels[p] + 1);
+        w[15] = leaf;
+        w[4] = witness_path(leaf, w + L.assoc_base, L.depth, L.lvl_size, L.perm, in.assoc_siblings + 32ull * L.depth * p,
+                            in.assoc_path_bits[p], flag);
+    } else {
+        labeled_change_witness(L, w, in, p, flag);
     }
 }
 
@@ -527,8 +565,8 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
     return OG_OK;
 }
 
-// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion and labeled kernels give a proof
-// more than one warp.
+// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion, labeled and labeled association
+// kernels give a proof more than one warp.
 int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
                               Fr* d_W) {
     if (batch == 0) return OG_OK;
@@ -565,6 +603,13 @@ int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t
                               (const uint32_t*)a[8], a[9], a[10], (const uint64_t*)a[11], (const uint64_t*)a[12], a[13],
                               (const uint32_t*)a[14]};
         OG_LAUNCH(ctx, k_labeled_witness, grid, 96, 0, LabeledLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
+        break;
+    }
+    case ST_LABELED_ASSOCIATION: {
+        const LabeledAssociationInputs t{a[0], a[1], (const uint64_t*)a[2], a[3], a[4], (const uint64_t*)a[5], (const uint32_t*)a[6], a[7],
+                                         (const uint32_t*)a[8], a[9], a[10], a[11], (const uint32_t*)a[12]};
+        OG_LAUNCH(ctx, k_labeled_association_witness, grid, 96, 0, LabeledAssociationLayout::make(depth), w_stride, t, batch, d_W,
+                  ctx->d_flag);
         break;
     }
     }

@@ -1,7 +1,8 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit, transfer, association, exclusion and labeled withdraw statements (DESIGN.md section 3; must equal
-// oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout,
-// oracle/association_circuit.py: Layout, oracle/exclusion_circuit.py: Layout and oracle/labeled_circuit.py: Layout).
+// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw statements (DESIGN.md section 3;
+// must equal oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout,
+// oracle/association_circuit.py: Layout, oracle/exclusion_circuit.py: Layout, oracle/labeled_circuit.py: Layout and
+// oracle/labeled_association_circuit.py: Layout).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -222,11 +223,62 @@ struct LabeledInputs {
     const uint32_t* excl_path_bits;
 };
 
+constexpr uint32_t LABELED_ASSOCIATION_N_PUB = 7;
+
+// 0 ONE | 1 root | 2 nullifier_hash | 3 recipient | 4 association_root | 5 token | 6 withdrawn | 7 change_commitment
+// | 8 nullifier | 9 secret | 10 recipient_sq | 11 amount | 12 label | 13 change_nullifier | 14 change_secret | 15 assoc_leaf
+// | 16.. nullifier-hash permutation | precommitment perm1, perm2, out | leaf perm[4], out | depth pool levels
+// | amount, withdrawn, change bits (64 each), label bits (32; all LSB first) | change precommitment perm1, perm2, out
+// | change commitment perm[4] | depth association levels (oracle/labeled_association_circuit.py); a level block is the
+// withdraw statement's.  The fields the labeled statement also has mean what they mean in LabeledLayout.
+struct LabeledAssociationLayout {
+    uint32_t depth, perm, pre_base, pre_out, leaf_base, leaf_out, pool_base, amount_bits, withdrawn_bits, change_bits, label_bits,
+        cpre_base, cpre_out, ccm_base, assoc_base, lvl_size, n_vars, n_constraints;
+    static LabeledAssociationLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        LabeledAssociationLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        const uint32_t P = L.perm;
+        L.lvl_size = 2 * P + 4;
+        L.pre_base = 16 + P;
+        L.pre_out = L.pre_base + 2 * P;
+        L.leaf_base = L.pre_out + 1;
+        L.leaf_out = L.leaf_base + 4 * P;
+        L.pool_base = L.leaf_out + 1;
+        L.amount_bits = L.pool_base + depth * L.lvl_size;
+        L.withdrawn_bits = L.amount_bits + LABELED_AMOUNT_BITS;
+        L.change_bits = L.withdrawn_bits + LABELED_AMOUNT_BITS;
+        L.label_bits = L.change_bits + LABELED_AMOUNT_BITS;
+        L.cpre_base = L.label_bits + LABELED_LABEL_BITS;
+        L.cpre_out = L.cpre_base + 2 * P;
+        L.ccm_base = L.cpre_out + 1;
+        L.assoc_base = L.ccm_base + 4 * P;
+        L.n_vars = L.assoc_base + depth * L.lvl_size;
+        L.n_constraints = 237 + 13 * P + depth * (4 * P + 6);
+        return L;
+    }
+};
+
+// the caller's inputs of a batch of labeled association withdrawals (k_labeled_association_witness's argument), in C ABI
+// order; the first eleven arrays are LabeledInputs', then depth association-tree siblings and a path-bits word per proof
+struct LabeledAssociationInputs {
+    const uint8_t *tokens, *recipients;
+    const uint64_t* withdrawn;
+    const uint8_t *nullifiers, *secrets;
+    const uint64_t* amounts;
+    const uint32_t* labels;
+    const uint8_t* siblings;
+    const uint32_t* path_bits;
+    const uint8_t *change_nullifiers, *change_secrets;
+    const uint8_t* assoc_siblings;
+    const uint32_t* assoc_path_bits;
+};
+
 // ---- the statement table ------------------------------------------------------------------------------------------------
 // What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
 // statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
 // statement_witness_dev) and its og_* forwarders (capi.cu).
-enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED };
+enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED, ST_LABELED_ASSOCIATION };
 constexpr uint32_t STATEMENT_MAX_INPUTS = 15;
 
 struct StatementShape { uint32_t n_vars, n_constraints; };
@@ -259,6 +311,10 @@ constexpr StatementDesc STATEMENTS[] = {
     // change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits
     {LABELED_N_PUB, layout_shape<LabeledLayout>, true, 15, {32, 32, 8, 32, 32, 8, 4, 0, 4, 32, 32, 8, 8, 0, 4},
      {0, 0, 0, 0, 0, 0, 0, 32, 0, 0, 0, 0, 0, 32, 0}},
+    // labeled_association: tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
+    // change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits
+    {LABELED_ASSOCIATION_N_PUB, layout_shape<LabeledAssociationLayout>, true, 13, {32, 32, 8, 32, 32, 8, 4, 0, 4, 32, 32, 0, 4},
+     {0, 0, 0, 0, 0, 0, 0, 32, 0, 0, 0, 32, 0}},
 };
 
 // the input arrays of a batch in the statement's C ABI order (host or device pointers)

@@ -1,10 +1,7 @@
-// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit, transfer, association, exclusion and
-// labeled withdraw statements' R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md section 0/8c); these
-// are the product's own definitions, checked entry for entry against the independently written
-// oracle/withdraw_circuit.py, oracle/deposit_circuit.py, oracle/transfer_circuit.py, oracle/association_circuit.py,
-// oracle/exclusion_circuit.py and oracle/labeled_circuit.py through og_withdraw_r1cs_export, og_deposit_r1cs_export,
-// og_transfer_r1cs_export, og_association_r1cs_export, og_exclusion_r1cs_export and og_labeled_r1cs_export (statement_r1cs
-// below).
+// owshen_b200/csrc/withdraw_circuit.hpp -- host-side builders of the withdraw, deposit, transfer, association, exclusion,
+// labeled and labeled association withdraw statements' R1CS (DESIGN.md section 3).  The reference defines no circuit (SURVEY.md
+// section 0/8c); these are the product's own definitions, checked entry for entry against the independently written
+// oracle/*_circuit.py specs through the og_<statement>_r1cs_export entry points (statement_r1cs below).
 //
 // withdraw
 //   public : root, nullifier_hash, recipient
@@ -39,6 +36,12 @@
 //   label], 2) reaching root along the pool path; amount, withdrawn, change = amount - withdrawn range-checked to 64 bits and
 //   label to 32; change_commitment = the leaf of (change_nullifier, change_secret, token, change, label); the exclusion
 //   statement's bracket on x = label + 1 and its blocklist path to exclusion_root; recipient^2 bound.
+// labeled_association
+//   public : root, nullifier_hash, recipient, association_root, token, withdrawn, change_commitment
+//   private: nullifier, secret, amount, label, siblings[depth], bits[depth], change_nullifier, change_secret,
+//            assoc_siblings[depth], assoc_bits[depth]
+//   the labeled statement's note part (LabeledNoteBuilder); assoc_leaf = label + 1 reaching association_root along the
+//   association path (one depth for both trees); recipient^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -281,47 +284,86 @@ struct ExclusionBuilder {
     }
 };
 
+// The note part of the labeled and labeled association statements, whose layouts share variables 0..14 (variable 4 is the
+// exclusion or association root) and the names of their note blocks; the nullifier-hash permutation sits just below the
+// precommitment block.
+struct LabeledNoteBuilder {
+    static constexpr uint32_t V_ONE = 0, V_ROOT = 1, V_NHASH = 2, V_RECIP = 3, V_TOKEN = 5, V_WITHDRAWN = 6, V_CHANGE_CM = 7,
+                              V_NULL = 8, V_SECRET = 9, V_RSQ = 10, V_AMOUNT = 11, V_LABEL = 12, V_CNULL = 13, V_CSECRET = 14;
+    static LC key() { LC k; k[V_ONE] = Fr::from_u32(LABELED_KEY); return k; }
+    static LC change() { LC am = lc_var(V_AMOUNT), nwd = lc_neg_var(V_WITHDRAWN); return lc_sum({&am, &nwd}); }   // amount - withdrawn
+
+    // recipient; the nullifier hash; the precommitment and the leaf, the pool levels and the pool root row; the amount,
+    // withdrawn, change and label ranges
+    template <class Layout> static void spend(Mimc7Builder& b, const Layout& L) {
+        // the base lists take copies: host GCC rejects the dependent member accesses inside these braced lists
+        const uint32_t P = L.perm, pre_base = L.pre_base, leaf_base = L.leaf_base;
+        const LC k = key();
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        LC nu = lc_var(V_NULL), se = lc_var(V_SECRET), tok = lc_var(V_TOKEN), am = lc_var(V_AMOUNT), la = lc_var(V_LABEL);
+        b.multi_hash({&nu}, lc_var(V_ONE), {pre_base - P}, V_NHASH);
+        b.multi_hash({&nu, &se}, k, {pre_base, pre_base + P}, L.pre_out);
+        LC pre = lc_var(L.pre_out);
+        b.multi_hash({&pre, &tok, &am, &la}, k, {leaf_base, leaf_base + P, leaf_base + 2 * P, leaf_base + 3 * P}, L.leaf_out);
+        const uint32_t pool_root = b.merkle_path(L.leaf_out, L.pool_base, L.lvl_size, L.depth);
+        LC vpool = lc_var(pool_root), nroot = lc_neg_var(V_ROOT);
+        b.cs.add(lc_sum({&vpool, &nroot}), lc_var(V_ONE), LC());
+        b.range(am, L.amount_bits, LABELED_AMOUNT_BITS);
+        b.range(lc_var(V_WITHDRAWN), L.withdrawn_bits, LABELED_AMOUNT_BITS);
+        b.range(change(), L.change_bits, LABELED_AMOUNT_BITS);
+        b.range(la, L.label_bits, LABELED_LABEL_BITS);
+    }
+    // the change precommitment, then the change commitment with its output row bound to change_commitment
+    template <class Layout> static void change_note(Mimc7Builder& b, const Layout& L) {
+        const uint32_t P = L.perm, cpre_base = L.cpre_base, ccm_base = L.ccm_base;
+        const LC k = key(), ch = change();
+        LC cnu = lc_var(V_CNULL), cse = lc_var(V_CSECRET), tok = lc_var(V_TOKEN), la = lc_var(V_LABEL);
+        b.multi_hash({&cnu, &cse}, k, {cpre_base, cpre_base + P}, L.cpre_out);
+        LC cpre = lc_var(L.cpre_out);
+        b.multi_hash({&cpre, &tok, &ch, &la}, k, {ccm_base, ccm_base + P, ccm_base + 2 * P, ccm_base + 3 * P}, V_CHANGE_CM);
+    }
+};
+
 struct LabeledBuilder {
     static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
         Mimc7Builder b(n_rounds);
         LabeledLayout L = LabeledLayout::make(depth, n_rounds);
         b.cs.n_vars = L.n_vars;
         b.cs.n_pub = LABELED_N_PUB;
-        const uint32_t V_ONE = 0, V_ROOT = 1, V_NHASH = 2, V_RECIP = 3, V_XROOT = 4, V_TOKEN = 5, V_WITHDRAWN = 6, V_CHANGE_CM = 7,
-                       V_NULL = 8, V_SECRET = 9, V_RSQ = 10, V_AMOUNT = 11, V_LABEL = 12, V_CNULL = 13, V_CSECRET = 14, V_LOW = 15,
-                       V_NEXT = 16, V_NH_PERM = 17;
-        const uint32_t P = L.perm;
-        LC key; key[V_ONE] = Fr::from_u32(LABELED_KEY);
-        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
-        LC nu = lc_var(V_NULL), se = lc_var(V_SECRET), tok = lc_var(V_TOKEN), am = lc_var(V_AMOUNT), la = lc_var(V_LABEL);
-        b.multi_hash({&nu}, lc_var(V_ONE), {V_NH_PERM}, V_NHASH);
-        b.multi_hash({&nu, &se}, key, {L.pre_base, L.pre_base + P}, L.pre_out);
-        LC pre = lc_var(L.pre_out);
-        b.multi_hash({&pre, &tok, &am, &la}, key, {L.leaf_base, L.leaf_base + P, L.leaf_base + 2 * P, L.leaf_base + 3 * P}, L.leaf_out);
-        const uint32_t pool_root = b.merkle_path(L.leaf_out, L.pool_base, L.lvl_size, depth);
-        LC vpool = lc_var(pool_root), nroot = lc_neg_var(V_ROOT);
-        b.cs.add(lc_sum({&vpool, &nroot}), lc_var(V_ONE), LC());
-        // change = amount - withdrawn; x = label + 1, the deposit's key in the blocklist tree
-        LC nwd = lc_neg_var(V_WITHDRAWN), change = lc_sum({&am, &nwd});
-        LC one = lc_var(V_ONE), x = lc_sum({&la, &one}), nx;
+        const uint32_t V_ONE = 0, V_XROOT = 4, V_LABEL = 12, V_LOW = 15, V_NEXT = 16;
+        LabeledNoteBuilder::spend(b, L);
+        // x = label + 1, the deposit's key in the blocklist tree
+        LC la = lc_var(V_LABEL), one = lc_var(V_ONE), x = lc_sum({&la, &one}), nx;
         for (auto& kv : x) lc_add_term(nx, kv.first, kv.second.neg());
         LC low = lc_var(V_LOW), next = lc_var(V_NEXT), nlow = lc_neg_var(V_LOW), m1 = lc_neg_var(V_ONE);
-        b.range(am, L.amount_bits, LABELED_AMOUNT_BITS);
-        b.range(lc_var(V_WITHDRAWN), L.withdrawn_bits, LABELED_AMOUNT_BITS);
-        b.range(change, L.change_bits, LABELED_AMOUNT_BITS);
-        b.range(la, L.label_bits, LABELED_LABEL_BITS);
         b.range(low, L.low_bits, EXCLUSION_RANGE_BITS);
         b.range(next, L.next_bits, EXCLUSION_RANGE_BITS);
         b.range(lc_sum({&x, &nlow, &m1}), L.gap_lo_bits, EXCLUSION_RANGE_BITS);      // x - low - 1
         b.range(lc_sum({&next, &nx, &m1}), L.gap_hi_bits, EXCLUSION_RANGE_BITS);     // next - x - 1
-        LC cnu = lc_var(V_CNULL), cse = lc_var(V_CSECRET);
-        b.multi_hash({&cnu, &cse}, key, {L.cpre_base, L.cpre_base + P}, L.cpre_out);
-        LC cpre = lc_var(L.cpre_out);
-        b.multi_hash({&cpre, &tok, &change, &la}, key, {L.ccm_base, L.ccm_base + P, L.ccm_base + 2 * P, L.ccm_base + 3 * P}, V_CHANGE_CM);
-        b.hash2(low, next, L.xleaf_base, L.xleaf_base + P, L.xleaf_out);
+        LabeledNoteBuilder::change_note(b, L);
+        b.hash2(low, next, L.xleaf_base, L.xleaf_base + L.perm, L.xleaf_out);
         const uint32_t excl_root = b.merkle_path(L.xleaf_out, L.excl_base, L.lvl_size, depth);
         LC vexcl = lc_var(excl_root), nxroot = lc_neg_var(V_XROOT);
         b.cs.add(lc_sum({&vexcl, &nxroot}), lc_var(V_ONE), LC());
+        return b.cs;
+    }
+};
+
+struct LabeledAssociationBuilder {
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        LabeledAssociationLayout L = LabeledAssociationLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = LABELED_ASSOCIATION_N_PUB;
+        const uint32_t V_ONE = 0, V_AROOT = 4, V_LABEL = 12, V_ALEAF = 15;
+        LabeledNoteBuilder::spend(b, L);
+        LabeledNoteBuilder::change_note(b, L);
+        // assoc_leaf = label + 1, the deposit's leaf in the provider's tree of approved labels
+        LC la = lc_var(V_LABEL), one = lc_var(V_ONE), nleaf = lc_neg_var(V_ALEAF);
+        b.cs.add(lc_sum({&la, &one, &nleaf}), lc_var(V_ONE), LC());
+        const uint32_t assoc_root = b.merkle_path(V_ALEAF, L.assoc_base, L.lvl_size, depth);
+        LC vassoc = lc_var(assoc_root), naroot = lc_neg_var(V_AROOT);
+        b.cs.add(lc_sum({&vassoc, &naroot}), lc_var(V_ONE), LC());
         return b.cs;
     }
 };
@@ -335,6 +377,7 @@ inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     case ST_ASSOCIATION: return AssociationBuilder::build(depth);
     case ST_EXCLUSION: return ExclusionBuilder::build(depth);
     case ST_LABELED: return LabeledBuilder::build(depth);
+    case ST_LABELED_ASSOCIATION: return LabeledAssociationBuilder::build(depth);
     }
     return R1cs();
 }
