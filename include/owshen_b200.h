@@ -156,6 +156,23 @@ int32_t og_note_scan(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, con
                      uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts);
 int32_t og_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments,
                          uint64_t n, uint32_t* d_out_owner, uint8_t* d_out_plaintexts);
+/* Spend-key notes (the owned transfer statement's, below): the same 160-byte record of the four words (owner P, blinding,
+ * token, amount), its commitment MultiMiMC7([P, blinding, token, amount], 4) and status as og_note_encrypt's. */
+int32_t og_owned_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners, const uint8_t* blindings,
+                              const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
+                              uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status);
+int32_t og_owned_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
+                                  const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals,
+                                  uint64_t n, uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status);
+/* og_note_scan for spend-key notes: key k is a view key v_k with the spend public key P_k (32 B, canonical, else
+ * OG_E_ENCODING) of the same wallet, and owns a record only if the record decrypts under v_k to an amount below 2^64, its
+ * first word is P_k, and the key-4 commitment of the four words matches.  A note sent to v_k but to another spend key is
+ * not owned: the wallet could not spend it.  view_keys and spend_public_keys are host memory in both variants. */
+int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys, const uint8_t* records,
+                           const uint8_t* commitments, uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts);
+int32_t og_owned_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                               const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
+                               uint8_t* d_out_plaintexts);
 
 /* ---- MSM (BASELINE configs 3 and 5) ----------------------------------------------------------- */
 int32_t og_msm_g1(og_ctx* ctx, const uint8_t* points, const uint8_t* scalars, uint64_t n, uint8_t* out64);
@@ -310,6 +327,33 @@ int32_t og_labeled_association_witness(og_ctx* ctx, uint32_t depth, const uint8_
                                        const uint8_t* change_nullifiers, const uint8_t* change_secrets, const uint8_t* assoc_siblings,
                                        const uint32_t* assoc_path_bits, uint32_t batch, uint8_t* witnesses);
 
+/* ---- spend-key notes and the owned transfer statement (DESIGN.md section 3): transfers whose outputs only the recipient's
+ * spending key can spend ---- */
+/* A spending key s is a canonical Fr element; its spend public key P = MultiMiMC7([s], 3).  A note is (P, blinding, token,
+ * amount < 2^64) with commitment MultiMiMC7([P, blinding, token, amount], 4); spending it at leaf index i publishes the
+ * nullifier MultiMiMC7([s, commitment, i], 5).  n items each, 32 B field elements in and out; indices uint32. */
+int32_t og_owned_public_keys(og_ctx* ctx, const uint8_t* spend_keys, uint64_t n, uint8_t* out);
+int32_t og_owned_commitments(og_ctx* ctx, const uint8_t* owners, const uint8_t* blindings, const uint8_t* tokens, const uint64_t* amounts,
+                             uint64_t n, uint8_t* out);
+int32_t og_owned_nullifiers(og_ctx* ctx, const uint8_t* spend_keys, const uint8_t* commitments, const uint32_t* indices, uint64_t n,
+                            uint8_t* out);
+/* The transfer statement's public inputs (root, public_amount, token, recipient, nullifier[2], out_commitment[2]), with
+ * spend-key notes: each input proves knowledge of s for its note's owner, and nullifier[i] is its key-5 nullifier.  depth
+ * 1..32; at depth 32: 55 867 variables, 55 793 constraints, domain 2^16. */
+int32_t og_owned_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_owned_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                      uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Inputs as og_transfer_witness's with in_spend_keys and
+ * in_blindings in place of in_nullifiers and in_secrets, out_owners (spend public keys) and out_blindings in place of
+ * out_nullifiers and out_secrets.  root is the caller's: a wrong spend key, an input of nonzero amount that does not reach
+ * root, or two inputs with one nullifier give a witness that does not satisfy the R1CS. */
+int32_t og_owned_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                  const uint8_t* in_spend_keys, const uint8_t* in_blindings, const uint64_t* in_amounts,
+                                  const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                  const uint8_t* out_owners, const uint8_t* out_blindings, const uint64_t* out_amounts,
+                                  uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -433,6 +477,19 @@ int32_t og_groth16_prove_labeled_association_dev(og_ctx* ctx, const og_pk* pk, c
                                                  const uint8_t* d_change_secrets, const uint8_t* d_assoc_siblings,
                                                  const uint32_t* d_assoc_path_bits, uint32_t batch, const uint8_t* d_rs,
                                                  uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of owned transfer proofs, witness generation on the GPU; inputs as in og_owned_transfer_witness.  OG_E_INVALID unless
+ * the key has an owned transfer statement's shape (the depth is recognised from it).  public_out (optional): batch * 8 * 32 B
+ * = root, public_amount, token, recipient, nullifier[2], out_commitment[2]. */
+int32_t og_groth16_prove_owned_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                        const uint8_t* in_spend_keys, const uint8_t* in_blindings, const uint64_t* in_amounts,
+                                        const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                        const uint8_t* out_owners, const uint8_t* out_blindings, const uint64_t* out_amounts,
+                                        uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out);
+int32_t og_groth16_prove_owned_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
+                                            const uint8_t* d_recipients, const uint8_t* d_in_spend_keys, const uint8_t* d_in_blindings,
+                                            const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
+                                            const uint8_t* d_out_owners, const uint8_t* d_out_blindings, const uint64_t* d_out_amounts,
+                                            uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

@@ -1,6 +1,6 @@
 """owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool deposit, withdraw, transfer, association-set
-withdraw, exclusion withdraw, labeled withdraw and labeled association withdraw proofs over BN254, with encrypted delivery
-of the notes they create.
+withdraw, exclusion withdraw, labeled withdraw, labeled association withdraw and owned transfer proofs over BN254, with
+encrypted delivery of the notes they create.
 
 Python is the host language here because the reference's (Rust) toolchain is absent from this image;
 everything below is a thin ctypes veneer over the C ABI in include/owshen_b200.h, which is the real
@@ -16,6 +16,7 @@ from .api import (Context, ProvingKey, MerkleTree, OwshenB200Error, lib, build_l
                   deposit_labeled, setup_labeled, labeled_r1cs_info, labeled_r1cs_export, ptau_prepare_labeled,
                   ApprovedLabels, setup_labeled_association, labeled_association_r1cs_info, labeled_association_r1cs_export,
                   ptau_prepare_labeled_association,
+                  setup_owned_transfer, owned_transfer_r1cs_info, owned_transfer_r1cs_export, ptau_prepare_owned_transfer,
                   ptau_new, ptau_contribute, ptau_verify, ptau_prepare, ptau_prepare_withdraw, ptau_prepare_deposit,
                   ptau_prepare_transfer, phase2_contribute, phase2_verify, NOTE_SUBGROUP_ORDER, NOTE_NOT_OWNED, NOTE_MALFORMED)
 
@@ -29,4 +30,5 @@ __all__ = ["Context", "ProvingKey", "MerkleTree", "OwshenB200Error", "lib", "bui
            "deposit_labeled", "setup_labeled", "labeled_r1cs_info", "labeled_r1cs_export", "ptau_prepare_labeled",
            "ApprovedLabels", "setup_labeled_association", "labeled_association_r1cs_info", "labeled_association_r1cs_export",
            "ptau_prepare_labeled_association",
+           "setup_owned_transfer", "owned_transfer_r1cs_info", "owned_transfer_r1cs_export", "ptau_prepare_owned_transfer",
            "NOTE_SUBGROUP_ORDER", "NOTE_NOT_OWNED", "NOTE_MALFORMED"]

@@ -77,6 +77,12 @@ _SIGS = {
     "og_note_encrypt_dev": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint64] + [C.c_void_p] * 3),
     "og_note_scan": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "og_note_scan_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "og_owned_note_encrypt": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint64] + [C.c_void_p] * 3),
+    "og_owned_note_encrypt_dev": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_uint64] + [C.c_void_p] * 3),
+    "og_owned_note_scan": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                                       C.c_void_p]),
+    "og_owned_note_scan_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                                           C.c_void_p]),
     "og_msm_g1": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "og_msm_g2": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "og_msm_g1_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -114,6 +120,12 @@ _SIGS = {
     "og_labeled_association_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_labeled_association_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_labeled_association_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 13 + [C.c_uint32, C.c_void_p]),
+    "og_owned_public_keys": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
+    "og_owned_commitments": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 4 + [C.c_uint64, C.c_void_p]),
+    "og_owned_nullifiers": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 3 + [C.c_uint64, C.c_void_p]),
+    "og_owned_transfer_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_owned_transfer_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_owned_transfer_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -137,6 +149,9 @@ _SIGS = {
     "og_groth16_prove_labeled_association": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 13 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_labeled_association_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 13
                                                  + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_owned_transfer": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_owned_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11
+                                            + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -275,6 +290,10 @@ _STATEMENTS = {
                                    ("labels", 4, 0, _label_array), ("siblings", 0, 32, None), ("path_bits", 4, 0, _u32_array),
                                    ("change_nullifiers", 32, 0, None), ("change_secrets", 32, 0, None), ("assoc_siblings", 0, 32, None),
                                    ("assoc_path_bits", 4, 0, _u32_array))),
+    "owned_transfer": (True, (("roots", 32, 0, None), ("tokens", 32, 0, None), ("recipients", 32, 0, None), ("in_spend_keys", 64, 0, None),
+                              ("in_blindings", 64, 0, None), ("in_amounts", 16, 0, _u64_array), ("in_siblings", 0, 64, None),
+                              ("in_path_bits", 8, 0, _u32_array), ("out_owners", 64, 0, None), ("out_blindings", 64, 0, None),
+                              ("out_amounts", 16, 0, _u64_array))),
 }
 
 
@@ -537,6 +556,85 @@ class Context:
         _check(lib().og_note_scan_dev(self._h, view_keys, len(view_keys) // 32, _ptr(d_records), _ptr(d_commitments), n,
                                       _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
 
+    # ---- spend-key notes (DESIGN.md section 3, "Owned transfers") ---------------------------------------------------
+    def owned_note_encrypt(self, pk_x: bytes, pk_is_odd: bytes, owners: bytes, blindings: bytes, tokens: bytes, amounts, ephemerals=None):
+        """note_encrypt for spend-key notes (owner P, blinding, token, amount): the same records, with commitments
+        MultiMiMC7([P, blinding, token, amount], 4) -> (records, commitments, status)."""
+        n = len(pk_is_odd)
+        if ephemerals is None:
+            ephemerals = b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n))
+        am = _u64_array(amounts)
+        for name, buf in (("pk_x", pk_x), ("owners", owners), ("blindings", blindings), ("tokens", tokens), ("ephemerals", ephemerals)):
+            _need(len(buf) == 32 * n, f"owned_note_encrypt: {name}: expected {32 * n} bytes, got {len(buf)}")
+        _need((C.sizeof(am) if isinstance(am, C.Array) else _blen(am)) == 8 * n, "owned_note_encrypt: expected one amount per note")
+        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
+        _check(lib().og_owned_note_encrypt(self._h, pk_x, pk_is_odd, owners, blindings, tokens, _ptr(am), ephemerals, n, rec, cm, st), self)
+        return rec.raw, cm.raw, st.raw[:n]
+
+    def owned_note_encrypt_dev(self, d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals, n: int,
+                               d_out_records, d_out_commitments, d_out_status):
+        """og_owned_note_encrypt_dev: device buffers (addresses or tensors), enqueued on the context's stream."""
+        _check(lib().og_owned_note_encrypt_dev(self._h, *[_ptr(x) for x in (d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens,
+                                                                           d_amounts, d_ephemerals)], n,
+                                               *[_ptr(x) for x in (d_out_records, d_out_commitments, d_out_status)]), self)
+
+    def owned_note_scan(self, view_keys: bytes, spend_public_keys: bytes, records: bytes, commitments: bytes):
+        """note_scan for spend-key notes: key k is (view_keys[k], spend_public_keys[k]) and owns a record only if the record
+        decrypts under the view key to a note whose owner is the spend public key and whose key-4 commitment matches ->
+        (owners, plaintexts) as note_scan's, the plaintext words being (owner, blinding, token, amount)."""
+        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
+              "owned_note_scan: view keys and spend public keys must be equally long multiples of 32 bytes")
+        _need(len(records) % 160 == 0, "owned_note_scan: records must be a multiple of 160 bytes")
+        n = len(records) // 160
+        _need(len(commitments) == 32 * n, "owned_note_scan: expected one 32-byte commitment per record")
+        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
+        _check(lib().og_owned_note_scan(self._h, view_keys, spend_public_keys, len(view_keys) // 32, records, commitments, n, owner, plain),
+               self)
+        return list(owner), plain.raw
+
+    def owned_note_scan_dev(self, view_keys: bytes, spend_public_keys: bytes, d_records, d_commitments, n: int, d_out_owner,
+                            d_out_plaintexts):
+        """og_owned_note_scan_dev: the keys on the host, every other buffer on the device, enqueued on the context's stream."""
+        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
+              "owned_note_scan_dev: view keys and spend public keys must be equally long multiples of 32 bytes")
+        _check(lib().og_owned_note_scan_dev(self._h, view_keys, spend_public_keys, len(view_keys) // 32, _ptr(d_records),
+                                            _ptr(d_commitments), n, _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
+
+    def owned_public_keys(self, spend_keys: bytes) -> bytes:
+        """MultiMiMC7([s], 3) of each spending key (32 bytes each in and out): the owner a sender puts in a note."""
+        _need(len(spend_keys) % 32 == 0, "owned_public_keys: spend keys must be a multiple of 32 bytes")
+        n = len(spend_keys) // 32
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_owned_public_keys(self._h, spend_keys, n, out), self)
+        return out.raw
+
+    def owned_commitments(self, owners: bytes, blindings: bytes, tokens: bytes, amounts) -> bytes:
+        """MultiMiMC7([owner, blinding, token, amount], 4) of each note: owners, blindings, tokens 32 bytes each, amounts
+        uint64 (a little-endian buffer, an array or a sequence of ints)."""
+        _need(len(owners) % 32 == 0 and len(blindings) == len(owners) and len(tokens) == len(owners),
+              "owned_commitments: owners, blindings and tokens must be equally long multiples of 32 bytes")
+        n = len(owners) // 32
+        am = _u64_array(amounts)
+        _need((C.sizeof(am) if isinstance(am, C.Array) else _blen(am)) == 8 * n, "owned_commitments: expected one amount per note")
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_owned_commitments(self._h, owners, blindings, tokens, _ptr(am), n, out), self)
+        return out.raw
+
+    def owned_nullifiers(self, spend_keys: bytes, commitments: bytes, indices) -> bytes:
+        """MultiMiMC7([s, commitment, index], 5) of each note at its leaf index (uint32): the nullifier its spend publishes,
+        so a wallet sees which of its notes the chain has spent."""
+        _need(len(spend_keys) % 32 == 0 and len(commitments) == len(spend_keys),
+              "owned_nullifiers: spend keys and commitments must be equally long multiples of 32 bytes")
+        n = len(spend_keys) // 32
+        if _blen(indices) is None:
+            indices = [int(x) for x in indices]
+            _need(all(0 <= x < 1 << 32 for x in indices), "owned_nullifiers: leaf indices must be integers in [0, 2^32)")
+        idx = _label_array(indices)
+        _need((C.sizeof(idx) if isinstance(idx, C.Array) else _blen(idx)) == 4 * n, "owned_nullifiers: expected one index per note")
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_owned_nullifiers(self._h, spend_keys, commitments, _ptr(idx), n, out), self)
+        return out.raw
+
     def msm_g1(self, points: bytes, scalars: bytes) -> bytes:
         _need(len(scalars) % 32 == 0, "msm_g1: scalars must be a multiple of 32 bytes")
         n = len(scalars) // 32
@@ -673,6 +771,14 @@ class Context:
                                                                       siblings, path_bits, change_nullifiers, change_secrets,
                                                                       assoc_siblings, assoc_path_bits))
 
+    def owned_transfer_witness(self, depth, roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings,
+                               in_path_bits, out_owners, out_blindings, out_amounts) -> bytes:
+        """Full assignments of the depth-`depth` owned transfer statement, n_vars * 32 bytes per transfer, computed on the GPU.
+        Inputs as in transfer_witness, with the inputs' spending keys and blindings in place of their nullifiers and secrets
+        and the outputs' owners (spend public keys) and blindings in place of theirs."""
+        return self._statement_witness("owned_transfer", depth, (roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts,
+                                                                 in_siblings, in_path_bits, out_owners, out_blindings, out_amounts))
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -763,6 +869,15 @@ def labeled_association_r1cs_export(depth: int, which: str):
     return _statement_r1cs_export("labeled_association", depth, which)
 
 
+def owned_transfer_r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("owned_transfer", depth)
+
+
+def owned_transfer_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` owned transfer R1CS."""
+    return _statement_r1cs_export("owned_transfer", depth, which)
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -834,6 +949,12 @@ def setup_labeled_association(ctx: Context, depth: int, tau: int, alpha: int, be
     """Development setup of the depth-`depth` labeled association withdraw statement -> (pk_bytes, vk_bytes): its exported
     R1CS through setup_r1cs.  The key records depth 0; the prover recognises it as a labeled association key by its shape."""
     return _setup_statement(ctx, "labeled_association", depth, (tau, alpha, beta, gamma, delta))
+
+
+def setup_owned_transfer(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` owned transfer statement -> (pk_bytes, vk_bytes): its exported R1CS through
+    setup_r1cs.  The key records depth 0; the prover recognises it as an owned transfer key by its shape."""
+    return _setup_statement(ctx, "owned_transfer", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -926,6 +1047,10 @@ def ptau_prepare_labeled(ctx: Context, acc: bytes, depth: int):
 
 def ptau_prepare_labeled_association(ctx: Context, acc: bytes, depth: int):
     return _ptau_prepare_statement(ctx, acc, "labeled_association", depth)
+
+
+def ptau_prepare_owned_transfer(ctx: Context, acc: bytes, depth: int):
+    return _ptau_prepare_statement(ctx, acc, "owned_transfer", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -1093,6 +1218,20 @@ class ProvingKey:
         return self._prove_statement("labeled_association", self.labeled_association_depth,
                                      (tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
                                       change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits), rs, want_public)
+
+    @property
+    def owned_transfer_depth(self):
+        """The depth d whose owned transfer statement has this key's shape (owned_transfer_r1cs_info), or None."""
+        return self._shape_depth("owned_transfer")
+
+    def prove_owned_transfer(self, roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings, in_path_bits,
+                             out_owners, out_blindings, out_amounts, rs, want_public=True):
+        """Batch of owned transfer proofs from the notes (witness generation on the GPU).  Inputs as in
+        Context.owned_transfer_witness; returns (proofs, public_inputs) with public inputs (root, public_amount, token,
+        recipient, nullifier[2], out_commitment[2]) per proof."""
+        return self._prove_statement("owned_transfer", self.owned_transfer_depth,
+                                     (roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings, in_path_bits,
+                                      out_owners, out_blindings, out_amounts), rs, want_public)
 
     def prover_plan(self, batch: int) -> dict:
         """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and

@@ -720,6 +720,84 @@ int32_t og_note_scan(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, con
     return OG_OK;
 }
 
+// ---- spend-key notes: encryption and scanning (note_impl.cuh with commitment key 4 and the owner check) ---------------
+int32_t og_owned_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
+                                  const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals,
+                                  uint64_t n, uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
+    OG_ENTER(ctx);
+    if (n && (!d_pk_x || !d_pk_is_odd || !d_owners || !d_blindings || !d_tokens || !d_amounts || !d_ephemerals || !d_out_records ||
+              !d_out_commitments || !d_out_status)) return OG_E_INVALID;
+    return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals}, n,
+                            d_out_records, d_out_commitments, d_out_status, true);
+}
+
+int32_t og_owned_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners, const uint8_t* blindings,
+                              const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
+                              uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
+    OG_ENTER(ctx);
+    if (n && (!pk_x || !pk_is_odd || !owners || !blindings || !tokens || !amounts || !ephemerals || !out_records || !out_commitments ||
+              !out_status)) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    // og_note_encrypt's staging
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 362ull * n);
+    uint64_t* da = reinterpret_cast<uint64_t*>(io);
+    uint8_t *dx = io + 8 * n, *dow = dx + 32 * n, *dbl = dow + 32 * n, *dto = dbl + 32 * n, *de = dto + 32 * n;
+    uint8_t *drec = de + 32 * n, *dcm = drec + 160 * n, *dodd = dcm + 32 * n, *dst = dodd + n;
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
+    H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n);
+    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dow, dbl, dto, da, de}, n, drec, dcm, dst, true));
+    D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
+    return check_flag(ctx);
+}
+
+// the view keys as og_note_scan stages them, and one spend public key per view key, canonical (OG_E_ENCODING), staged beside
+static int32_t owned_note_stage_keys(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                                     const uint32_t** d_keys, const uint32_t** d_spend) {
+    OG_TRY(note_stage_keys(ctx, view_keys, n_keys, d_keys));
+    for (uint32_t j = 0; j < n_keys; j++) {
+        uint32_t v[8];
+        memcpy(v, spend_public_keys + 32ull * j, 32);
+        if (!Fr::canonical_lt_mod(v)) {
+            snprintf(ctx->err, sizeof(ctx->err), "spend public key %u is not a canonical field element", j);
+            return OG_E_ENCODING;
+        }
+    }
+    OG_SLOT(ctx, ds, uint32_t, S_NOTE_SPEND_KEYS, 32ull * (n_keys ? n_keys : 1));
+    if (n_keys) H2D(ctx, ds, spend_public_keys, 32ull * n_keys);
+    *d_spend = ds;
+    return OG_OK;
+}
+
+int32_t og_owned_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                               const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
+                               uint8_t* d_out_plaintexts) {
+    OG_ENTER(ctx);
+    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!d_records || !d_commitments || !d_out_owner || !d_out_plaintexts)))
+        return OG_E_INVALID;
+    const uint32_t *dk, *ds;
+    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
+    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, ds);
+}
+
+int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys, const uint8_t* records,
+                           const uint8_t* commitments, uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts) {
+    OG_ENTER(ctx);
+    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!records || !commitments || !out_owner || !out_plaintexts)))
+        return OG_E_INVALID;
+    const uint32_t *dk, *ds;
+    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // og_note_scan's staging
+    uint32_t* downer = reinterpret_cast<uint32_t*>(io);
+    uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
+    H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
+    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, ds));
+    D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
+    OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return OG_OK;
+}
+
 // ---- MSM --------------------------------------------------------------------------------------------------
 }  // extern "C"
 
@@ -1054,6 +1132,65 @@ int32_t og_labeled_association_witness(og_ctx* ctx, uint32_t depth, const uint8_
                                                                   assoc_path_bits}, batch, witnesses);
 }
 
+// ---- spend-key notes and the owned transfer statement ---------------------------------------------------------------
+int32_t og_owned_public_keys(og_ctx* ctx, const uint8_t* spend_keys, uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !spend_keys || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dk, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_B, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dk, spend_keys, 32 * n);
+    OG_TRY(owned_public_keys_dev(ctx, dk, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_owned_commitments(og_ctx* ctx, const uint8_t* owners, const uint8_t* blindings, const uint8_t* tokens, const uint64_t* amounts,
+                             uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !owners || !blindings || !tokens || !amounts || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dow, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, dbl, uint8_t, S_IO_B, 32 * n);
+    OG_SLOT(ctx, dt, uint8_t, S_IO_C, 32 * n);
+    OG_SLOT(ctx, da, uint64_t, S_IO_D, 8 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_E, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n); H2D(ctx, dt, tokens, 32 * n); H2D(ctx, da, amounts, 8 * n);
+    OG_TRY(owned_commitments_dev(ctx, dow, dbl, dt, da, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_owned_nullifiers(og_ctx* ctx, const uint8_t* spend_keys, const uint8_t* commitments, const uint32_t* indices, uint64_t n,
+                            uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !spend_keys || !commitments || !indices || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dk, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, dc, uint8_t, S_IO_B, 32 * n);
+    OG_SLOT(ctx, di, uint32_t, S_IO_C, 4 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_D, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dk, spend_keys, 32 * n); H2D(ctx, dc, commitments, 32 * n); H2D(ctx, di, indices, 4 * n);
+    OG_TRY(owned_nullifiers_dev(ctx, dk, dc, di, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_owned_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_OWNED_TRANSFER, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_owned_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    return statement_r1cs_export(ST_OWNED_TRANSFER, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
+int32_t og_owned_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                  const uint8_t* in_spend_keys, const uint8_t* in_blindings, const uint64_t* in_amounts,
+                                  const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                  const uint8_t* out_owners, const uint8_t* out_blindings, const uint64_t* out_amounts,
+                                  uint32_t batch, uint8_t* witnesses) {
+    return statement_witness(ctx, ST_OWNED_TRANSFER, depth, {roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings,
+                                                             in_path_bits, out_owners, out_blindings, out_amounts}, batch, witnesses);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1230,6 +1367,25 @@ int32_t og_groth16_prove_labeled_association(og_ctx* ctx, const og_pk* pk, const
     return statement_prove(ctx, pk, ST_LABELED_ASSOCIATION, {tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings,
                                                              path_bits, change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits},
                            batch, rs, proofs, public_out);
+}
+
+int32_t og_groth16_prove_owned_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
+                                            const uint8_t* d_recipients, const uint8_t* d_in_spend_keys, const uint8_t* d_in_blindings,
+                                            const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
+                                            const uint8_t* d_out_owners, const uint8_t* d_out_blindings, const uint64_t* d_out_amounts,
+                                            uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    return statement_prove_dev(ctx, pk, ST_OWNED_TRANSFER, {d_roots, d_tokens, d_recipients, d_in_spend_keys, d_in_blindings, d_in_amounts,
+                                                            d_in_siblings, d_in_path_bits, d_out_owners, d_out_blindings, d_out_amounts},
+                               batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_owned_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                        const uint8_t* in_spend_keys, const uint8_t* in_blindings, const uint64_t* in_amounts,
+                                        const uint8_t* in_siblings, const uint32_t* in_path_bits,
+                                        const uint8_t* out_owners, const uint8_t* out_blindings, const uint64_t* out_amounts,
+                                        uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
+    return statement_prove(ctx, pk, ST_OWNED_TRANSFER, {roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings,
+                                                        in_path_bits, out_owners, out_blindings, out_amounts}, batch, rs, proofs, public_out);
 }
 
 int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {

@@ -104,6 +104,7 @@ enum Slot {
     S_PR_SORT_STAGE, S_L1_SORT_STAGE, S_PR_SORT_TILES, S_L1_SORT_TILES,   // only for keys whose sort scratch outgrows the buckets / heavy scratch
     S_IO_STATEMENT,                                                         // the staged input arrays of a statement's batch
     S_IO_NOTE, S_NOTE_KEYS, S_NOTE_PREP,                                    // note encryption / scanning (note_impl.cuh)
+    S_NOTE_SPEND_KEYS,                                                      // the spend public keys of an owned-note scan
     S_COUNT
 };
 static_assert(S_COUNT <= N_SLOTS, "grow N_SLOTS");

@@ -1,7 +1,7 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
-// paths (BASELINE config 2), level-by-level tree build, the labeled-note hashes, and the witness generators of the withdraw,
-// deposit, transfer, association, exclusion, labeled and labeled association withdraw statements (every t^2, t^4, t^6, t^7 of
-// every round is a circuit variable).
+// paths (BASELINE config 2), level-by-level tree build, the labeled-note and spend-key-note hashes, and the witness generators
+// of the withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw and owned transfer
+// statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //
 // Not in the reference (its only field "hash" is a placeholder product,
 // /root/reference/src/blockchain/tx/owshen_airdrop/babyjubjub/mod.rs:202-204); the algorithm is the
@@ -493,6 +493,109 @@ __global__ void __launch_bounds__(96) k_labeled_association_witness(LabeledAssoc
     }
 }
 
+// Spend-key notes (oracle/owned_circuit.py), one thread per item: the spend public key MultiMiMC7([s], 3) and the commitment
+// MultiMiMC7([P, blinding, token, amount], 4) for wallets and nodes, the nullifier MultiMiMC7([s, cm, index], 5) for the wallet
+// that watches its notes being spent
+__global__ void __launch_bounds__(64) k_owned_public_keys(const uint8_t* __restrict__ keys, uint64_t n, uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[1] = {load_canonical<Fr>(keys + 32 * i, flag)};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_OWNER_KEY), nullptr, 0));
+}
+
+__global__ void __launch_bounds__(64) k_owned_commitments(const uint8_t* __restrict__ owners, const uint8_t* __restrict__ blindings,
+                                                          const uint8_t* __restrict__ tokens, const uint64_t* __restrict__ amounts, uint64_t n,
+                                                          uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[4] = {load_canonical<Fr>(owners + 32 * i, flag), load_canonical<Fr>(blindings + 32 * i, flag),
+                      load_canonical<Fr>(tokens + 32 * i, flag), fr_from_u64(amounts[i])};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_COMMITMENT_KEY), nullptr, 0));
+}
+
+__global__ void __launch_bounds__(64) k_owned_nullifiers(const uint8_t* __restrict__ keys, const uint8_t* __restrict__ commitments,
+                                                         const uint32_t* __restrict__ indices, uint64_t n, uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[3] = {load_canonical<Fr>(keys + 32 * i, flag), load_canonical<Fr>(commitments + 32 * i, flag), Fr::from_u32(indices[i])};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_NULLIFIER_KEY), nullptr, 0));
+}
+
+// An owned note block's first variable (an input's spend key, an output's owner), blinding, amount (< 2^64), its 64 bits and
+// the commitment MultiMiMC7([owner, blinding, token, amount], 4) with every round value, written into the block v.  Returns
+// the commitment.
+__device__ __forceinline__ Fr owned_note(const OwnedTransferLayout& L, Fr* v, const Fr& first, const Fr& owner, const Fr& bl,
+                                         const Fr& token, uint64_t amount, uint32_t cm, uint32_t cm_out) {
+    const Fr one = Fr::one(), zero = Fr::zero();
+    const Fr am = fr_from_u64(amount);
+    v[0] = first; v[1] = bl; v[2] = am;
+#pragma unroll 8
+    for (uint32_t k = 0; k < TRANSFER_AMOUNT_BITS; k++) v[3 + k] = ((amount >> k) & 1) ? one : zero;
+    const Fr xs[4] = {owner, bl, token, am};
+    const Fr r = mimc7_multi_hash<true>(xs, Fr::from_u32(OWNED_COMMITMENT_KEY), v + cm, L.perm);
+    v[cm_out] = r;
+    return r;
+}
+
+// Witness of the owned transfer statement, layout of DESIGN.md section 3 (== oracle/owned_circuit.py); row p starts at
+// W + p * w_stride, Montgomery form.  The transfer kernel's shape: a CTA covers 32 proofs with four warps, one per
+// independent hash chain of a proof, so no warp diverges and a proof's critical path is one input's owner, commitment and
+// Merkle path (5 + 2 * depth permutations):
+//   warps 0, 1   input i: the owner with its round values, amount bits, commitment, the depth levels
+//   warps 2, 3   input j - 2's owner and commitment again in registers (no stores), its nullifier with its round values,
+//                then output j - 2: amount bits, commitment (12 permutations)
+// After the barrier, warp 0 writes the proof's remaining scalars (public amount, recipient, nf_diff_inv).  Only the low
+// `depth` bits of a path word count, in the levels and in the nullifier's index alike.
+__global__ void __launch_bounds__(128) k_owned_transfer_witness(OwnedTransferLayout L, uint32_t w_stride, OwnedTransferInputs in,
+                                                                uint32_t batch, Fr* __restrict__ W, int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    const bool active = p < batch;
+    Fr* w = W + (uint64_t)p * w_stride;
+    const Fr one = Fr::one();
+    if (active) {
+        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+        const Fr k3 = Fr::from_u32(OWNED_OWNER_KEY);
+        const uint32_t i = role & 1;
+        Fr* v = w + L.inp(i);
+        const Fr s = load_canonical<Fr>(in.in_keys + 64ull * p + 32 * i, flag);
+        const Fr bl = load_canonical<Fr>(in.in_blindings + 64ull * p + 32 * i, flag);
+        const uint64_t amount = in.in_amounts[2ull * p + i];
+        const uint32_t bits = in.in_bits[2ull * p + i];
+        if (role < 2) {
+            const Fr s1[1] = {s};
+            const Fr owner = mimc7_multi_hash<true>(s1, k3, v + L.owner_perm, L.perm);
+            const Fr cm = owned_note(L, v, s, owner, bl, token, amount, L.in_cm, L.in_cm_out);
+            witness_path(cm, v + L.lvl_base, L.depth, L.lvl_size, L.perm, in.in_sib + 32ull * L.depth * (2ull * p + i), bits, flag);
+        } else {
+            const Fr s1[1] = {s};
+            const Fr owner = mimc7_multi_hash<false>(s1, k3, nullptr, 0);
+            const Fr note[4] = {owner, bl, token, fr_from_u64(amount)};
+            const Fr cm = mimc7_multi_hash<false>(note, Fr::from_u32(OWNED_COMMITMENT_KEY), nullptr, 0);
+            const uint32_t mask = L.depth >= 32 ? 0xffffffffu : (1u << L.depth) - 1;
+            const Fr nf_in[3] = {s, cm, Fr::from_u32(bits & mask)};
+            w[5 + i] = mimc7_multi_hash<true>(nf_in, Fr::from_u32(OWNED_NULLIFIER_KEY), v + L.nf_perm, L.perm);
+            Fr* o = w + L.out(i);
+            const Fr oo = load_canonical<Fr>(in.out_owners + 64ull * p + 32 * i, flag);
+            const Fr ob = load_canonical<Fr>(in.out_blindings + 64ull * p + 32 * i, flag);
+            w[7 + i] = owned_note(L, o, oo, oo, ob, token, in.out_amounts[2ull * p + i], L.out_cm, L.out_cm_out);
+        }
+        if (role == 0) {
+            Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+            w[0] = one;
+            w[1] = load_canonical<Fr>(in.roots + 32ull * p, flag);
+            w[3] = token; w[4] = re;
+            w[9] = re.sqr();
+        }
+    }
+    __syncthreads();   // warps 1..3 wrote the amounts and nullifiers read below
+    if (active && role == 0) {
+        Fr a_in = w[L.inp(0) + 2] + w[L.inp(1) + 2], a_out = w[L.out(0) + 2] + w[L.out(1) + 2];
+        w[2] = a_out - a_in;
+        w[10] = (w[5] - w[6]).inv();   // inv(0) = 0: two inputs with one nullifier leave the row unsatisfiable
+    }
+}
+
 // ---- host side ------------------------------------------------------------------------------------
 void mimc_constants_host(Fr* out91) { mimc7_round_constants(out91); }
 
@@ -540,6 +643,26 @@ int32_t labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_t
     return OG_OK;
 }
 
+int32_t owned_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_owned_public_keys, (unsigned)((n + 63) / 64), 64, 0, d_keys, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t owned_commitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, const uint8_t* d_tokens,
+                              const uint64_t* d_amounts, uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_owned_commitments, (unsigned)((n + 63) / 64), 64, 0, d_owners, d_blindings, d_tokens, d_amounts, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t owned_nullifiers_dev(og_ctx* ctx, const uint8_t* d_keys, const uint8_t* d_commitments, const uint32_t* d_indices, uint64_t n,
+                             uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_owned_nullifiers, (unsigned)((n + 63) / 64), 64, 0, d_keys, d_commitments, d_indices, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
 // levels: Montgomery-form buffer holding n + n/2 + ... + 1 elements, level 0 already filled
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves) {
     Fr* in = d_levels;
@@ -565,8 +688,8 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
     return OG_OK;
 }
 
-// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion, labeled and labeled association
-// kernels give a proof more than one warp.
+// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion, labeled, labeled association and
+// owned transfer kernels give a proof more than one warp.
 int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
                               Fr* d_W) {
     if (batch == 0) return OG_OK;
@@ -610,6 +733,12 @@ int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t
                                          (const uint32_t*)a[8], a[9], a[10], a[11], (const uint32_t*)a[12]};
         OG_LAUNCH(ctx, k_labeled_association_witness, grid, 96, 0, LabeledAssociationLayout::make(depth), w_stride, t, batch, d_W,
                   ctx->d_flag);
+        break;
+    }
+    case ST_OWNED_TRANSFER: {
+        const OwnedTransferInputs t{a[0], a[1], a[2], a[3], a[4], (const uint64_t*)a[5], a[6], (const uint32_t*)a[7], a[8], a[9],
+                                    (const uint64_t*)a[10]};
+        OG_LAUNCH(ctx, k_owned_transfer_witness, grid, 128, 0, OwnedTransferLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
         break;
     }
     }

@@ -1,8 +1,8 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw statements (DESIGN.md section 3;
-// must equal oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout,
-// oracle/association_circuit.py: Layout, oracle/exclusion_circuit.py: Layout, oracle/labeled_circuit.py: Layout and
-// oracle/labeled_association_circuit.py: Layout).
+// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw and owned transfer statements
+// (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout,
+// oracle/transfer_circuit.py: Layout, oracle/association_circuit.py: Layout, oracle/exclusion_circuit.py: Layout,
+// oracle/labeled_circuit.py: Layout, oracle/labeled_association_circuit.py: Layout and oracle/owned_circuit.py: Layout).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -274,11 +274,61 @@ struct LabeledAssociationInputs {
     const uint32_t* assoc_path_bits;
 };
 
+constexpr uint32_t OWNED_TRANSFER_N_PUB = 8;
+// MultiMiMC7 keys of spend-key notes: spend public key P = MultiMiMC7([s], 3), commitment MultiMiMC7([P, blinding, token,
+// amount], 4), nullifier MultiMiMC7([s, cm, index], 5)
+constexpr uint32_t OWNED_OWNER_KEY = 3, OWNED_COMMITMENT_KEY = 4, OWNED_NULLIFIER_KEY = 5;
+
+// 0 ONE | 1 root | 2 public_amount | 3 token | 4 recipient | 5, 6 nf[2] | 7, 8 out_cm[2] | 9 recipient_sq | 10 nf_diff_inv
+// | input blocks 0, 1 | output blocks 0, 1 (oracle/owned_circuit.py).  An input block starts with spend_key, blinding,
+// amount and the 64 amount bits, then the owner permutation, the commitment, the depth levels and the nullifier's three
+// permutations; an output block is the transfer's with owner in place of nullifier and blinding in place of secret.
+// Offsets below are relative to the block.
+struct OwnedTransferLayout {
+    uint32_t depth, perm;
+    uint32_t in_base, in_size, out_base, out_size;
+    uint32_t owner_perm, in_cm, in_cm_out, lvl_base, lvl_size, nf_perm;   // input block
+    uint32_t out_cm, out_cm_out;                                          // output block
+    uint32_t n_vars, n_constraints;
+    static OwnedTransferLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        OwnedTransferLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        const uint32_t P = L.perm;
+        L.lvl_size = 2 * P + 4;
+        L.owner_perm = 67; L.in_cm = 67 + P; L.in_cm_out = 67 + 5 * P; L.lvl_base = 68 + 5 * P;
+        L.nf_perm = L.lvl_base + depth * L.lvl_size;
+        L.out_cm = 67; L.out_cm_out = 67 + 4 * P;
+        L.in_base = 11;
+        L.in_size = 68 + 8 * P + depth * L.lvl_size;
+        L.out_size = 68 + 4 * P;
+        L.out_base = L.in_base + 2 * L.in_size;
+        L.n_vars = L.out_base + 2 * L.out_size;
+        L.n_constraints = 273 + 24 * P + depth * (4 * P + 6);
+        return L;
+    }
+    OG_HD uint32_t inp(uint32_t i) const { return in_base + i * in_size; }
+    OG_HD uint32_t out(uint32_t j) const { return out_base + j * out_size; }
+};
+
+// the caller's inputs of a batch of owned transfers (k_owned_transfer_witness's argument), TransferInputs' shapes: per proof,
+// input (output) 0 then 1 in the in_* (out_*) arrays, in_siblings holds 2 * depth elements and in_path_bits 2 words
+struct OwnedTransferInputs {
+    const uint8_t *roots, *tokens, *recipients;
+    const uint8_t *in_keys, *in_blindings;
+    const uint64_t* in_amounts;
+    const uint8_t* in_sib;
+    const uint32_t* in_bits;
+    const uint8_t *out_owners, *out_blindings;
+    const uint64_t* out_amounts;
+};
+
 // ---- the statement table ------------------------------------------------------------------------------------------------
 // What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
 // statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
 // statement_witness_dev) and its og_* forwarders (capi.cu).
-enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED, ST_LABELED_ASSOCIATION };
+enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED, ST_LABELED_ASSOCIATION,
+                            ST_OWNED_TRANSFER };
 constexpr uint32_t STATEMENT_MAX_INPUTS = 15;
 
 struct StatementShape { uint32_t n_vars, n_constraints; };
@@ -315,6 +365,10 @@ constexpr StatementDesc STATEMENTS[] = {
     // change_nullifiers, change_secrets, assoc_siblings, assoc_path_bits
     {LABELED_ASSOCIATION_N_PUB, layout_shape<LabeledAssociationLayout>, true, 13, {32, 32, 8, 32, 32, 8, 4, 0, 4, 32, 32, 0, 4},
      {0, 0, 0, 0, 0, 0, 0, 32, 0, 0, 0, 32, 0}},
+    // owned_transfer: roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings, in_path_bits, out_owners,
+    // out_blindings, out_amounts
+    {OWNED_TRANSFER_N_PUB, layout_shape<OwnedTransferLayout>, true, 11, {32, 32, 32, 64, 64, 16, 0, 8, 64, 64, 16},
+     {0, 0, 0, 0, 0, 0, 64, 0, 0, 0, 0}},
 };
 
 // the input arrays of a batch in the statement's C ABI order (host or device pointers)
@@ -340,6 +394,13 @@ int32_t mimc_merkle_paths_dev(og_ctx* ctx, const uint8_t* d_leaves, const uint8_
 int32_t labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_nullifiers, const uint8_t* d_secrets, uint64_t n, uint8_t* d_out);
 int32_t labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint32_t* d_labels,
                            uint64_t n, uint8_t* d_out);
+// spend-key notes (oracle/owned_circuit.py): P = MultiMiMC7([s], 3), cm = MultiMiMC7([P, blinding, token, amount], 4) and
+// nullifier = MultiMiMC7([s, cm, index], 5)
+int32_t owned_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint64_t n, uint8_t* d_out);
+int32_t owned_commitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, const uint8_t* d_tokens,
+                              const uint64_t* d_amounts, uint64_t n, uint8_t* d_out);
+int32_t owned_nullifiers_dev(og_ctx* ctx, const uint8_t* d_keys, const uint8_t* d_commitments, const uint32_t* d_indices, uint64_t n,
+                             uint8_t* d_out);
 int32_t mimc_to_mont_dev(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Fr* d_out);
 int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_out);
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves);
@@ -366,8 +427,12 @@ struct NoteEncryptInputs {
 };
 int32_t note_check_view_keys(og_ctx* ctx, const uint8_t* h_keys, uint32_t n);
 int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uint8_t* d_pk_x, uint8_t* d_pk_odd);
-int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status);
+// owned = false: transfer notes, commitment key 0.  owned = true: spend-key notes (the nullifier and secret fields carry the
+// owner P and the blinding), commitment key 4, and a scan's d_spend_keys holds one spend public key P_k per view key (canonical
+// limbs): a record is owned by key k only if its m0 is P_k as well.
+int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status,
+                         bool owned = false);
 int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
-                      uint32_t* d_owner, uint8_t* d_plaintexts);
+                      uint32_t* d_owner, uint8_t* d_plaintexts, const uint32_t* d_spend_keys = nullptr);
 
 }  // namespace og

@@ -34,19 +34,21 @@ OG_HD void note_pads(Fr pad[4], const Fr& sx, const Fr& sy, CFn c) {
     for (uint32_t i = 0; i < 4; i++) pad[i] = mimc7_perm_lazy<false>(Fr::from_u32(i), k, c);
 }
 
-// the transfer statement's note commitment MultiMiMC7([nullifier, secret, token, amount], 0)
-template <class CFn>
+// a note's commitment MultiMiMC7(m, KEY): key 0 is the transfer statement's (nullifier, secret, token, amount), key 4 the owned
+// transfer statement's (owner, blinding, token, amount)
+template <uint32_t KEY = 0, class CFn>
 OG_HD Fr note_commitment(const Fr m[4], CFn c) {
-    Fr r = m[0] + mimc7_perm_lazy<true>(m[0], Fr::zero(), c);
+    const Fr k = Fr::from_u32(KEY);
+    Fr r = KEY == 0 ? m[0] + mimc7_perm_lazy<true>(m[0], k, c) : k + m[0] + mimc7_perm_lazy<false>(m[0], k, c);
     for (int i = 1; i < 4; i++) r = r + m[i] + mimc7_perm_lazy<false>(m[i], r, c);
     return r;
 }
 
 OG_HD void note_store_word(uint32_t* w, const Fr& v) { v.to_canonical(w); }
 
-// one note to the compressed key (pk_x, pk_odd) under ephemeral e; writes the record and the commitment when the status is
-// NOTE_ENC_OK and zeros otherwise
-template <class CFn>
+// one note to the compressed key (pk_x, pk_odd) under ephemeral e; writes the record and the commitment under KEY when the
+// status is NOTE_ENC_OK and zeros otherwise
+template <uint32_t KEY = 0, class CFn>
 OG_HD uint8_t note_encrypt_one(const Fr& pk_x, bool pk_odd, const Fr m[4], const Fr& e, const BjjBase& base, CFn c,
                                uint32_t rec[NOTE_RECORD_WORDS], Fr* cm) {
     const Fr A = bjj_a(), D = bjj_d();
@@ -67,7 +69,7 @@ OG_HD uint8_t note_encrypt_one(const Fr& pk_x, bool pk_odd, const Fr m[4], const
     note_store_word(rec, ex);
     if (fr_is_odd(ey)) rec[7] |= 0x80000000u;
     for (int i = 0; i < 4; i++) note_store_word(rec + 8 * (i + 1), m[i] + pad[i]);
-    *cm = note_commitment(m, c);
+    *cm = note_commitment<KEY>(m, c);
     return NOTE_ENC_OK;
 }
 
@@ -105,8 +107,8 @@ OG_HD void note_mul_window(BjjPoint* out, const Fr& px, const Fr& py, const uint
     *out = acc;
 }
 
-// the per-(record, key) half: the note if view key v (canonical limbs) owns the prepared record
-template <bool WINDOW, class CFn>
+// the per-(record, key) half: the note if view key v (canonical limbs) owns the prepared record, its commitment taken under KEY
+template <bool WINDOW, uint32_t KEY = 0, class CFn>
 OG_HD bool note_decrypt_one(const Fr& epx, const Fr& epy, const uint32_t v[8], const uint32_t* rec, const uint32_t* cm, CFn c,
                             Fr m[4]) {
     BjjPoint s;
@@ -125,7 +127,7 @@ OG_HD bool note_decrypt_one(const Fr& epx, const Fr& epy, const uint32_t v[8], c
     m[3].to_canonical(a);
     for (int i = 2; i < 8; i++)
         if (a[i]) return false;                       // amount >= 2^64: not a note (and no need to hash it)
-    return note_commitment(m, c) == Fr::from_canonical(cm);
+    return note_commitment<KEY>(m, c) == Fr::from_canonical(cm);
 }
 
 }  // namespace og

@@ -9,6 +9,8 @@
 //                        double-and-add (or the window digits) never diverge.  An owner is recorded with atomicMin, so the
 //                        lowest owning key index wins whatever the scheduling
 //   k_note_finish        one thread per record: zero plaintext, or the note decrypted again under the winning key
+// The encrypt, scan and finish kernels serve transfer notes (commitment key 0) and, with OWNED, spend-key notes (commitment
+// key 4, and a record is owned by key k only if its m0 is the spend public key P_k as well).
 #include "note_core.cuh"
 
 namespace og {
@@ -28,6 +30,7 @@ __global__ void __launch_bounds__(64) k_note_public_keys(const Fr* __restrict__ 
     pk_odd[i] = fr_is_odd(y) ? 1 : 0;
 }
 
+template <bool OWNED>
 __global__ void __launch_bounds__(64) k_note_encrypt(const Fr* __restrict__ base_tab, NoteEncryptInputs in, uint64_t n,
                                                      uint8_t* __restrict__ records, uint8_t* __restrict__ commitments,
                                                      uint8_t* __restrict__ status, int* flag) {
@@ -39,7 +42,8 @@ __global__ void __launch_bounds__(64) k_note_encrypt(const Fr* __restrict__ base
                load_canonical<Fr>(in.tokens + 32 * i, flag), Fr::from_canonical(a)};
     Fr pk_x = load_canonical<Fr>(in.pk_x + 32 * i, flag), e = load_canonical<Fr>(in.ephemerals + 32 * i, flag), cm;
     uint32_t w[NOTE_RECORD_WORDS];
-    status[i] = note_encrypt_one(pk_x, in.pk_odd[i] != 0, m, e, BjjBase{Fr::zero(), Fr::zero(), base_tab}, NoteC{}, w, &cm);
+    status[i] = note_encrypt_one<OWNED ? OWNED_COMMITMENT_KEY : 0>(pk_x, in.pk_odd[i] != 0, m, e, BjjBase{Fr::zero(), Fr::zero(), base_tab},
+                                                                  NoteC{}, w, &cm);
     uint32_t* out = reinterpret_cast<uint32_t*>(records + 160 * i);
 #pragma unroll
     for (uint32_t k = 0; k < NOTE_RECORD_WORDS; k++) out[k] = w[k];
@@ -58,10 +62,10 @@ __global__ void __launch_bounds__(128) k_note_prepare(const uint8_t* __restrict_
     owner[i] = ok ? NOTE_NOT_OWNED : NOTE_MALFORMED;
 }
 
-template <bool WINDOW>
-__global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ keys, const uint8_t* __restrict__ records,
-                                                  const uint8_t* __restrict__ commitments, const Fr* __restrict__ prepared, uint64_t n,
-                                                  uint32_t* owner) {
+template <bool WINDOW, bool OWNED>
+__global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ spend_keys,
+                                                  const uint8_t* __restrict__ records, const uint8_t* __restrict__ commitments,
+                                                  const Fr* __restrict__ prepared, uint64_t n, uint32_t* owner) {
     const uint32_t key = blockIdx.y;
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || owner[i] == NOTE_MALFORMED) return;     // MALFORMED is written by k_note_prepare only, never by atomicMin
@@ -69,11 +73,14 @@ __global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ k
 #pragma unroll
     for (int k = 0; k < 8; k++) v[k] = keys[8 * key + k];
     Fr m[4];
-    if (note_decrypt_one<WINDOW>(prepared[2 * i], prepared[2 * i + 1], v, reinterpret_cast<const uint32_t*>(records + 160 * i),
-                                 reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m))
+    if (note_decrypt_one<WINDOW, OWNED ? OWNED_COMMITMENT_KEY : 0>(prepared[2 * i], prepared[2 * i + 1], v,
+                                                                   reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                                                   reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m) &&
+        (!OWNED || m[0] == Fr::from_canonical(spend_keys + 8 * key)))
         atomicMin(owner + i, key);
 }
 
+template <bool OWNED>
 __global__ void __launch_bounds__(64) k_note_finish(const uint32_t* __restrict__ keys, uint32_t n_keys, const uint8_t* __restrict__ records,
                                                     const uint8_t* __restrict__ commitments, const Fr* __restrict__ prepared, uint64_t n,
                                                     const uint32_t* __restrict__ owner, uint8_t* __restrict__ plaintexts) {
@@ -82,8 +89,9 @@ __global__ void __launch_bounds__(64) k_note_finish(const uint32_t* __restrict__
     const uint32_t o = owner[i];
     Fr m[4] = {Fr::zero(), Fr::zero(), Fr::zero(), Fr::zero()};
     if (o < n_keys)
-        note_decrypt_one<false>(prepared[2 * i], prepared[2 * i + 1], keys + 8ull * o, reinterpret_cast<const uint32_t*>(records + 160 * i),
-                                reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m);
+        note_decrypt_one<false, OWNED ? OWNED_COMMITMENT_KEY : 0>(prepared[2 * i], prepared[2 * i + 1], keys + 8ull * o,
+                                                                  reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                                                  reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m);
     for (int k = 0; k < 4; k++) store_canonical(plaintexts + 128 * i + 32 * k, m[k]);
 }
 
@@ -121,17 +129,22 @@ int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uin
     return OG_OK;
 }
 
-int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status) {
+int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status,
+                         bool owned) {
     if (n == 0) return OG_OK;
     const Fr* tab;
     OG_TRY(bjj_table(ctx, &tab));
-    OG_LAUNCH(ctx, k_note_encrypt, (unsigned)((n + 63) / 64), 64, 0, tab, in, n, d_records, d_commitments, d_status, ctx->d_flag);
+    const unsigned blocks = (unsigned)((n + 63) / 64);
+    // profile names: the transfer-note kernels keep theirs, the spend-key-note instances are named k_owned_note_*
+    if (owned) OG_LAUNCHN(ctx, "k_owned_note_encrypt", k_note_encrypt<true>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status, ctx->d_flag);
+    else OG_LAUNCHN(ctx, "k_note_encrypt", k_note_encrypt<false>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status, ctx->d_flag);
     return OG_OK;
 }
 
-// d_keys: n_keys checked view keys (canonical limbs) in device memory; the prepared points go to a context slot
+// d_keys: n_keys checked view keys (canonical limbs) in device memory, and d_spend_keys their checked spend public keys for
+// spend-key notes or nullptr for transfer notes; the prepared points go to a context slot
 int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
-                      uint32_t* d_owner, uint8_t* d_plaintexts) {
+                      uint32_t* d_owner, uint8_t* d_plaintexts, const uint32_t* d_spend_keys) {
     if (n == 0) return OG_OK;
     if (n_keys > 65535) { snprintf(ctx->err, sizeof(ctx->err), "at most 65535 view keys per scan"); return OG_E_INVALID; }
     OG_SLOT(ctx, prep, Fr, S_NOTE_PREP, sizeof(Fr) * 2 * n);
@@ -141,10 +154,19 @@ int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, cons
         // the variable-base multiplier: the 4-bit window, or plain double-and-add with OG_NOTE_WINDOW=0 (DESIGN.md section 8:
         // the window is 15 % faster at 2^20 records x 8 keys on an H100)
         const char* w = getenv("OG_NOTE_WINDOW");
-        if (!w || atoi(w) != 0) OG_LAUNCH(ctx, k_note_scan<true>, dim3(blocks, n_keys), 64, 0, d_keys, d_records, d_commitments, prep, n, d_owner);
-        else OG_LAUNCH(ctx, k_note_scan<false>, dim3(blocks, n_keys), 64, 0, d_keys, d_records, d_commitments, prep, n, d_owner);
+        const bool window = !w || atoi(w) != 0;
+        const dim3 grid(blocks, n_keys);
+        const bool owned = d_spend_keys != nullptr;
+        const auto kernel = owned ? (window ? k_note_scan<true, true> : k_note_scan<false, true>)
+                                  : (window ? k_note_scan<true, false> : k_note_scan<false, false>);
+        const char* name = owned ? (window ? "k_owned_note_scan<true>" : "k_owned_note_scan<false>")
+                                 : (window ? "k_note_scan<true>" : "k_note_scan<false>");
+        OG_LAUNCHN(ctx, name, kernel, grid, 64, 0, d_keys, d_spend_keys, d_records, d_commitments, prep, n, d_owner);
     }
-    OG_LAUNCH(ctx, k_note_finish, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n, d_owner, d_plaintexts);
+    if (d_spend_keys) OG_LAUNCHN(ctx, "k_owned_note_finish", k_note_finish<true>, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n,
+                                 d_owner, d_plaintexts);
+    else OG_LAUNCHN(ctx, "k_note_finish", k_note_finish<false>, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n, d_owner,
+                    d_plaintexts);
     return OG_OK;
 }
 

@@ -42,6 +42,12 @@
 //            assoc_siblings[depth], assoc_bits[depth]
 //   the labeled statement's note part (LabeledNoteBuilder); assoc_leaf = label + 1 reaching association_root along the
 //   association path (one depth for both trees); recipient^2 bound.
+// owned_transfer
+//   public : root, public_amount, token, recipient, nullifier[2], out_commitment[2]
+//   private: two input notes (spend_key, blinding, amount, siblings[depth], bits[depth]), two output notes (owner, blinding,
+//            amount)
+//   owner = MultiMiMC7([spend_key], 3); note commitment = MultiMiMC7([owner, blinding, token, amount], 4); nullifier =
+//   MultiMiMC7([spend_key, commitment, leaf index], 5); otherwise the transfer statement's rows.
 #pragma once
 #include <map>
 #include <vector>
@@ -368,6 +374,59 @@ struct LabeledAssociationBuilder {
     }
 };
 
+struct OwnedTransferBuilder {
+    // commitment = MultiMiMC7([owner, blinding, token, amount], 4) of the note block at `v`, rounds from `cm`
+    static void commitment(Mimc7Builder& b, const LC& owner, uint32_t v, uint32_t cm, uint32_t cm_out, uint32_t P) {
+        LC key; key[0] = Fr::from_u32(OWNED_COMMITMENT_KEY);
+        LC bl = lc_var(v + 1), tok = lc_var(3), am = lc_var(v + 2);
+        b.multi_hash({&owner, &bl, &tok, &am}, key, {cm, cm + P, cm + 2 * P, cm + 3 * P}, cm_out);
+    }
+
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        OwnedTransferLayout L = OwnedTransferLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = OWNED_TRANSFER_N_PUB;
+        const uint32_t V_ONE = 0, V_ROOT = 1, V_PUB_AMOUNT = 2, V_RECIP = 4, V_NF = 5, V_OUT_CM = 7, V_RSQ = 9, V_NF_INV = 10;
+        const uint32_t P = L.perm;
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        for (uint32_t i = 0; i < 2; i++) {
+            const uint32_t v = L.inp(i);
+            // owner P = MultiMiMC7([s], 3) = 3 + s + hash(s, 3), kept as a linear combination
+            LC s = lc_var(v), k3; k3[V_ONE] = Fr::from_u32(OWNED_OWNER_KEY);
+            LC h = b.perm(s, k3, v + L.owner_perm);
+            LC owner = lc_sum({&k3, &s, &h});
+            commitment(b, owner, v, v + L.in_cm, v + L.in_cm_out, P);
+            const uint32_t cur = b.merkle_path(v + L.in_cm_out, v + L.lvl_base, L.lvl_size, depth);
+            LC vroot = lc_var(V_ROOT), ncur = lc_neg_var(cur);
+            b.cs.add(lc_sum({&vroot, &ncur}), lc_var(v + 2), LC());
+            b.range(lc_var(v + 2), v + 3, TRANSFER_AMOUNT_BITS);
+            // nullifier = MultiMiMC7([s, cm, index], 5), index = sum 2^l bit_l over the path bits, bound to nf[i] directly
+            LC cm = lc_var(v + L.in_cm_out), index, k5; k5[V_ONE] = Fr::from_u32(OWNED_NULLIFIER_KEY);
+            Fr pow2 = Fr::one();
+            for (uint32_t l = 0; l < depth; l++) {
+                lc_add_term(index, v + L.lvl_base + l * L.lvl_size + 1, pow2);
+                pow2 = pow2 + pow2;
+            }
+            const uint32_t nf = v + L.nf_perm;
+            b.multi_hash({&s, &cm, &index}, k5, {nf, nf + P, nf + 2 * P}, V_NF + i);
+        }
+        for (uint32_t j = 0; j < 2; j++) {
+            const uint32_t v = L.out(j);
+            b.range(lc_var(v + 2), v + 3, TRANSFER_AMOUNT_BITS);
+            commitment(b, lc_var(v), v, v + L.out_cm, v + L.out_cm_out, P);
+            LC vout = lc_var(v + L.out_cm_out), ncm = lc_neg_var(V_OUT_CM + j);
+            b.cs.add(lc_sum({&vout, &ncm}), lc_var(V_ONE), LC());
+        }
+        LC i0 = lc_var(L.inp(0) + 2), i1 = lc_var(L.inp(1) + 2), pa = lc_var(V_PUB_AMOUNT);
+        LC o0 = lc_neg_var(L.out(0) + 2), o1 = lc_neg_var(L.out(1) + 2);
+        b.cs.add(lc_sum({&i0, &i1, &pa, &o0, &o1}), lc_var(V_ONE), LC());
+        LC nf0 = lc_var(V_NF), nf1 = lc_neg_var(V_NF + 1);
+        b.cs.add(lc_sum({&nf0, &nf1}), lc_var(V_NF_INV), lc_var(V_ONE));
+        return b.cs;
+    }
+};
+
 // the statement's R1CS at `depth` (ignored by deposit)
 inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     switch (s) {
@@ -378,6 +437,7 @@ inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     case ST_EXCLUSION: return ExclusionBuilder::build(depth);
     case ST_LABELED: return LabeledBuilder::build(depth);
     case ST_LABELED_ASSOCIATION: return LabeledAssociationBuilder::build(depth);
+    case ST_OWNED_TRANSFER: return OwnedTransferBuilder::build(depth);
     }
     return R1cs();
 }
