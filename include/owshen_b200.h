@@ -173,6 +173,26 @@ int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t*
 int32_t og_owned_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
                                const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
                                uint8_t* d_out_plaintexts);
+/* Owned labeled notes (the owned labeled transfer statement's, below): the same 160-byte record of the four words (owner P,
+ * blinding, token, amount + 2^64 label), the note's key-7 leaf as commitment and status as og_note_encrypt's; labels are
+ * uint32, one per note. */
+int32_t og_owned_labeled_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners,
+                                      const uint8_t* blindings, const uint8_t* tokens, const uint64_t* amounts, const uint32_t* labels,
+                                      const uint8_t* ephemerals, uint64_t n, uint8_t* out_records, uint8_t* out_commitments,
+                                      uint8_t* out_status);
+int32_t og_owned_labeled_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
+                                          const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts,
+                                          const uint32_t* d_labels, const uint8_t* d_ephemerals, uint64_t n, uint8_t* d_out_records,
+                                          uint8_t* d_out_commitments, uint8_t* d_out_status);
+/* og_owned_note_scan for owned labeled notes: key k owns a record only if the record decrypts under v_k, word 3 is below
+ * 2^96, the first word is P_k, and the key-7 leaf of (MultiMiMC7([m0, m1], 6), m2, word 3 mod 2^64, word 3 >> 64) matches.
+ * A plaintext is the four words, word 3 = amount + 2^64 label. */
+int32_t og_owned_labeled_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                                   const uint8_t* records, const uint8_t* commitments, uint64_t n, uint32_t* out_owner,
+                                   uint8_t* out_plaintexts);
+int32_t og_owned_labeled_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                                       const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
+                                       uint8_t* d_out_plaintexts);
 
 /* ---- MSM (BASELINE configs 3 and 5) ----------------------------------------------------------- */
 int32_t og_msm_g1(og_ctx* ctx, const uint8_t* points, const uint8_t* scalars, uint64_t n, uint8_t* out64);
@@ -354,6 +374,35 @@ int32_t og_owned_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* ro
                                   const uint8_t* out_owners, const uint8_t* out_blindings, const uint64_t* out_amounts,
                                   uint32_t batch, uint8_t* witnesses);
 
+/* ---- owned labeled notes and the owned labeled transfer statement (DESIGN.md section 3): private transfers of spend-key
+ * notes that carry their deposit's label, checked against a provider's approved list ---- */
+/* An owned labeled note is (P, blinding, token, amount < 2^64, label < 2^32): precommitment MultiMiMC7([P, blinding], 6),
+ * leaf MultiMiMC7([precommitment, token, amount, label], 7); its nullifier is og_owned_nullifiers' of (s, leaf, index).
+ * n items each, 32 B field elements in and out; amounts uint64, labels uint32. */
+int32_t og_owned_labeled_precommitments(og_ctx* ctx, const uint8_t* owners, const uint8_t* blindings, uint64_t n, uint8_t* out);
+int32_t og_owned_labeled_leaves(og_ctx* ctx, const uint8_t* precommitments, const uint8_t* tokens, const uint64_t* amounts,
+                                const uint32_t* labels, uint64_t n, uint8_t* out);
+/* Public inputs (root, association_root, token, withdrawn, recipient, nullifier[2], out_commitment[2]): two owned labeled
+ * notes of one label in, two out under the same label, withdrawn (< 2^64) paid to recipient, in0 + in1 = out0 + out1 +
+ * withdrawn, and label + 1 a leaf of the approved-label tree under association_root.  depth 1..32; at depth 32: 82 306
+ * variables, 82 201 constraints, domain 2^17. */
+int32_t og_owned_labeled_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_owned_labeled_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                              uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: root, token, recipient (32 B each), withdrawn
+ * (uint64), label (uint32), in_spend_keys, in_blindings (2 x 32 B), in_amounts (2 x uint64), in_siblings (2 x depth x 32 B),
+ * in_path_bits (2 x uint32), out_owners, out_blindings (2 x 32 B), out_amounts (2 x uint64), assoc_siblings (depth x 32 B),
+ * assoc_path_bits (uint32).  root is the caller's and association_root is derived: a wrong spend key, an input of nonzero
+ * amount that does not reach root under this label, an unapproved label, an overdraw or two inputs with one nullifier give
+ * a witness that does not satisfy the R1CS. */
+int32_t og_owned_labeled_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                          const uint64_t* withdrawn, const uint32_t* labels, const uint8_t* in_spend_keys,
+                                          const uint8_t* in_blindings, const uint64_t* in_amounts, const uint8_t* in_siblings,
+                                          const uint32_t* in_path_bits, const uint8_t* out_owners, const uint8_t* out_blindings,
+                                          const uint64_t* out_amounts, const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits,
+                                          uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -490,6 +539,24 @@ int32_t og_groth16_prove_owned_transfer_dev(og_ctx* ctx, const og_pk* pk, const 
                                             const uint64_t* d_in_amounts, const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits,
                                             const uint8_t* d_out_owners, const uint8_t* d_out_blindings, const uint64_t* d_out_amounts,
                                             uint32_t batch, const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of owned labeled transfer proofs, witness generation on the GPU; inputs as in og_owned_labeled_transfer_witness.
+ * OG_E_INVALID unless the key has an owned labeled transfer statement's shape (the depth is recognised from it).
+ * public_out (optional): batch * 9 * 32 B = root, association_root, token, withdrawn, recipient, nullifier[2],
+ * out_commitment[2]. */
+int32_t og_groth16_prove_owned_labeled_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens,
+                                                const uint8_t* recipients, const uint64_t* withdrawn, const uint32_t* labels,
+                                                const uint8_t* in_spend_keys, const uint8_t* in_blindings, const uint64_t* in_amounts,
+                                                const uint8_t* in_siblings, const uint32_t* in_path_bits, const uint8_t* out_owners,
+                                                const uint8_t* out_blindings, const uint64_t* out_amounts, const uint8_t* assoc_siblings,
+                                                const uint32_t* assoc_path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
+                                                uint8_t* public_out);
+int32_t og_groth16_prove_owned_labeled_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
+                                                    const uint8_t* d_recipients, const uint64_t* d_withdrawn, const uint32_t* d_labels,
+                                                    const uint8_t* d_in_spend_keys, const uint8_t* d_in_blindings, const uint64_t* d_in_amounts,
+                                                    const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits, const uint8_t* d_out_owners,
+                                                    const uint8_t* d_out_blindings, const uint64_t* d_out_amounts,
+                                                    const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
+                                                    const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

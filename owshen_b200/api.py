@@ -83,6 +83,12 @@ _SIGS = {
                                        C.c_void_p]),
     "og_owned_note_scan_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
                                            C.c_void_p]),
+    "og_owned_labeled_note_encrypt": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 8 + [C.c_uint64] + [C.c_void_p] * 3),
+    "og_owned_labeled_note_encrypt_dev": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 8 + [C.c_uint64] + [C.c_void_p] * 3),
+    "og_owned_labeled_note_scan": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64,
+                                               C.c_void_p, C.c_void_p]),
+    "og_owned_labeled_note_scan_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64,
+                                                   C.c_void_p, C.c_void_p]),
     "og_msm_g1": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "og_msm_g2": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "og_msm_g1_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -126,6 +132,11 @@ _SIGS = {
     "og_owned_transfer_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_owned_transfer_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_owned_transfer_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p]),
+    "og_owned_labeled_precommitments": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 2 + [C.c_uint64, C.c_void_p]),
+    "og_owned_labeled_leaves": (C.c_int32, [C.c_void_p] + [C.c_void_p] * 4 + [C.c_uint64, C.c_void_p]),
+    "og_owned_labeled_transfer_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_owned_labeled_transfer_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_owned_labeled_transfer_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -152,6 +163,10 @@ _SIGS = {
     "og_groth16_prove_owned_transfer": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_owned_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 11
                                             + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_owned_labeled_transfer": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15
+                                                + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_owned_labeled_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15
+                                                    + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -294,6 +309,12 @@ _STATEMENTS = {
                               ("in_blindings", 64, 0, None), ("in_amounts", 16, 0, _u64_array), ("in_siblings", 0, 64, None),
                               ("in_path_bits", 8, 0, _u32_array), ("out_owners", 64, 0, None), ("out_blindings", 64, 0, None),
                               ("out_amounts", 16, 0, _u64_array))),
+    "owned_labeled_transfer": (True, (("roots", 32, 0, None), ("tokens", 32, 0, None), ("recipients", 32, 0, None),
+                                      ("withdrawn", 8, 0, _u64_array), ("labels", 4, 0, _label_array), ("in_spend_keys", 64, 0, None),
+                                      ("in_blindings", 64, 0, None), ("in_amounts", 16, 0, _u64_array), ("in_siblings", 0, 64, None),
+                                      ("in_path_bits", 8, 0, _u32_array), ("out_owners", 64, 0, None), ("out_blindings", 64, 0, None),
+                                      ("out_amounts", 16, 0, _u64_array), ("assoc_siblings", 0, 32, None),
+                                      ("assoc_path_bits", 4, 0, _u32_array))),
 }
 
 
@@ -635,6 +656,80 @@ class Context:
         _check(lib().og_owned_nullifiers(self._h, spend_keys, commitments, _ptr(idx), n, out), self)
         return out.raw
 
+    # ---- owned labeled notes (DESIGN.md section 3, "Owned labeled transfers") ----------------------------------------
+    def owned_labeled_precommitments(self, owners: bytes, blindings: bytes) -> bytes:
+        """MultiMiMC7([owner, blinding], 6) of each note (32 bytes each in and out): what a depositor sends the node, which
+        does not reveal the owner."""
+        _need(len(owners) % 32 == 0 and len(blindings) == len(owners),
+              "owned_labeled_precommitments: owners and blindings must be equally long multiples of 32 bytes")
+        n = len(owners) // 32
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_owned_labeled_precommitments(self._h, owners, blindings, n, out), self)
+        return out.raw
+
+    def owned_labeled_leaves(self, precommitments: bytes, tokens: bytes, amounts, labels) -> bytes:
+        """MultiMiMC7([precommitment, token, amount, label], 7) of each note: precommitments and tokens 32 bytes each, amounts
+        uint64 and labels uint32 (little-endian buffers, arrays or sequences of ints)."""
+        _need(len(precommitments) % 32 == 0 and len(tokens) == len(precommitments),
+              "owned_labeled_leaves: precommitments and tokens must be equally long multiples of 32 bytes")
+        n = len(precommitments) // 32
+        am, la = _u64_array(amounts), _label_array(labels)
+        for name, buf, size in (("amounts", am, 8), ("labels", la, 4)):
+            _need((C.sizeof(buf) if isinstance(buf, C.Array) else _blen(buf)) == size * n,
+                  f"owned_labeled_leaves: expected one {name[:-1]} per note")
+        out = C.create_string_buffer(32 * n)
+        _check(lib().og_owned_labeled_leaves(self._h, precommitments, tokens, _ptr(am), _ptr(la), n, out), self)
+        return out.raw
+
+    def owned_labeled_note_encrypt(self, pk_x: bytes, pk_is_odd: bytes, owners: bytes, blindings: bytes, tokens: bytes, amounts,
+                                   labels, ephemerals=None):
+        """note_encrypt for owned labeled notes (owner P, blinding, token, amount, label): the records of the four words (P,
+        blinding, token, amount + 2^64 label), with the notes' key-7 leaves as commitments -> (records, commitments, status)."""
+        n = len(pk_is_odd)
+        if ephemerals is None:
+            ephemerals = b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n))
+        am, la = _u64_array(amounts), _label_array(labels)
+        for name, buf in (("pk_x", pk_x), ("owners", owners), ("blindings", blindings), ("tokens", tokens), ("ephemerals", ephemerals)):
+            _need(len(buf) == 32 * n, f"owned_labeled_note_encrypt: {name}: expected {32 * n} bytes, got {len(buf)}")
+        for name, buf, size in (("amounts", am, 8), ("labels", la, 4)):
+            _need((C.sizeof(buf) if isinstance(buf, C.Array) else _blen(buf)) == size * n,
+                  f"owned_labeled_note_encrypt: expected one {name[:-1]} per note")
+        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
+        _check(lib().og_owned_labeled_note_encrypt(self._h, pk_x, pk_is_odd, owners, blindings, tokens, _ptr(am), _ptr(la), ephemerals, n,
+                                                   rec, cm, st), self)
+        return rec.raw, cm.raw, st.raw[:n]
+
+    def owned_labeled_note_encrypt_dev(self, d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_labels, d_ephemerals,
+                                       n: int, d_out_records, d_out_commitments, d_out_status):
+        """og_owned_labeled_note_encrypt_dev: device buffers (addresses or tensors), enqueued on the context's stream."""
+        _check(lib().og_owned_labeled_note_encrypt_dev(self._h, *[_ptr(x) for x in (d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens,
+                                                                                   d_amounts, d_labels, d_ephemerals)], n,
+                                                       *[_ptr(x) for x in (d_out_records, d_out_commitments, d_out_status)]), self)
+
+    def owned_labeled_note_scan(self, view_keys: bytes, spend_public_keys: bytes, records: bytes, commitments: bytes):
+        """owned_note_scan for owned labeled notes -> (owners, plaintexts, amounts, labels): owners as note_scan's, the
+        plaintext words (owner, blinding, token, amount + 2^64 label) as og_owned_labeled_note_scan returns them, and each
+        record's amount and label split from word 3 (0 unless owned)."""
+        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
+              "owned_labeled_note_scan: view keys and spend public keys must be equally long multiples of 32 bytes")
+        _need(len(records) % 160 == 0, "owned_labeled_note_scan: records must be a multiple of 160 bytes")
+        n = len(records) // 160
+        _need(len(commitments) == 32 * n, "owned_labeled_note_scan: expected one 32-byte commitment per record")
+        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
+        _check(lib().og_owned_labeled_note_scan(self._h, view_keys, spend_public_keys, len(view_keys) // 32, records, commitments, n,
+                                                owner, plain), self)
+        words3 = [int.from_bytes(plain.raw[128 * i + 96:128 * i + 128], "little") for i in range(n)]
+        return list(owner), plain.raw, [w & ((1 << 64) - 1) for w in words3], [w >> 64 for w in words3]
+
+    def owned_labeled_note_scan_dev(self, view_keys: bytes, spend_public_keys: bytes, d_records, d_commitments, n: int, d_out_owner,
+                                    d_out_plaintexts):
+        """og_owned_labeled_note_scan_dev: the keys on the host, every other buffer on the device, enqueued on the context's
+        stream; the plaintexts keep word 3 = amount + 2^64 label."""
+        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
+              "owned_labeled_note_scan_dev: view keys and spend public keys must be equally long multiples of 32 bytes")
+        _check(lib().og_owned_labeled_note_scan_dev(self._h, view_keys, spend_public_keys, len(view_keys) // 32, _ptr(d_records),
+                                                    _ptr(d_commitments), n, _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
+
     def msm_g1(self, points: bytes, scalars: bytes) -> bytes:
         _need(len(scalars) % 32 == 0, "msm_g1: scalars must be a multiple of 32 bytes")
         n = len(scalars) // 32
@@ -779,6 +874,17 @@ class Context:
         return self._statement_witness("owned_transfer", depth, (roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts,
                                                                  in_siblings, in_path_bits, out_owners, out_blindings, out_amounts))
 
+    def owned_labeled_transfer_witness(self, depth, roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings,
+                                       in_amounts, in_siblings, in_path_bits, out_owners, out_blindings, out_amounts, assoc_siblings,
+                                       assoc_path_bits) -> bytes:
+        """Full assignments of the depth-`depth` owned labeled transfer statement, n_vars * 32 bytes per transfer, computed on
+        the GPU.  Per transfer: root, token, recipient 32 bytes each; withdrawn one uint64 and the label one uint32; the inputs
+        and outputs as in owned_transfer_witness; assoc_siblings depth elements and assoc_path_bits one word, the path of
+        label + 1 in the provider's approved-label tree (ApprovedLabels.witness)."""
+        return self._statement_witness("owned_labeled_transfer", depth, (roots, tokens, recipients, withdrawn, labels, in_spend_keys,
+                                                                         in_blindings, in_amounts, in_siblings, in_path_bits, out_owners,
+                                                                         out_blindings, out_amounts, assoc_siblings, assoc_path_bits))
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -878,6 +984,15 @@ def owned_transfer_r1cs_export(depth: int, which: str):
     return _statement_r1cs_export("owned_transfer", depth, which)
 
 
+def owned_labeled_transfer_r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("owned_labeled_transfer", depth)
+
+
+def owned_labeled_transfer_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` owned labeled transfer R1CS."""
+    return _statement_r1cs_export("owned_labeled_transfer", depth, which)
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -955,6 +1070,12 @@ def setup_owned_transfer(ctx: Context, depth: int, tau: int, alpha: int, beta: i
     """Development setup of the depth-`depth` owned transfer statement -> (pk_bytes, vk_bytes): its exported R1CS through
     setup_r1cs.  The key records depth 0; the prover recognises it as an owned transfer key by its shape."""
     return _setup_statement(ctx, "owned_transfer", depth, (tau, alpha, beta, gamma, delta))
+
+
+def setup_owned_labeled_transfer(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` owned labeled transfer statement -> (pk_bytes, vk_bytes): its exported R1CS
+    through setup_r1cs.  The key records depth 0; the prover recognises it as an owned labeled transfer key by its shape."""
+    return _setup_statement(ctx, "owned_labeled_transfer", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -1051,6 +1172,10 @@ def ptau_prepare_labeled_association(ctx: Context, acc: bytes, depth: int):
 
 def ptau_prepare_owned_transfer(ctx: Context, acc: bytes, depth: int):
     return _ptau_prepare_statement(ctx, acc, "owned_transfer", depth)
+
+
+def ptau_prepare_owned_labeled_transfer(ctx: Context, acc: bytes, depth: int):
+    return _ptau_prepare_statement(ctx, acc, "owned_labeled_transfer", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -1232,6 +1357,23 @@ class ProvingKey:
         return self._prove_statement("owned_transfer", self.owned_transfer_depth,
                                      (roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings, in_path_bits,
                                       out_owners, out_blindings, out_amounts), rs, want_public)
+
+    @property
+    def owned_labeled_transfer_depth(self):
+        """The depth d whose owned labeled transfer statement has this key's shape (owned_labeled_transfer_r1cs_info), or
+        None."""
+        return self._shape_depth("owned_labeled_transfer")
+
+    def prove_owned_labeled_transfer(self, roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings, in_amounts,
+                                     in_siblings, in_path_bits, out_owners, out_blindings, out_amounts, assoc_siblings, assoc_path_bits,
+                                     rs, want_public=True):
+        """Batch of owned labeled transfer proofs from the notes (witness generation on the GPU).  Inputs as in
+        Context.owned_labeled_transfer_witness; returns (proofs, public_inputs) with public inputs (root, association_root,
+        token, withdrawn, recipient, nullifier[2], out_commitment[2]) per proof."""
+        return self._prove_statement("owned_labeled_transfer", self.owned_labeled_transfer_depth,
+                                     (roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings, in_amounts, in_siblings,
+                                      in_path_bits, out_owners, out_blindings, out_amounts, assoc_siblings, assoc_path_bits), rs,
+                                     want_public)
 
     def prover_plan(self, batch: int) -> dict:
         """How the prover runs `batch` proofs with this key: chunk (proofs per chunk), lanes (chunks in flight) and
@@ -1425,6 +1567,22 @@ def deposit_labeled(tree: MerkleTree, precommitments: bytes, tokens: bytes, amou
         raise OverflowError(f"tree of depth {tree.depth} holds {1 << tree.depth} leaves; {start} present, {n} more requested")
     labels = list(range(start, start + n))
     leaves = tree.ctx.labeled_leaves(precommitments, tokens, amounts, labels)
+    tree.insert_batch([leaves[32 * k:32 * k + 32] for k in range(n)])
+    return labels
+
+
+def deposit_owned_labeled(tree: MerkleTree, precommitments: bytes, tokens: bytes, amounts):
+    """Append owned labeled deposits to the pool tree -> their labels: deposit_labeled for owned labeled notes.  The node
+    assigns each deposit the next pool leaf index as its label, computes the leaf MultiMiMC7([precommitment, token, amount,
+    label], 7) on the GPU from what the depositor sent (precommitments MultiMiMC7([P, blinding], 6) and tokens 32 bytes each,
+    amounts uint64), and inserts the leaves in one insert_batch.  It never takes a leaf from the depositor."""
+    _need(len(precommitments) % 32 == 0 and len(tokens) == len(precommitments),
+          "deposit_owned_labeled: precommitments and tokens must be equally long multiples of 32 bytes")
+    n, start = len(precommitments) // 32, tree.n_leaves
+    if start + n > (1 << tree.depth):
+        raise OverflowError(f"tree of depth {tree.depth} holds {1 << tree.depth} leaves; {start} present, {n} more requested")
+    labels = list(range(start, start + n))
+    leaves = tree.ctx.owned_labeled_leaves(precommitments, tokens, amounts, labels)
     tree.insert_batch([leaves[32 * k:32 * k + 32] for k in range(n)])
     return labels
 

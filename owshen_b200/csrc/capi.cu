@@ -728,7 +728,7 @@ int32_t og_owned_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint
     if (n && (!d_pk_x || !d_pk_is_odd || !d_owners || !d_blindings || !d_tokens || !d_amounts || !d_ephemerals || !d_out_records ||
               !d_out_commitments || !d_out_status)) return OG_E_INVALID;
     return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals}, n,
-                            d_out_records, d_out_commitments, d_out_status, true);
+                            d_out_records, d_out_commitments, d_out_status, NOTE_OWNED);
 }
 
 int32_t og_owned_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners, const uint8_t* blindings,
@@ -746,7 +746,7 @@ int32_t og_owned_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* p
     OG_TRY(clear_flag(ctx));
     H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
     H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n);
-    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dow, dbl, dto, da, de}, n, drec, dcm, dst, true));
+    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dow, dbl, dto, da, de}, n, drec, dcm, dst, NOTE_OWNED));
     D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
     return check_flag(ctx);
 }
@@ -777,7 +777,7 @@ int32_t og_owned_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint
         return OG_E_INVALID;
     const uint32_t *dk, *ds;
     OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
-    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, ds);
+    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, NOTE_OWNED, ds);
 }
 
 int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys, const uint8_t* records,
@@ -792,7 +792,71 @@ int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t*
     uint32_t* downer = reinterpret_cast<uint32_t*>(io);
     uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
     H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
-    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, ds));
+    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, NOTE_OWNED, ds));
+    D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
+    OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return OG_OK;
+}
+
+// ---- owned labeled notes: encryption and scanning (note_impl.cuh, NOTE_OWNED_LABELED) ----------------------------------
+int32_t og_owned_labeled_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
+                                          const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts,
+                                          const uint32_t* d_labels, const uint8_t* d_ephemerals, uint64_t n, uint8_t* d_out_records,
+                                          uint8_t* d_out_commitments, uint8_t* d_out_status) {
+    OG_ENTER(ctx);
+    if (n && (!d_pk_x || !d_pk_is_odd || !d_owners || !d_blindings || !d_tokens || !d_amounts || !d_labels || !d_ephemerals ||
+              !d_out_records || !d_out_commitments || !d_out_status)) return OG_E_INVALID;
+    return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals}, n,
+                            d_out_records, d_out_commitments, d_out_status, NOTE_OWNED_LABELED, d_labels);
+}
+
+int32_t og_owned_labeled_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners,
+                                      const uint8_t* blindings, const uint8_t* tokens, const uint64_t* amounts, const uint32_t* labels,
+                                      const uint8_t* ephemerals, uint64_t n, uint8_t* out_records, uint8_t* out_commitments,
+                                      uint8_t* out_status) {
+    OG_ENTER(ctx);
+    if (n && (!pk_x || !pk_is_odd || !owners || !blindings || !tokens || !amounts || !labels || !ephemerals || !out_records ||
+              !out_commitments || !out_status)) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    // og_note_encrypt's staging with the labels after the amounts, where they stay 4-byte aligned
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 366ull * n);
+    uint64_t* da = reinterpret_cast<uint64_t*>(io);
+    uint32_t* dla = reinterpret_cast<uint32_t*>(io + 8 * n);
+    uint8_t *dx = io + 12 * n, *dow = dx + 32 * n, *dbl = dow + 32 * n, *dto = dbl + 32 * n, *de = dto + 32 * n;
+    uint8_t *drec = de + 32 * n, *dcm = drec + 160 * n, *dodd = dcm + 32 * n, *dst = dodd + n;
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
+    H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n); H2D(ctx, dla, labels, 4 * n);
+    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dow, dbl, dto, da, de}, n, drec, dcm, dst, NOTE_OWNED_LABELED, dla));
+    D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
+    return check_flag(ctx);
+}
+
+int32_t og_owned_labeled_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                                       const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
+                                       uint8_t* d_out_plaintexts) {
+    OG_ENTER(ctx);
+    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!d_records || !d_commitments || !d_out_owner || !d_out_plaintexts)))
+        return OG_E_INVALID;
+    const uint32_t *dk, *ds;
+    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
+    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, NOTE_OWNED_LABELED, ds);
+}
+
+int32_t og_owned_labeled_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                                   const uint8_t* records, const uint8_t* commitments, uint64_t n, uint32_t* out_owner,
+                                   uint8_t* out_plaintexts) {
+    OG_ENTER(ctx);
+    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!records || !commitments || !out_owner || !out_plaintexts)))
+        return OG_E_INVALID;
+    const uint32_t *dk, *ds;
+    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // og_note_scan's staging
+    uint32_t* downer = reinterpret_cast<uint32_t*>(io);
+    uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
+    H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
+    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, NOTE_OWNED_LABELED, ds));
     D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return OG_OK;
@@ -1191,6 +1255,54 @@ int32_t og_owned_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* ro
                                                              in_path_bits, out_owners, out_blindings, out_amounts}, batch, witnesses);
 }
 
+// ---- owned labeled notes and the owned labeled transfer statement ----------------------------------------------------
+int32_t og_owned_labeled_precommitments(og_ctx* ctx, const uint8_t* owners, const uint8_t* blindings, uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !owners || !blindings || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dow, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, dbl, uint8_t, S_IO_B, 32 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_C, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
+    OG_TRY(owned_labeled_precommitments_dev(ctx, dow, dbl, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_owned_labeled_leaves(og_ctx* ctx, const uint8_t* precommitments, const uint8_t* tokens, const uint64_t* amounts,
+                                const uint32_t* labels, uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    if (!ctx || !precommitments || !tokens || !amounts || !labels || !out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    OG_SLOT(ctx, dp, uint8_t, S_IO_A, 32 * n);
+    OG_SLOT(ctx, dt, uint8_t, S_IO_B, 32 * n);
+    OG_SLOT(ctx, da, uint64_t, S_IO_C, 8 * n);
+    OG_SLOT(ctx, dl, uint32_t, S_IO_D, 4 * n);
+    OG_SLOT(ctx, dout, uint8_t, S_IO_E, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    H2D(ctx, dp, precommitments, 32 * n); H2D(ctx, dt, tokens, 32 * n); H2D(ctx, da, amounts, 8 * n); H2D(ctx, dl, labels, 4 * n);
+    OG_TRY(owned_labeled_leaves_dev(ctx, dp, dt, da, dl, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+int32_t og_owned_labeled_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_OWNED_LABELED_TRANSFER, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_owned_labeled_transfer_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs,
+                                              uint64_t* nnz) {
+    return statement_r1cs_export(ST_OWNED_LABELED_TRANSFER, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
+int32_t og_owned_labeled_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                          const uint64_t* withdrawn, const uint32_t* labels, const uint8_t* in_spend_keys,
+                                          const uint8_t* in_blindings, const uint64_t* in_amounts, const uint8_t* in_siblings,
+                                          const uint32_t* in_path_bits, const uint8_t* out_owners, const uint8_t* out_blindings,
+                                          const uint64_t* out_amounts, const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits,
+                                          uint32_t batch, uint8_t* witnesses) {
+    return statement_witness(ctx, ST_OWNED_LABELED_TRANSFER, depth, {roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings,
+                                                                     in_amounts, in_siblings, in_path_bits, out_owners, out_blindings,
+                                                                     out_amounts, assoc_siblings, assoc_path_bits}, batch, witnesses);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1386,6 +1498,31 @@ int32_t og_groth16_prove_owned_transfer(og_ctx* ctx, const og_pk* pk, const uint
                                         uint32_t batch, const uint8_t* rs, uint8_t* proofs, uint8_t* public_out) {
     return statement_prove(ctx, pk, ST_OWNED_TRANSFER, {roots, tokens, recipients, in_spend_keys, in_blindings, in_amounts, in_siblings,
                                                         in_path_bits, out_owners, out_blindings, out_amounts}, batch, rs, proofs, public_out);
+}
+
+int32_t og_groth16_prove_owned_labeled_transfer_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens,
+                                                    const uint8_t* d_recipients, const uint64_t* d_withdrawn, const uint32_t* d_labels,
+                                                    const uint8_t* d_in_spend_keys, const uint8_t* d_in_blindings, const uint64_t* d_in_amounts,
+                                                    const uint8_t* d_in_siblings, const uint32_t* d_in_path_bits, const uint8_t* d_out_owners,
+                                                    const uint8_t* d_out_blindings, const uint64_t* d_out_amounts,
+                                                    const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
+                                                    const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    return statement_prove_dev(ctx, pk, ST_OWNED_LABELED_TRANSFER, {d_roots, d_tokens, d_recipients, d_withdrawn, d_labels, d_in_spend_keys,
+                                                                    d_in_blindings, d_in_amounts, d_in_siblings, d_in_path_bits, d_out_owners,
+                                                                    d_out_blindings, d_out_amounts, d_assoc_siblings, d_assoc_path_bits},
+                               batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_owned_labeled_transfer(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens,
+                                                const uint8_t* recipients, const uint64_t* withdrawn, const uint32_t* labels,
+                                                const uint8_t* in_spend_keys, const uint8_t* in_blindings, const uint64_t* in_amounts,
+                                                const uint8_t* in_siblings, const uint32_t* in_path_bits, const uint8_t* out_owners,
+                                                const uint8_t* out_blindings, const uint64_t* out_amounts, const uint8_t* assoc_siblings,
+                                                const uint32_t* assoc_path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
+                                                uint8_t* public_out) {
+    return statement_prove(ctx, pk, ST_OWNED_LABELED_TRANSFER, {roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings,
+                                                                in_amounts, in_siblings, in_path_bits, out_owners, out_blindings, out_amounts,
+                                                                assoc_siblings, assoc_path_bits}, batch, rs, proofs, public_out);
 }
 
 int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {

@@ -596,6 +596,114 @@ __global__ void __launch_bounds__(128) k_owned_transfer_witness(OwnedTransferLay
     }
 }
 
+// Owned labeled notes (oracle/owned_labeled_circuit.py), one thread per item: the precommitment MultiMiMC7([P, blinding], 6)
+// for wallets and the leaf MultiMiMC7([pre, token, amount, label], 7) for nodes
+__global__ void __launch_bounds__(64) k_owned_labeled_precommitments(const uint8_t* __restrict__ owners, const uint8_t* __restrict__ blindings,
+                                                                     uint64_t n, uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[2] = {load_canonical<Fr>(owners + 32 * i, flag), load_canonical<Fr>(blindings + 32 * i, flag)};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_LABELED_PRE_KEY), nullptr, 0));
+}
+
+__global__ void __launch_bounds__(64) k_owned_labeled_leaves(const uint8_t* __restrict__ pre, const uint8_t* __restrict__ tokens,
+                                                             const uint64_t* __restrict__ amounts, const uint32_t* __restrict__ labels,
+                                                             uint64_t n, uint8_t* __restrict__ out, int* flag) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fr xs[4] = {load_canonical<Fr>(pre + 32 * i, flag), load_canonical<Fr>(tokens + 32 * i, flag), fr_from_u64(amounts[i]),
+                      Fr::from_u32(labels[i])};
+    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_LABELED_LEAF_KEY), nullptr, 0));
+}
+
+// An owned labeled note block's first variable (an input's spend key, an output's owner), blinding, amount (< 2^64), its 64
+// bits, and the precommitment and the leaf with every round value, their rounds from v + n + L.pre and v + n + L.leaf.
+// Returns the leaf.
+__device__ __forceinline__ Fr owned_labeled_note(const OwnedLabeledTransferLayout& L, Fr* v, uint32_t n, const Fr& first, const Fr& owner,
+                                                 const Fr& bl, const Fr& token, uint64_t amount, const Fr& label) {
+    const Fr one = Fr::one(), zero = Fr::zero();
+    const Fr am = fr_from_u64(amount);
+    v[0] = first; v[1] = bl; v[2] = am;
+#pragma unroll 8
+    for (uint32_t k = 0; k < LABELED_AMOUNT_BITS; k++) v[3 + k] = ((amount >> k) & 1) ? one : zero;
+    const Fr pre_in[2] = {owner, bl};
+    const Fr pre = mimc7_multi_hash<true>(pre_in, Fr::from_u32(OWNED_LABELED_PRE_KEY), v + n + L.pre, L.perm);
+    v[n + L.pre_out] = pre;
+    const Fr leaf_in[4] = {pre, token, am, label};
+    const Fr leaf = mimc7_multi_hash<true>(leaf_in, Fr::from_u32(OWNED_LABELED_LEAF_KEY), v + n + L.leaf, L.perm);
+    v[n + L.leaf_out] = leaf;
+    return leaf;
+}
+
+// Witness of the owned labeled transfer statement, layout of DESIGN.md section 3 (== oracle/owned_labeled_circuit.py); row p
+// starts at W + p * w_stride, Montgomery form.  The owned transfer kernel's split plus a fifth warp for the association path:
+// a CTA covers 32 proofs with five warps, one per independent hash chain of a proof, so no warp diverges and a proof's
+// critical path is one input's owner, precommitment, leaf and pool path (7 + 2 * depth permutations):
+//   warps 0, 1   input i: the owner with its round values, amount bits, precommitment, leaf, the depth pool levels
+//   warps 2, 3   input j - 2's owner, precommitment and leaf again in registers (no stores), its nullifier with its round
+//                values, then output j - 2: amount bits, precommitment, leaf (16 permutations)
+//   warp 4       the scalars, the label and withdrawn bits, assoc_leaf = label + 1 and the association path (2 * depth)
+// After the barrier, warp 0 writes nf_diff_inv.  Only the low `depth` bits of a path word count, in the levels and in the
+// nullifier's index alike.
+__global__ void __launch_bounds__(160) k_owned_labeled_transfer_witness(OwnedLabeledTransferLayout L, uint32_t w_stride,
+                                                                        OwnedLabeledTransferInputs in, uint32_t batch, Fr* __restrict__ W,
+                                                                        int* flag) {
+    const uint32_t role = threadIdx.x >> 5;
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    const bool active = p < batch;
+    Fr* w = W + (uint64_t)p * w_stride;
+    if (active) {
+        const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+        const uint32_t label = in.labels[p];
+        const Fr la = Fr::from_u32(label);
+        if (role < 4) {
+            const Fr k3 = Fr::from_u32(OWNED_OWNER_KEY);
+            const uint32_t i = role & 1;
+            Fr* v = w + L.inp(i);
+            const Fr s = load_canonical<Fr>(in.in_keys + 64ull * p + 32 * i, flag);
+            const Fr bl = load_canonical<Fr>(in.in_blindings + 64ull * p + 32 * i, flag);
+            const uint64_t amount = in.in_amounts[2ull * p + i];
+            const uint32_t bits = in.in_bits[2ull * p + i];
+            const Fr s1[1] = {s};
+            if (role < 2) {
+                const Fr owner = mimc7_multi_hash<true>(s1, k3, v + L.owner_perm, L.perm);
+                const Fr leaf = owned_labeled_note(L, v, L.perm, s, owner, bl, token, amount, la);
+                witness_path(leaf, v + L.lvl_base, L.depth, L.lvl_size, L.perm, in.in_sib + 32ull * L.depth * (2ull * p + i), bits, flag);
+            } else {
+                const Fr owner = mimc7_multi_hash<false>(s1, k3, nullptr, 0);
+                const Fr pre_in[2] = {owner, bl};
+                const Fr pre = mimc7_multi_hash<false>(pre_in, Fr::from_u32(OWNED_LABELED_PRE_KEY), nullptr, 0);
+                const Fr leaf_in[4] = {pre, token, fr_from_u64(amount), la};
+                const Fr leaf = mimc7_multi_hash<false>(leaf_in, Fr::from_u32(OWNED_LABELED_LEAF_KEY), nullptr, 0);
+                const uint32_t mask = L.depth >= 32 ? 0xffffffffu : (1u << L.depth) - 1;
+                const Fr nf_in[3] = {s, leaf, Fr::from_u32(bits & mask)};
+                w[6 + i] = mimc7_multi_hash<true>(nf_in, Fr::from_u32(OWNED_NULLIFIER_KEY), v + L.nf_perm, L.perm);
+                Fr* o = w + L.out(i);
+                const Fr oo = load_canonical<Fr>(in.out_owners + 64ull * p + 32 * i, flag);
+                const Fr ob = load_canonical<Fr>(in.out_blindings + 64ull * p + 32 * i, flag);
+                w[8 + i] = owned_labeled_note(L, o, 0, oo, oo, ob, token, in.out_amounts[2ull * p + i], la);
+            }
+        } else {
+            const Fr one = Fr::one();
+            const Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+            const uint64_t wd = in.withdrawn[p];
+            w[0] = one;
+            w[1] = load_canonical<Fr>(in.roots + 32ull * p, flag);
+            w[3] = token; w[4] = fr_from_u64(wd); w[5] = re;
+            w[10] = re.sqr();
+            w[12] = la;
+            store_range_bits(w + L.label_bits, label, LABELED_LABEL_BITS);
+            store_range_bits(w + L.withdrawn_bits, wd, LABELED_AMOUNT_BITS);
+            const Fr aleaf = fr_from_u64((uint64_t)label + 1);
+            w[13] = aleaf;
+            w[2] = witness_path(aleaf, w + L.assoc_base, L.depth, L.lvl_size, L.perm, in.assoc_sib + 32ull * L.depth * p,
+                                in.assoc_bits[p], flag);
+        }
+    }
+    __syncthreads();   // warps 2 and 3 wrote the nullifiers read below
+    if (active && role == 0) w[11] = (w[6] - w[7]).inv();   // inv(0) = 0: two inputs with one nullifier leave the row unsatisfiable
+}
+
 // ---- host side ------------------------------------------------------------------------------------
 void mimc_constants_host(Fr* out91) { mimc7_round_constants(out91); }
 
@@ -660,6 +768,19 @@ int32_t owned_nullifiers_dev(og_ctx* ctx, const uint8_t* d_keys, const uint8_t* 
                              uint8_t* d_out) {
     if (n == 0) return OG_OK;
     OG_LAUNCH(ctx, k_owned_nullifiers, (unsigned)((n + 63) / 64), 64, 0, d_keys, d_commitments, d_indices, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t owned_labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_owned_labeled_precommitments, (unsigned)((n + 63) / 64), 64, 0, d_owners, d_blindings, n, d_out, ctx->d_flag);
+    return OG_OK;
+}
+
+int32_t owned_labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts,
+                                 const uint32_t* d_labels, uint64_t n, uint8_t* d_out) {
+    if (n == 0) return OG_OK;
+    OG_LAUNCH(ctx, k_owned_labeled_leaves, (unsigned)((n + 63) / 64), 64, 0, d_pre, d_tokens, d_amounts, d_labels, n, d_out, ctx->d_flag);
     return OG_OK;
 }
 
@@ -739,6 +860,13 @@ int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t
         const OwnedTransferInputs t{a[0], a[1], a[2], a[3], a[4], (const uint64_t*)a[5], a[6], (const uint32_t*)a[7], a[8], a[9],
                                     (const uint64_t*)a[10]};
         OG_LAUNCH(ctx, k_owned_transfer_witness, grid, 128, 0, OwnedTransferLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
+        break;
+    }
+    case ST_OWNED_LABELED_TRANSFER: {
+        const OwnedLabeledTransferInputs t{a[0], a[1], a[2], (const uint64_t*)a[3], (const uint32_t*)a[4], a[5], a[6], (const uint64_t*)a[7],
+                                           a[8], (const uint32_t*)a[9], a[10], a[11], (const uint64_t*)a[12], a[13], (const uint32_t*)a[14]};
+        OG_LAUNCH(ctx, k_owned_labeled_transfer_witness, grid, 160, 0, OwnedLabeledTransferLayout::make(depth), w_stride, t, batch, d_W,
+                  ctx->d_flag);
         break;
     }
     }

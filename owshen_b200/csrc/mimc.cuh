@@ -1,8 +1,9 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw and owned transfer statements
-// (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout, oracle/deposit_circuit.py: Layout,
-// oracle/transfer_circuit.py: Layout, oracle/association_circuit.py: Layout, oracle/exclusion_circuit.py: Layout,
-// oracle/labeled_circuit.py: Layout, oracle/labeled_association_circuit.py: Layout and oracle/owned_circuit.py: Layout).
+// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw, owned transfer and owned
+// labeled transfer statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
+// oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout, oracle/association_circuit.py: Layout,
+// oracle/exclusion_circuit.py: Layout, oracle/labeled_circuit.py: Layout, oracle/labeled_association_circuit.py: Layout,
+// oracle/owned_circuit.py: Layout and oracle/owned_labeled_circuit.py: Layout).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -323,12 +324,71 @@ struct OwnedTransferInputs {
     const uint64_t* out_amounts;
 };
 
+constexpr uint32_t OWNED_LABELED_TRANSFER_N_PUB = 9;
+// MultiMiMC7 keys of owned labeled notes: precommitment MultiMiMC7([P, blinding], 6), leaf MultiMiMC7([pre, token, amount,
+// label], 7); the spend public key and the nullifier are the owned notes' (keys 3 and 5)
+constexpr uint32_t OWNED_LABELED_PRE_KEY = 6, OWNED_LABELED_LEAF_KEY = 7;
+
+// 0 ONE | 1 root | 2 association_root | 3 token | 4 withdrawn | 5 recipient | 6, 7 nf[2] | 8, 9 out_cm[2] | 10 recipient_sq
+// | 11 nf_diff_inv | 12 label | 13 assoc_leaf | 14.. label bits (32) | 46.. withdrawn bits (64) | input blocks 0, 1 | output
+// blocks 0, 1 | depth association levels (oracle/owned_labeled_circuit.py).  An input block starts with spend_key, blinding,
+// amount and the 64 amount bits, then the owner permutation, the precommitment, the leaf, the depth pool levels and the
+// nullifier's three permutations; an output block is owner, blinding, amount, its bits, the precommitment and the leaf.
+// Note offsets below are relative to the block; an input's precommitment and leaf sit P later than an output's.
+struct OwnedLabeledTransferLayout {
+    uint32_t depth, perm;
+    uint32_t label_bits, withdrawn_bits;
+    uint32_t in_base, in_size, out_base, out_size, assoc_base, lvl_size;
+    uint32_t owner_perm, lvl_base, nf_perm;          // input block
+    uint32_t pre, pre_out, leaf, leaf_out;           // output block; + perm in an input block
+    uint32_t n_vars, n_constraints;
+    static OwnedLabeledTransferLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        OwnedLabeledTransferLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        const uint32_t P = L.perm;
+        L.lvl_size = 2 * P + 4;
+        L.label_bits = 14;
+        L.withdrawn_bits = L.label_bits + LABELED_LABEL_BITS;
+        L.pre = 67; L.pre_out = 67 + 2 * P; L.leaf = 68 + 2 * P; L.leaf_out = 68 + 6 * P;
+        L.owner_perm = 67; L.lvl_base = 69 + 7 * P;
+        L.nf_perm = L.lvl_base + depth * L.lvl_size;
+        L.in_base = L.withdrawn_bits + LABELED_AMOUNT_BITS;
+        L.in_size = 69 + 10 * P + depth * L.lvl_size;
+        L.out_size = 69 + 6 * P;
+        L.out_base = L.in_base + 2 * L.in_size;
+        L.assoc_base = L.out_base + 2 * L.out_size;
+        L.n_vars = L.assoc_base + depth * L.lvl_size;
+        L.n_constraints = 377 + 32 * P + depth * (6 * P + 9);
+        return L;
+    }
+    OG_HD uint32_t inp(uint32_t i) const { return in_base + i * in_size; }
+    OG_HD uint32_t out(uint32_t j) const { return out_base + j * out_size; }
+};
+
+// the caller's inputs of a batch of owned labeled transfers (k_owned_labeled_transfer_witness's argument), in C ABI order;
+// per proof: root, token, recipient (32 B each), withdrawn (u64), label (u32), then OwnedTransferInputs' input and output
+// arrays, then depth association-tree siblings and a path-bits word
+struct OwnedLabeledTransferInputs {
+    const uint8_t *roots, *tokens, *recipients;
+    const uint64_t* withdrawn;
+    const uint32_t* labels;
+    const uint8_t *in_keys, *in_blindings;
+    const uint64_t* in_amounts;
+    const uint8_t* in_sib;
+    const uint32_t* in_bits;
+    const uint8_t *out_owners, *out_blindings;
+    const uint64_t* out_amounts;
+    const uint8_t* assoc_sib;
+    const uint32_t* assoc_bits;
+};
+
 // ---- the statement table ------------------------------------------------------------------------------------------------
 // What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
 // statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
 // statement_witness_dev) and its og_* forwarders (capi.cu).
 enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED, ST_LABELED_ASSOCIATION,
-                            ST_OWNED_TRANSFER };
+                            ST_OWNED_TRANSFER, ST_OWNED_LABELED_TRANSFER };
 constexpr uint32_t STATEMENT_MAX_INPUTS = 15;
 
 struct StatementShape { uint32_t n_vars, n_constraints; };
@@ -369,6 +429,10 @@ constexpr StatementDesc STATEMENTS[] = {
     // out_blindings, out_amounts
     {OWNED_TRANSFER_N_PUB, layout_shape<OwnedTransferLayout>, true, 11, {32, 32, 32, 64, 64, 16, 0, 8, 64, 64, 16},
      {0, 0, 0, 0, 0, 0, 64, 0, 0, 0, 0}},
+    // owned_labeled_transfer: roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings, in_amounts,
+    // in_siblings, in_path_bits, out_owners, out_blindings, out_amounts, assoc_siblings, assoc_path_bits
+    {OWNED_LABELED_TRANSFER_N_PUB, layout_shape<OwnedLabeledTransferLayout>, true, 15,
+     {32, 32, 32, 8, 4, 64, 64, 16, 0, 8, 64, 64, 16, 0, 4}, {0, 0, 0, 0, 0, 0, 0, 0, 64, 0, 0, 0, 0, 32, 0}},
 };
 
 // the input arrays of a batch in the statement's C ABI order (host or device pointers)
@@ -401,6 +465,11 @@ int32_t owned_commitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_
                               const uint64_t* d_amounts, uint64_t n, uint8_t* d_out);
 int32_t owned_nullifiers_dev(og_ctx* ctx, const uint8_t* d_keys, const uint8_t* d_commitments, const uint32_t* d_indices, uint64_t n,
                              uint8_t* d_out);
+// owned labeled notes (oracle/owned_labeled_circuit.py): MultiMiMC7([P, blinding], 6) and MultiMiMC7([pre, token, amount,
+// label], 7)
+int32_t owned_labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, uint64_t n, uint8_t* d_out);
+int32_t owned_labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts,
+                                 const uint32_t* d_labels, uint64_t n, uint8_t* d_out);
 int32_t mimc_to_mont_dev(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Fr* d_out);
 int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_out);
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves);
@@ -427,12 +496,16 @@ struct NoteEncryptInputs {
 };
 int32_t note_check_view_keys(og_ctx* ctx, const uint8_t* h_keys, uint32_t n);
 int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uint8_t* d_pk_x, uint8_t* d_pk_odd);
-// owned = false: transfer notes, commitment key 0.  owned = true: spend-key notes (the nullifier and secret fields carry the
-// owner P and the blinding), commitment key 4, and a scan's d_spend_keys holds one spend public key P_k per view key (canonical
-// limbs): a record is owned by key k only if its m0 is P_k as well.
+// The note kinds: NOTE_TRANSFER, commitment key 0.  NOTE_OWNED: spend-key notes (the nullifier and secret fields carry the
+// owner P and the blinding), commitment key 4.  NOTE_OWNED_LABELED: owned labeled notes, the owned notes' fields with word 3 =
+// amount + 2^64 label (d_labels: one u32 per note, read by this kind only) and the key-7 leaf as commitment (note_core.cuh:
+// NOTE_LABELED_KEY).  For the last two a scan's d_spend_keys holds one spend public key P_k per view key (canonical limbs): a
+// record is owned by key k only if its m0 is P_k as well.
+enum NoteKind : uint32_t { NOTE_TRANSFER, NOTE_OWNED, NOTE_OWNED_LABELED };
+OG_HD constexpr uint32_t note_kind_key(NoteKind k) { return k == NOTE_TRANSFER ? 0 : k == NOTE_OWNED ? OWNED_COMMITMENT_KEY : OWNED_LABELED_LEAF_KEY; }
 int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status,
-                         bool owned = false);
+                         NoteKind kind = NOTE_TRANSFER, const uint32_t* d_labels = nullptr);
 int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
-                      uint32_t* d_owner, uint8_t* d_plaintexts, const uint32_t* d_spend_keys = nullptr);
+                      uint32_t* d_owner, uint8_t* d_plaintexts, NoteKind kind = NOTE_TRANSFER, const uint32_t* d_spend_keys = nullptr);
 
 }  // namespace og

@@ -34,10 +34,30 @@ OG_HD void note_pads(Fr pad[4], const Fr& sx, const Fr& sy, CFn c) {
     for (uint32_t i = 0; i < 4; i++) pad[i] = mimc7_perm_lazy<false>(Fr::from_u32(i), k, c);
 }
 
+// KEY 7 names the owned labeled note (oracle/owned_labeled_circuit.py): its words are (owner, blinding, token, amount + 2^64
+// label), word 3 may reach 2^96, and its commitment is the leaf MultiMiMC7([MultiMiMC7([owner, blinding], 6), token, amount,
+// label], 7)
+constexpr uint32_t NOTE_LABELED_KEY = 7;
+
+template <class CFn>
+OG_HD Fr note_labeled_leaf(const Fr m[4], CFn c) {
+    const Fr k6 = Fr::from_u32(6), k7 = Fr::from_u32(NOTE_LABELED_KEY);
+    Fr pre = k6 + m[0] + mimc7_perm_lazy<false>(m[0], k6, c);
+    pre = pre + m[1] + mimc7_perm_lazy<false>(m[1], pre, c);
+    uint32_t a[8], lo[8] = {0, 0, 0, 0, 0, 0, 0, 0}, hi[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    m[3].to_canonical(a);
+    lo[0] = a[0]; lo[1] = a[1]; hi[0] = a[2];
+    const Fr xs[3] = {m[2], Fr::from_canonical(lo), Fr::from_canonical(hi)};
+    Fr r = k7 + pre + mimc7_perm_lazy<false>(pre, k7, c);
+    for (int i = 0; i < 3; i++) r = r + xs[i] + mimc7_perm_lazy<false>(xs[i], r, c);
+    return r;
+}
+
 // a note's commitment MultiMiMC7(m, KEY): key 0 is the transfer statement's (nullifier, secret, token, amount), key 4 the owned
-// transfer statement's (owner, blinding, token, amount)
+// transfer statement's (owner, blinding, token, amount); NOTE_LABELED_KEY the owned labeled note's leaf
 template <uint32_t KEY = 0, class CFn>
 OG_HD Fr note_commitment(const Fr m[4], CFn c) {
+    if (KEY == NOTE_LABELED_KEY) return note_labeled_leaf(m, c);
     const Fr k = Fr::from_u32(KEY);
     Fr r = KEY == 0 ? m[0] + mimc7_perm_lazy<true>(m[0], k, c) : k + m[0] + mimc7_perm_lazy<false>(m[0], k, c);
     for (int i = 1; i < 4; i++) r = r + m[i] + mimc7_perm_lazy<false>(m[i], r, c);
@@ -125,8 +145,8 @@ OG_HD bool note_decrypt_one(const Fr& epx, const Fr& epy, const uint32_t v[8], c
     for (int i = 0; i < 4; i++) m[i] = Fr::from_canonical(rec + 8 * (i + 1)) - pad[i];
     uint32_t a[8];
     m[3].to_canonical(a);
-    for (int i = 2; i < 8; i++)
-        if (a[i]) return false;                       // amount >= 2^64: not a note (and no need to hash it)
+    for (int i = KEY == NOTE_LABELED_KEY ? 3 : 2; i < 8; i++)
+        if (a[i]) return false;                       // amount >= 2^64 (2^96 for a labeled word): not a note, no need to hash it
     return note_commitment<KEY>(m, c) == Fr::from_canonical(cm);
 }
 

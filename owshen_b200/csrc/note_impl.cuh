@@ -9,8 +9,9 @@
 //                        double-and-add (or the window digits) never diverge.  An owner is recorded with atomicMin, so the
 //                        lowest owning key index wins whatever the scheduling
 //   k_note_finish        one thread per record: zero plaintext, or the note decrypted again under the winning key
-// The encrypt, scan and finish kernels serve transfer notes (commitment key 0) and, with OWNED, spend-key notes (commitment
-// key 4, and a record is owned by key k only if its m0 is the spend public key P_k as well).
+// The encrypt, scan and finish kernels take the note kind: transfer notes (commitment key 0), spend-key notes (commitment key
+// 4) and owned labeled notes (the key-7 leaf, word 3 = amount + 2^64 label); for the last two a record is owned by key k only
+// if its m0 is the spend public key P_k as well.
 #include "note_core.cuh"
 
 namespace og {
@@ -30,20 +31,21 @@ __global__ void __launch_bounds__(64) k_note_public_keys(const Fr* __restrict__ 
     pk_odd[i] = fr_is_odd(y) ? 1 : 0;
 }
 
-template <bool OWNED>
+// labels: one label per note for NOTE_OWNED_LABELED (word 3 = amount + 2^64 label), unread otherwise
+template <NoteKind KIND>
 __global__ void __launch_bounds__(64) k_note_encrypt(const Fr* __restrict__ base_tab, NoteEncryptInputs in, uint64_t n,
                                                      uint8_t* __restrict__ records, uint8_t* __restrict__ commitments,
-                                                     uint8_t* __restrict__ status, int* flag) {
+                                                     uint8_t* __restrict__ status, int* flag, const uint32_t* __restrict__ labels) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint64_t amount = in.amounts[i];
-    uint32_t a[8] = {(uint32_t)amount, (uint32_t)(amount >> 32), 0, 0, 0, 0, 0, 0};
+    uint32_t a[8] = {(uint32_t)amount, (uint32_t)(amount >> 32), KIND == NOTE_OWNED_LABELED ? labels[i] : 0, 0, 0, 0, 0, 0};
     Fr m[4] = {load_canonical<Fr>(in.nullifiers + 32 * i, flag), load_canonical<Fr>(in.secrets + 32 * i, flag),
                load_canonical<Fr>(in.tokens + 32 * i, flag), Fr::from_canonical(a)};
     Fr pk_x = load_canonical<Fr>(in.pk_x + 32 * i, flag), e = load_canonical<Fr>(in.ephemerals + 32 * i, flag), cm;
     uint32_t w[NOTE_RECORD_WORDS];
-    status[i] = note_encrypt_one<OWNED ? OWNED_COMMITMENT_KEY : 0>(pk_x, in.pk_odd[i] != 0, m, e, BjjBase{Fr::zero(), Fr::zero(), base_tab},
-                                                                  NoteC{}, w, &cm);
+    status[i] = note_encrypt_one<note_kind_key(KIND)>(pk_x, in.pk_odd[i] != 0, m, e, BjjBase{Fr::zero(), Fr::zero(), base_tab},
+                                                      NoteC{}, w, &cm);
     uint32_t* out = reinterpret_cast<uint32_t*>(records + 160 * i);
 #pragma unroll
     for (uint32_t k = 0; k < NOTE_RECORD_WORDS; k++) out[k] = w[k];
@@ -62,7 +64,7 @@ __global__ void __launch_bounds__(128) k_note_prepare(const uint8_t* __restrict_
     owner[i] = ok ? NOTE_NOT_OWNED : NOTE_MALFORMED;
 }
 
-template <bool WINDOW, bool OWNED>
+template <bool WINDOW, NoteKind KIND>
 __global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ spend_keys,
                                                   const uint8_t* __restrict__ records, const uint8_t* __restrict__ commitments,
                                                   const Fr* __restrict__ prepared, uint64_t n, uint32_t* owner) {
@@ -73,14 +75,14 @@ __global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ k
 #pragma unroll
     for (int k = 0; k < 8; k++) v[k] = keys[8 * key + k];
     Fr m[4];
-    if (note_decrypt_one<WINDOW, OWNED ? OWNED_COMMITMENT_KEY : 0>(prepared[2 * i], prepared[2 * i + 1], v,
-                                                                   reinterpret_cast<const uint32_t*>(records + 160 * i),
-                                                                   reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m) &&
-        (!OWNED || m[0] == Fr::from_canonical(spend_keys + 8 * key)))
+    if (note_decrypt_one<WINDOW, note_kind_key(KIND)>(prepared[2 * i], prepared[2 * i + 1], v,
+                                                      reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                                      reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m) &&
+        (KIND == NOTE_TRANSFER || m[0] == Fr::from_canonical(spend_keys + 8 * key)))
         atomicMin(owner + i, key);
 }
 
-template <bool OWNED>
+template <NoteKind KIND>
 __global__ void __launch_bounds__(64) k_note_finish(const uint32_t* __restrict__ keys, uint32_t n_keys, const uint8_t* __restrict__ records,
                                                     const uint8_t* __restrict__ commitments, const Fr* __restrict__ prepared, uint64_t n,
                                                     const uint32_t* __restrict__ owner, uint8_t* __restrict__ plaintexts) {
@@ -89,9 +91,9 @@ __global__ void __launch_bounds__(64) k_note_finish(const uint32_t* __restrict__
     const uint32_t o = owner[i];
     Fr m[4] = {Fr::zero(), Fr::zero(), Fr::zero(), Fr::zero()};
     if (o < n_keys)
-        note_decrypt_one<false, OWNED ? OWNED_COMMITMENT_KEY : 0>(prepared[2 * i], prepared[2 * i + 1], keys + 8ull * o,
-                                                                  reinterpret_cast<const uint32_t*>(records + 160 * i),
-                                                                  reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m);
+        note_decrypt_one<false, note_kind_key(KIND)>(prepared[2 * i], prepared[2 * i + 1], keys + 8ull * o,
+                                                     reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                                     reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m);
     for (int k = 0; k < 4; k++) store_canonical(plaintexts + 128 * i + 32 * k, m[k]);
 }
 
@@ -130,43 +132,68 @@ int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uin
 }
 
 int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status,
-                         bool owned) {
+                         NoteKind kind, const uint32_t* d_labels) {
     if (n == 0) return OG_OK;
     const Fr* tab;
     OG_TRY(bjj_table(ctx, &tab));
     const unsigned blocks = (unsigned)((n + 63) / 64);
-    // profile names: the transfer-note kernels keep theirs, the spend-key-note instances are named k_owned_note_*
-    if (owned) OG_LAUNCHN(ctx, "k_owned_note_encrypt", k_note_encrypt<true>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status, ctx->d_flag);
-    else OG_LAUNCHN(ctx, "k_note_encrypt", k_note_encrypt<false>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status, ctx->d_flag);
+    // profile names: the transfer-note kernels keep theirs, the other kinds' instances are named k_owned_note_* and
+    // k_owned_labeled_note_*
+    switch (kind) {
+    case NOTE_TRANSFER:
+        OG_LAUNCHN(ctx, "k_note_encrypt", k_note_encrypt<NOTE_TRANSFER>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status,
+                   ctx->d_flag, d_labels);
+        break;
+    case NOTE_OWNED:
+        OG_LAUNCHN(ctx, "k_owned_note_encrypt", k_note_encrypt<NOTE_OWNED>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status,
+                   ctx->d_flag, d_labels);
+        break;
+    case NOTE_OWNED_LABELED:
+        OG_LAUNCHN(ctx, "k_owned_labeled_note_encrypt", k_note_encrypt<NOTE_OWNED_LABELED>, blocks, 64, 0, tab, in, n, d_records,
+                   d_commitments, d_status, ctx->d_flag, d_labels);
+        break;
+    }
+    return OG_OK;
+}
+
+// the scan and finish kernels of one note kind; names: the profile names of the window scan, the plain scan and finish
+template <NoteKind KIND>
+static int32_t note_scan_launch(og_ctx* ctx, const char* const names[3], bool window, dim3 grid, const uint32_t* d_keys, uint32_t n_keys,
+                                const uint32_t* d_spend_keys, const uint8_t* d_records, const uint8_t* d_commitments, const Fr* prep,
+                                uint64_t n, uint32_t* d_owner, uint8_t* d_plaintexts) {
+    if (n_keys) {
+        const auto kernel = window ? k_note_scan<true, KIND> : k_note_scan<false, KIND>;
+        OG_LAUNCHN(ctx, window ? names[0] : names[1], kernel, grid, 64, 0, d_keys, d_spend_keys, d_records, d_commitments, prep, n, d_owner);
+    }
+    OG_LAUNCHN(ctx, names[2], k_note_finish<KIND>, grid.x, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n, d_owner, d_plaintexts);
     return OG_OK;
 }
 
 // d_keys: n_keys checked view keys (canonical limbs) in device memory, and d_spend_keys their checked spend public keys for
-// spend-key notes or nullptr for transfer notes; the prepared points go to a context slot
+// spend-key and owned labeled notes (unread for transfer notes); the prepared points go to a context slot
 int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
-                      uint32_t* d_owner, uint8_t* d_plaintexts, const uint32_t* d_spend_keys) {
+                      uint32_t* d_owner, uint8_t* d_plaintexts, NoteKind kind, const uint32_t* d_spend_keys) {
     if (n == 0) return OG_OK;
     if (n_keys > 65535) { snprintf(ctx->err, sizeof(ctx->err), "at most 65535 view keys per scan"); return OG_E_INVALID; }
     OG_SLOT(ctx, prep, Fr, S_NOTE_PREP, sizeof(Fr) * 2 * n);
     const unsigned blocks = (unsigned)((n + 63) / 64);
     OG_LAUNCH(ctx, k_note_prepare, (unsigned)((n + 127) / 128), 128, 0, d_records, d_commitments, n, prep, d_owner);
-    if (n_keys) {
-        // the variable-base multiplier: the 4-bit window, or plain double-and-add with OG_NOTE_WINDOW=0 (DESIGN.md section 8:
-        // the window is 15 % faster at 2^20 records x 8 keys on an H100)
-        const char* w = getenv("OG_NOTE_WINDOW");
-        const bool window = !w || atoi(w) != 0;
-        const dim3 grid(blocks, n_keys);
-        const bool owned = d_spend_keys != nullptr;
-        const auto kernel = owned ? (window ? k_note_scan<true, true> : k_note_scan<false, true>)
-                                  : (window ? k_note_scan<true, false> : k_note_scan<false, false>);
-        const char* name = owned ? (window ? "k_owned_note_scan<true>" : "k_owned_note_scan<false>")
-                                 : (window ? "k_note_scan<true>" : "k_note_scan<false>");
-        OG_LAUNCHN(ctx, name, kernel, grid, 64, 0, d_keys, d_spend_keys, d_records, d_commitments, prep, n, d_owner);
+    // the variable-base multiplier: the 4-bit window, or plain double-and-add with OG_NOTE_WINDOW=0 (DESIGN.md section 8:
+    // the window is 15 % faster at 2^20 records x 8 keys on an H100)
+    const char* w = getenv("OG_NOTE_WINDOW");
+    const bool window = !w || atoi(w) != 0;
+    const dim3 grid(blocks, n_keys);
+    static const char* const transfer[3] = {"k_note_scan<true>", "k_note_scan<false>", "k_note_finish"};
+    static const char* const owned[3] = {"k_owned_note_scan<true>", "k_owned_note_scan<false>", "k_owned_note_finish"};
+    static const char* const labeled[3] = {"k_owned_labeled_note_scan<true>", "k_owned_labeled_note_scan<false>", "k_owned_labeled_note_finish"};
+    const auto run = [&](auto launch, const char* const names[3]) {
+        return launch(ctx, names, window, grid, d_keys, n_keys, d_spend_keys, d_records, d_commitments, prep, n, d_owner, d_plaintexts);
+    };
+    switch (kind) {
+    case NOTE_TRANSFER: return run(note_scan_launch<NOTE_TRANSFER>, transfer);
+    case NOTE_OWNED: return run(note_scan_launch<NOTE_OWNED>, owned);
+    case NOTE_OWNED_LABELED: return run(note_scan_launch<NOTE_OWNED_LABELED>, labeled);
     }
-    if (d_spend_keys) OG_LAUNCHN(ctx, "k_owned_note_finish", k_note_finish<true>, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n,
-                                 d_owner, d_plaintexts);
-    else OG_LAUNCHN(ctx, "k_note_finish", k_note_finish<false>, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n, d_owner,
-                    d_plaintexts);
     return OG_OK;
 }
 

@@ -48,6 +48,14 @@
 //            amount)
 //   owner = MultiMiMC7([spend_key], 3); note commitment = MultiMiMC7([owner, blinding, token, amount], 4); nullifier =
 //   MultiMiMC7([spend_key, commitment, leaf index], 5); otherwise the transfer statement's rows.
+// owned_labeled_transfer
+//   public : root, association_root, token, withdrawn, recipient, nullifier[2], out_commitment[2]
+//   private: label, two input notes (spend_key, blinding, amount, siblings[depth], bits[depth]), two output notes (owner,
+//            blinding, amount), assoc_siblings[depth], assoc_bits[depth]
+//   owner = MultiMiMC7([spend_key], 3); precommitment = MultiMiMC7([owner, blinding], 6); leaf = MultiMiMC7([pre, token,
+//   amount, label], 7) with one label for all four notes; nullifier = MultiMiMC7([spend_key, leaf, leaf index], 5); label
+//   range-checked to 32 bits, withdrawn and the amounts to 64; in0 + in1 = out0 + out1 + withdrawn; nonzero inputs open
+//   under root; nf[0] != nf[1]; assoc_leaf = label + 1 reaching association_root; recipient^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -427,6 +435,74 @@ struct OwnedTransferBuilder {
     }
 };
 
+struct OwnedLabeledTransferBuilder {
+    static constexpr uint32_t V_ONE = 0, V_ROOT = 1, V_AROOT = 2, V_TOKEN = 3, V_WITHDRAWN = 4, V_RECIP = 5, V_NF = 6, V_OUT_CM = 8,
+                              V_RSQ = 10, V_NF_INV = 11, V_LABEL = 12, V_ALEAF = 13;
+    // the precommitment MultiMiMC7([owner, blinding], 6) and the leaf MultiMiMC7([pre, token, amount, label], 7) of the note
+    // block at `v`, each with its output row; `n` is the block's precommitment offset (an input's sits P after an output's)
+    static void note(Mimc7Builder& b, const OwnedLabeledTransferLayout& L, const LC& owner, uint32_t v, uint32_t n) {
+        const uint32_t P = L.perm, pre = v + n + L.pre, leaf = v + n + L.leaf;
+        LC k6, k7; k6[V_ONE] = Fr::from_u32(OWNED_LABELED_PRE_KEY); k7[V_ONE] = Fr::from_u32(OWNED_LABELED_LEAF_KEY);
+        LC bl = lc_var(v + 1), tok = lc_var(V_TOKEN), am = lc_var(v + 2), la = lc_var(V_LABEL);
+        b.multi_hash({&owner, &bl}, k6, {pre, pre + P}, v + n + L.pre_out);
+        LC vpre = lc_var(v + n + L.pre_out);
+        b.multi_hash({&vpre, &tok, &am, &la}, k7, {leaf, leaf + P, leaf + 2 * P, leaf + 3 * P}, v + n + L.leaf_out);
+    }
+
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        OwnedLabeledTransferLayout L = OwnedLabeledTransferLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = OWNED_LABELED_TRANSFER_N_PUB;
+        const uint32_t P = L.perm;
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        b.range(lc_var(V_LABEL), L.label_bits, LABELED_LABEL_BITS);
+        b.range(lc_var(V_WITHDRAWN), L.withdrawn_bits, LABELED_AMOUNT_BITS);
+        for (uint32_t i = 0; i < 2; i++) {
+            const uint32_t v = L.inp(i);
+            // owner P = MultiMiMC7([s], 3) = 3 + s + hash(s, 3), kept as a linear combination
+            LC s = lc_var(v), k3; k3[V_ONE] = Fr::from_u32(OWNED_OWNER_KEY);
+            LC h = b.perm(s, k3, v + L.owner_perm);
+            LC owner = lc_sum({&k3, &s, &h});
+            note(b, L, owner, v, P);
+            const uint32_t leaf = v + P + L.leaf_out;
+            const uint32_t cur = b.merkle_path(leaf, v + L.lvl_base, L.lvl_size, depth);
+            LC vroot = lc_var(V_ROOT), ncur = lc_neg_var(cur);
+            b.cs.add(lc_sum({&vroot, &ncur}), lc_var(v + 2), LC());
+            b.range(lc_var(v + 2), v + 3, LABELED_AMOUNT_BITS);
+            // nullifier = MultiMiMC7([s, leaf, index], 5), index = sum 2^l bit_l over the path bits, bound to nf[i] directly
+            LC vleaf = lc_var(leaf), index, k5; k5[V_ONE] = Fr::from_u32(OWNED_NULLIFIER_KEY);
+            Fr pow2 = Fr::one();
+            for (uint32_t l = 0; l < depth; l++) {
+                lc_add_term(index, v + L.lvl_base + l * L.lvl_size + 1, pow2);
+                pow2 = pow2 + pow2;
+            }
+            const uint32_t nf = v + L.nf_perm;
+            b.multi_hash({&s, &vleaf, &index}, k5, {nf, nf + P, nf + 2 * P}, V_NF + i);
+        }
+        for (uint32_t j = 0; j < 2; j++) {
+            const uint32_t v = L.out(j);
+            b.range(lc_var(v + 2), v + 3, LABELED_AMOUNT_BITS);
+            note(b, L, lc_var(v), v, 0);
+            LC vout = lc_var(v + L.leaf_out), ncm = lc_neg_var(V_OUT_CM + j);
+            b.cs.add(lc_sum({&vout, &ncm}), lc_var(V_ONE), LC());
+        }
+        // in0 + in1 = out0 + out1 + withdrawn: every term is range-checked below 2^64, so it holds over the integers
+        LC i0 = lc_var(L.inp(0) + 2), i1 = lc_var(L.inp(1) + 2), nwd = lc_neg_var(V_WITHDRAWN);
+        LC o0 = lc_neg_var(L.out(0) + 2), o1 = lc_neg_var(L.out(1) + 2);
+        b.cs.add(lc_sum({&i0, &i1, &o0, &o1, &nwd}), lc_var(V_ONE), LC());
+        LC nf0 = lc_var(V_NF), nf1 = lc_neg_var(V_NF + 1);
+        b.cs.add(lc_sum({&nf0, &nf1}), lc_var(V_NF_INV), lc_var(V_ONE));
+        // assoc_leaf = label + 1, the deposit's leaf in the provider's tree of approved labels
+        LC la = lc_var(V_LABEL), one = lc_var(V_ONE), nleaf = lc_neg_var(V_ALEAF);
+        b.cs.add(lc_sum({&la, &one, &nleaf}), lc_var(V_ONE), LC());
+        const uint32_t assoc_root = b.merkle_path(V_ALEAF, L.assoc_base, L.lvl_size, depth);
+        LC vassoc = lc_var(assoc_root), naroot = lc_neg_var(V_AROOT);
+        b.cs.add(lc_sum({&vassoc, &naroot}), lc_var(V_ONE), LC());
+        return b.cs;
+    }
+};
+
 // the statement's R1CS at `depth` (ignored by deposit)
 inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     switch (s) {
@@ -438,6 +514,7 @@ inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     case ST_LABELED: return LabeledBuilder::build(depth);
     case ST_LABELED_ASSOCIATION: return LabeledAssociationBuilder::build(depth);
     case ST_OWNED_TRANSFER: return OwnedTransferBuilder::build(depth);
+    case ST_OWNED_LABELED_TRANSFER: return OwnedLabeledTransferBuilder::build(depth);
     }
     return R1cs();
 }

@@ -85,6 +85,10 @@ SHIELDED_WITHDRAW_KIND = "shielded-withdraw"
 # outputs (out 0, then out 1; DESIGN.md section 3, "Encrypted notes"):
 #     ["shielded-transfer", proof (256 B), 8 public inputs (32 B LE each), record 0, record 1 (160 B each)]
 SHIELDED_TRANSFER_KIND = "shielded-transfer"
+# A shielded labeled transfer (the owned labeled transfer statement) has a kind of its own and 9 public inputs; its records are
+# the owned labeled notes of its outputs:
+#     ["shielded-labeled-transfer", proof (256 B), 9 public inputs (32 B LE each), record 0, record 1 (160 B each)]
+SHIELDED_LABELED_TRANSFER_KIND = "shielded-labeled-transfer"
 
 
 def rlp_encode(item) -> bytes:
@@ -187,5 +191,28 @@ def shielded_transfer_from_rlp(msg: bytes):
         raise ValueError("Invalid tx!")
     kind, proof, pub, recs = item[0], item[1], item[2:10], item[10:12]
     if kind != SHIELDED_TRANSFER_KIND.encode() or len(proof) != 256 or any(len(x) != 32 for x in pub) or any(len(r) != 160 for r in recs):
+        raise ValueError("Invalid tx!")
+    return proof, b"".join(pub), b"".join(recs)
+
+
+def shielded_labeled_transfer_to_rlp(proof: bytes, public_inputs: bytes, records: bytes) -> bytes:
+    """CustomTxMsg-shaped message for one owned labeled transfer proof: public_inputs = the 9 inputs of
+    og_groth16_prove_owned_labeled_transfer's `public_out` row (288 B), records = the encrypted notes of output 0 and output 1
+    (2 x 160 B, og_owned_labeled_note_encrypt)."""
+    if len(proof) != 256 or len(public_inputs) != 288 or len(records) != 320:
+        raise ValueError("shielded_labeled_transfer_to_rlp: proof must be 256 bytes, public inputs 288, records 320")
+    return rlp_encode([SHIELDED_LABELED_TRANSFER_KIND, proof] + [public_inputs[32 * i:32 * i + 32] for i in range(9)]
+                      + [records[0:160], records[160:320]])
+
+
+def shielded_labeled_transfer_from_rlp(msg: bytes):
+    """-> (proof, public_inputs, records); raises ValueError("Invalid tx!") on anything that is not a well-formed
+    shielded-labeled-transfer message."""
+    item = rlp_decode(msg)
+    if not isinstance(item, list) or len(item) != 13 or any(isinstance(x, list) for x in item):
+        raise ValueError("Invalid tx!")
+    kind, proof, pub, recs = item[0], item[1], item[2:11], item[11:13]
+    if (kind != SHIELDED_LABELED_TRANSFER_KIND.encode() or len(proof) != 256 or any(len(x) != 32 for x in pub)
+            or any(len(r) != 160 for r in recs)):
         raise ValueError("Invalid tx!")
     return proof, b"".join(pub), b"".join(recs)
