@@ -323,18 +323,59 @@ def _depth_arg(stmt, depth):
     return [depth] if _STATEMENTS[stmt][0] else []
 
 
-def _statement_args(stmt, fn, batch, depth, arrays):
-    """Length checks of a batch's input arrays (sequences of ints converted first) -> their pointers in C ABI order."""
+def _batch_args(fn, columns, sizes, arrays):
+    """Length checks of a batch's input arrays (sequences of ints converted first) -> their pointers in C ABI order: array k
+    is columns[k] = (name, ..., conversion of a sequence of ints) and must hold sizes[k] bytes."""
     out = []
-    for (name, per_proof, per_level, conv), buf in zip(_STATEMENTS[stmt][1], arrays):
+    for (name, *_, conv), size, buf in zip(columns, sizes, arrays):
         buf = conv(buf) if conv else buf
-        size = (per_proof + per_level * depth) * batch
         if isinstance(buf, C.Array):        # converted from a sequence
             _need(C.sizeof(buf) == size, f"{fn}: {name}: expected {size // C.sizeof(buf._type_)} values, got {len(buf)}")
         else:
             _need_len(buf, size, f"{fn}: {name}")
         out.append(_ptr(buf))
     return out
+
+
+def _statement_args(stmt, fn, batch, depth, arrays):
+    """_batch_args of statement `stmt`'s input arrays for `batch` proofs at `depth`."""
+    columns = _STATEMENTS[stmt][1]
+    return _batch_args(fn, columns, [(per_proof + per_level * depth) * batch for _, per_proof, per_level, _ in columns], arrays)
+
+
+# The note hashes' boundary, mirroring the note-hash table of csrc/mimc.cuh: hash -> its columns in C ABI order as (name, bytes
+# per item, conversion of a sequence of ints).  The C entry point is og_<hash>, and Context.<hash> wraps it.
+_NOTE_HASHES = {
+    "labeled_precommitments": (("nullifiers", 32, None), ("secrets", 32, None)),
+    "labeled_leaves": (("precommitments", 32, None), ("tokens", 32, None), ("amounts", 8, _u64_array), ("labels", 4, _label_array)),
+    "owned_public_keys": (("spend_keys", 32, None),),
+    "owned_commitments": (("owners", 32, None), ("blindings", 32, None), ("tokens", 32, None), ("amounts", 8, _u64_array)),
+    "owned_nullifiers": (("spend_keys", 32, None), ("commitments", 32, None), ("indices", 4, _label_array)),
+    "owned_labeled_precommitments": (("owners", 32, None), ("blindings", 32, None)),
+    "owned_labeled_leaves": (("precommitments", 32, None), ("tokens", 32, None), ("amounts", 8, _u64_array), ("labels", 4, _label_array)),
+}
+
+
+# The note kinds' encryption inputs in C ABI order, as (name, bytes per note, conversion of a sequence of ints); the C entry
+# points are og_<kind>_encrypt(_dev) and og_<kind>_scan(_dev), the owned kinds' scans taking a spend public key per view key.
+_NOTE_KINDS = {
+    "note": (("pk_x", 32, None), ("pk_is_odd", 1, None), ("nullifiers", 32, None), ("secrets", 32, None), ("tokens", 32, None),
+             ("amounts", 8, _u64_array), ("ephemerals", 32, None)),
+    "owned_note": (("pk_x", 32, None), ("pk_is_odd", 1, None), ("owners", 32, None), ("blindings", 32, None), ("tokens", 32, None),
+                   ("amounts", 8, _u64_array), ("ephemerals", 32, None)),
+    "owned_labeled_note": (("pk_x", 32, None), ("pk_is_odd", 1, None), ("owners", 32, None), ("blindings", 32, None),
+                           ("tokens", 32, None), ("amounts", 8, _u64_array), ("labels", 4, _label_array), ("ephemerals", 32, None)),
+}
+
+
+def _note_keys(fn, view_keys, spend_public_keys):
+    """The key arguments of a scan: the view keys, the spend public keys unless None (transfer notes), and the key count."""
+    if spend_public_keys is None:
+        _need(len(view_keys) % 32 == 0, f"{fn}: view keys must be a multiple of 32 bytes")
+        return [view_keys, len(view_keys) // 32]
+    _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
+          f"{fn}: view keys and spend public keys must be equally long multiples of 32 bytes")
+    return [view_keys, spend_public_keys, len(view_keys) // 32]
 
 
 def fr_bytes(x: int) -> bytes:
@@ -527,6 +568,51 @@ class Context:
         _check(lib().og_bjj_sign_batch(self._h, secret_keys, randomness, messages, n, hash_kind, px, odd, sg, st), self)
         return px.raw, odd.raw[:n], sg.raw, st.raw[:n]
 
+    # ---- encrypted notes: one encryption and one scan for every note kind (_NOTE_KINDS) -----------------------------------
+    def _note_encrypt(self, kind, arrays):
+        """og_<kind>_encrypt of the notes in `arrays` (_NOTE_KINDS[kind] order, one note per pk_is_odd byte), ephemerals drawn
+        with the `secrets` module in [1, l) when None -> (records, commitments, status)."""
+        n = len(arrays[1])
+        if arrays[-1] is None:
+            arrays = (*arrays[:-1], b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n)))
+        columns = _NOTE_KINDS[kind]
+        args = _batch_args(f"{kind}_encrypt", columns, [size * n for _, size, _ in columns], arrays)
+        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
+        _check(getattr(lib(), f"og_{kind}_encrypt")(self._h, *args, n, rec, cm, st), self)
+        return rec.raw, cm.raw, st.raw[:n]
+
+    def _note_encrypt_dev(self, kind, d_arrays, n, d_outs):
+        _check(getattr(lib(), f"og_{kind}_encrypt_dev")(self._h, *[_ptr(x) for x in d_arrays], n, *[_ptr(x) for x in d_outs]), self)
+
+    def _note_scan(self, kind, view_keys, spend_public_keys, records, commitments):
+        """og_<kind>_scan -> (owners, plaintexts); spend_public_keys is None for transfer notes."""
+        fn = f"{kind}_scan"
+        keys = _note_keys(fn, view_keys, spend_public_keys)
+        _need(len(records) % 160 == 0, f"{fn}: records must be a multiple of 160 bytes")
+        n = len(records) // 160
+        _need(len(commitments) == 32 * n, f"{fn}: expected one 32-byte commitment per record")
+        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
+        _check(getattr(lib(), f"og_{fn}")(self._h, *keys, records, commitments, n, owner, plain), self)
+        return list(owner), plain.raw
+
+    def _note_scan_dev(self, kind, view_keys, spend_public_keys, d_args):
+        keys = _note_keys(f"{kind}_scan_dev", view_keys, spend_public_keys)
+        d_records, d_commitments, n, d_owner, d_plaintexts = d_args
+        _check(getattr(lib(), f"og_{kind}_scan_dev")(self._h, *keys, _ptr(d_records), _ptr(d_commitments), n, _ptr(d_owner),
+                                                     _ptr(d_plaintexts)), self)
+
+    # ---- the note hashes: one body for every row of _NOTE_HASHES -----------------------------------------------------
+    def _note_hash(self, h, arrays) -> bytes:
+        """og_<h> of the items in `arrays` (_NOTE_HASHES[h] order, as many items as the first column has 32-byte elements)
+        -> 32 bytes per item."""
+        columns = _NOTE_HASHES[h]
+        _need(_blen(arrays[0]) is not None and _blen(arrays[0]) % 32 == 0, f"{h}: {columns[0][0]} must be a multiple of 32 bytes")
+        n = _blen(arrays[0]) // 32
+        args = _batch_args(h, columns, [size * n for _, size, _ in columns], arrays)
+        out = C.create_string_buffer(32 * n)
+        _check(getattr(lib(), f"og_{h}")(self._h, *args, n, out), self)
+        return out.raw
+
     # ---- encrypted notes (DESIGN.md section 3, "Encrypted notes") ----------------------------------------------------
     def note_public_keys(self, view_keys: bytes):
         """View keys (32 bytes each, canonical, nonzero mod l) -> (pk_x, pk_is_odd): the compressed addresses v BASE."""
@@ -541,194 +627,98 @@ class Context:
         with status 1 = written, 2 = the address does not decompress or has 8 V = O, 3 = the ephemeral is 0 mod l.
         Amounts: a sequence of ints < 2^64 or little-endian u64 bytes.  Ephemerals (32 B each) are drawn with the `secrets`
         module in [1, l) when not given; given ones make every byte reproducible."""
-        n = len(pk_is_odd)
-        if ephemerals is None:
-            ephemerals = b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n))
-        am = _u64_array(amounts)
-        for name, buf in (("pk_x", pk_x), ("nullifiers", nullifiers), ("secrets", secrets), ("tokens", tokens), ("ephemerals", ephemerals)):
-            _need(len(buf) == 32 * n, f"note_encrypt: {name}: expected {32 * n} bytes, got {len(buf)}")
-        _need((C.sizeof(am) if isinstance(am, C.Array) else _blen(am)) == 8 * n, "note_encrypt: expected one amount per note")
-        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
-        _check(lib().og_note_encrypt(self._h, pk_x, pk_is_odd, nullifiers, secrets, tokens, _ptr(am), ephemerals, n, rec, cm, st), self)
-        return rec.raw, cm.raw, st.raw[:n]
+        return self._note_encrypt("note", (pk_x, pk_is_odd, nullifiers, secrets, tokens, amounts, ephemerals))
 
     def note_encrypt_dev(self, d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts, d_ephemerals, n: int,
                          d_out_records, d_out_commitments, d_out_status):
         """og_note_encrypt_dev: device buffers (addresses or tensors), enqueued on the context's stream."""
-        _check(lib().og_note_encrypt_dev(self._h, *[_ptr(x) for x in (d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts,
-                                                                     d_ephemerals)], n,
-                                         *[_ptr(x) for x in (d_out_records, d_out_commitments, d_out_status)]), self)
+        self._note_encrypt_dev("note", (d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts, d_ephemerals), n,
+                               (d_out_records, d_out_commitments, d_out_status))
 
     def note_scan(self, view_keys: bytes, records: bytes, commitments: bytes):
         """Trial-decrypt every record under every view key -> (owners, plaintexts): owners[i] is the lowest index of a key
         that owns record i, NOTE_NOT_OWNED or NOTE_MALFORMED; plaintexts holds 128 bytes per record (nullifier, secret, token,
         amount), zero unless owned."""
-        _need(len(view_keys) % 32 == 0, "note_scan: view keys must be a multiple of 32 bytes")
-        _need(len(records) % 160 == 0, "note_scan: records must be a multiple of 160 bytes")
-        n = len(records) // 160
-        _need(len(commitments) == 32 * n, "note_scan: expected one 32-byte commitment per record")
-        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
-        _check(lib().og_note_scan(self._h, view_keys, len(view_keys) // 32, records, commitments, n, owner, plain), self)
-        return list(owner), plain.raw
+        return self._note_scan("note", view_keys, None, records, commitments)
 
     def note_scan_dev(self, view_keys: bytes, d_records, d_commitments, n: int, d_out_owner, d_out_plaintexts):
         """og_note_scan_dev: view keys on the host, every other buffer on the device, enqueued on the context's stream."""
-        _need(len(view_keys) % 32 == 0, "note_scan_dev: view keys must be a multiple of 32 bytes")
-        _check(lib().og_note_scan_dev(self._h, view_keys, len(view_keys) // 32, _ptr(d_records), _ptr(d_commitments), n,
-                                      _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
+        self._note_scan_dev("note", view_keys, None, (d_records, d_commitments, n, d_out_owner, d_out_plaintexts))
 
     # ---- spend-key notes (DESIGN.md section 3, "Owned transfers") ---------------------------------------------------
     def owned_note_encrypt(self, pk_x: bytes, pk_is_odd: bytes, owners: bytes, blindings: bytes, tokens: bytes, amounts, ephemerals=None):
         """note_encrypt for spend-key notes (owner P, blinding, token, amount): the same records, with commitments
         MultiMiMC7([P, blinding, token, amount], 4) -> (records, commitments, status)."""
-        n = len(pk_is_odd)
-        if ephemerals is None:
-            ephemerals = b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n))
-        am = _u64_array(amounts)
-        for name, buf in (("pk_x", pk_x), ("owners", owners), ("blindings", blindings), ("tokens", tokens), ("ephemerals", ephemerals)):
-            _need(len(buf) == 32 * n, f"owned_note_encrypt: {name}: expected {32 * n} bytes, got {len(buf)}")
-        _need((C.sizeof(am) if isinstance(am, C.Array) else _blen(am)) == 8 * n, "owned_note_encrypt: expected one amount per note")
-        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
-        _check(lib().og_owned_note_encrypt(self._h, pk_x, pk_is_odd, owners, blindings, tokens, _ptr(am), ephemerals, n, rec, cm, st), self)
-        return rec.raw, cm.raw, st.raw[:n]
+        return self._note_encrypt("owned_note", (pk_x, pk_is_odd, owners, blindings, tokens, amounts, ephemerals))
 
     def owned_note_encrypt_dev(self, d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals, n: int,
                                d_out_records, d_out_commitments, d_out_status):
         """og_owned_note_encrypt_dev: device buffers (addresses or tensors), enqueued on the context's stream."""
-        _check(lib().og_owned_note_encrypt_dev(self._h, *[_ptr(x) for x in (d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens,
-                                                                           d_amounts, d_ephemerals)], n,
-                                               *[_ptr(x) for x in (d_out_records, d_out_commitments, d_out_status)]), self)
+        self._note_encrypt_dev("owned_note", (d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals), n,
+                               (d_out_records, d_out_commitments, d_out_status))
 
     def owned_note_scan(self, view_keys: bytes, spend_public_keys: bytes, records: bytes, commitments: bytes):
         """note_scan for spend-key notes: key k is (view_keys[k], spend_public_keys[k]) and owns a record only if the record
         decrypts under the view key to a note whose owner is the spend public key and whose key-4 commitment matches ->
         (owners, plaintexts) as note_scan's, the plaintext words being (owner, blinding, token, amount)."""
-        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
-              "owned_note_scan: view keys and spend public keys must be equally long multiples of 32 bytes")
-        _need(len(records) % 160 == 0, "owned_note_scan: records must be a multiple of 160 bytes")
-        n = len(records) // 160
-        _need(len(commitments) == 32 * n, "owned_note_scan: expected one 32-byte commitment per record")
-        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
-        _check(lib().og_owned_note_scan(self._h, view_keys, spend_public_keys, len(view_keys) // 32, records, commitments, n, owner, plain),
-               self)
-        return list(owner), plain.raw
+        return self._note_scan("owned_note", view_keys, spend_public_keys, records, commitments)
 
     def owned_note_scan_dev(self, view_keys: bytes, spend_public_keys: bytes, d_records, d_commitments, n: int, d_out_owner,
                             d_out_plaintexts):
         """og_owned_note_scan_dev: the keys on the host, every other buffer on the device, enqueued on the context's stream."""
-        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
-              "owned_note_scan_dev: view keys and spend public keys must be equally long multiples of 32 bytes")
-        _check(lib().og_owned_note_scan_dev(self._h, view_keys, spend_public_keys, len(view_keys) // 32, _ptr(d_records),
-                                            _ptr(d_commitments), n, _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
+        self._note_scan_dev("owned_note", view_keys, spend_public_keys, (d_records, d_commitments, n, d_out_owner, d_out_plaintexts))
 
     def owned_public_keys(self, spend_keys: bytes) -> bytes:
         """MultiMiMC7([s], 3) of each spending key (32 bytes each in and out): the owner a sender puts in a note."""
-        _need(len(spend_keys) % 32 == 0, "owned_public_keys: spend keys must be a multiple of 32 bytes")
-        n = len(spend_keys) // 32
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_owned_public_keys(self._h, spend_keys, n, out), self)
-        return out.raw
+        return self._note_hash("owned_public_keys", (spend_keys,))
 
     def owned_commitments(self, owners: bytes, blindings: bytes, tokens: bytes, amounts) -> bytes:
         """MultiMiMC7([owner, blinding, token, amount], 4) of each note: owners, blindings, tokens 32 bytes each, amounts
         uint64 (a little-endian buffer, an array or a sequence of ints)."""
-        _need(len(owners) % 32 == 0 and len(blindings) == len(owners) and len(tokens) == len(owners),
-              "owned_commitments: owners, blindings and tokens must be equally long multiples of 32 bytes")
-        n = len(owners) // 32
-        am = _u64_array(amounts)
-        _need((C.sizeof(am) if isinstance(am, C.Array) else _blen(am)) == 8 * n, "owned_commitments: expected one amount per note")
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_owned_commitments(self._h, owners, blindings, tokens, _ptr(am), n, out), self)
-        return out.raw
+        return self._note_hash("owned_commitments", (owners, blindings, tokens, amounts))
 
     def owned_nullifiers(self, spend_keys: bytes, commitments: bytes, indices) -> bytes:
         """MultiMiMC7([s, commitment, index], 5) of each note at its leaf index (uint32): the nullifier its spend publishes,
         so a wallet sees which of its notes the chain has spent."""
-        _need(len(spend_keys) % 32 == 0 and len(commitments) == len(spend_keys),
-              "owned_nullifiers: spend keys and commitments must be equally long multiples of 32 bytes")
-        n = len(spend_keys) // 32
-        if _blen(indices) is None:
-            indices = [int(x) for x in indices]
-            _need(all(0 <= x < 1 << 32 for x in indices), "owned_nullifiers: leaf indices must be integers in [0, 2^32)")
-        idx = _label_array(indices)
-        _need((C.sizeof(idx) if isinstance(idx, C.Array) else _blen(idx)) == 4 * n, "owned_nullifiers: expected one index per note")
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_owned_nullifiers(self._h, spend_keys, commitments, _ptr(idx), n, out), self)
-        return out.raw
+        return self._note_hash("owned_nullifiers", (spend_keys, commitments, indices))
 
     # ---- owned labeled notes (DESIGN.md section 3, "Owned labeled transfers") ----------------------------------------
     def owned_labeled_precommitments(self, owners: bytes, blindings: bytes) -> bytes:
         """MultiMiMC7([owner, blinding], 6) of each note (32 bytes each in and out): what a depositor sends the node, which
         does not reveal the owner."""
-        _need(len(owners) % 32 == 0 and len(blindings) == len(owners),
-              "owned_labeled_precommitments: owners and blindings must be equally long multiples of 32 bytes")
-        n = len(owners) // 32
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_owned_labeled_precommitments(self._h, owners, blindings, n, out), self)
-        return out.raw
+        return self._note_hash("owned_labeled_precommitments", (owners, blindings))
 
     def owned_labeled_leaves(self, precommitments: bytes, tokens: bytes, amounts, labels) -> bytes:
         """MultiMiMC7([precommitment, token, amount, label], 7) of each note: precommitments and tokens 32 bytes each, amounts
         uint64 and labels uint32 (little-endian buffers, arrays or sequences of ints)."""
-        _need(len(precommitments) % 32 == 0 and len(tokens) == len(precommitments),
-              "owned_labeled_leaves: precommitments and tokens must be equally long multiples of 32 bytes")
-        n = len(precommitments) // 32
-        am, la = _u64_array(amounts), _label_array(labels)
-        for name, buf, size in (("amounts", am, 8), ("labels", la, 4)):
-            _need((C.sizeof(buf) if isinstance(buf, C.Array) else _blen(buf)) == size * n,
-                  f"owned_labeled_leaves: expected one {name[:-1]} per note")
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_owned_labeled_leaves(self._h, precommitments, tokens, _ptr(am), _ptr(la), n, out), self)
-        return out.raw
+        return self._note_hash("owned_labeled_leaves", (precommitments, tokens, amounts, labels))
 
     def owned_labeled_note_encrypt(self, pk_x: bytes, pk_is_odd: bytes, owners: bytes, blindings: bytes, tokens: bytes, amounts,
                                    labels, ephemerals=None):
         """note_encrypt for owned labeled notes (owner P, blinding, token, amount, label): the records of the four words (P,
         blinding, token, amount + 2^64 label), with the notes' key-7 leaves as commitments -> (records, commitments, status)."""
-        n = len(pk_is_odd)
-        if ephemerals is None:
-            ephemerals = b"".join(fr_bytes(_rand.randbelow(NOTE_SUBGROUP_ORDER - 1) + 1) for _ in range(n))
-        am, la = _u64_array(amounts), _label_array(labels)
-        for name, buf in (("pk_x", pk_x), ("owners", owners), ("blindings", blindings), ("tokens", tokens), ("ephemerals", ephemerals)):
-            _need(len(buf) == 32 * n, f"owned_labeled_note_encrypt: {name}: expected {32 * n} bytes, got {len(buf)}")
-        for name, buf, size in (("amounts", am, 8), ("labels", la, 4)):
-            _need((C.sizeof(buf) if isinstance(buf, C.Array) else _blen(buf)) == size * n,
-                  f"owned_labeled_note_encrypt: expected one {name[:-1]} per note")
-        rec, cm, st = C.create_string_buffer(160 * n), C.create_string_buffer(32 * n), C.create_string_buffer(n)
-        _check(lib().og_owned_labeled_note_encrypt(self._h, pk_x, pk_is_odd, owners, blindings, tokens, _ptr(am), _ptr(la), ephemerals, n,
-                                                   rec, cm, st), self)
-        return rec.raw, cm.raw, st.raw[:n]
+        return self._note_encrypt("owned_labeled_note", (pk_x, pk_is_odd, owners, blindings, tokens, amounts, labels, ephemerals))
 
     def owned_labeled_note_encrypt_dev(self, d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_labels, d_ephemerals,
                                        n: int, d_out_records, d_out_commitments, d_out_status):
         """og_owned_labeled_note_encrypt_dev: device buffers (addresses or tensors), enqueued on the context's stream."""
-        _check(lib().og_owned_labeled_note_encrypt_dev(self._h, *[_ptr(x) for x in (d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens,
-                                                                                   d_amounts, d_labels, d_ephemerals)], n,
-                                                       *[_ptr(x) for x in (d_out_records, d_out_commitments, d_out_status)]), self)
+        self._note_encrypt_dev("owned_labeled_note", (d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_labels,
+                                                      d_ephemerals), n, (d_out_records, d_out_commitments, d_out_status))
 
     def owned_labeled_note_scan(self, view_keys: bytes, spend_public_keys: bytes, records: bytes, commitments: bytes):
         """owned_note_scan for owned labeled notes -> (owners, plaintexts, amounts, labels): owners as note_scan's, the
         plaintext words (owner, blinding, token, amount + 2^64 label) as og_owned_labeled_note_scan returns them, and each
         record's amount and label split from word 3 (0 unless owned)."""
-        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
-              "owned_labeled_note_scan: view keys and spend public keys must be equally long multiples of 32 bytes")
-        _need(len(records) % 160 == 0, "owned_labeled_note_scan: records must be a multiple of 160 bytes")
-        n = len(records) // 160
-        _need(len(commitments) == 32 * n, "owned_labeled_note_scan: expected one 32-byte commitment per record")
-        owner, plain = (C.c_uint32 * n)(), C.create_string_buffer(128 * n)
-        _check(lib().og_owned_labeled_note_scan(self._h, view_keys, spend_public_keys, len(view_keys) // 32, records, commitments, n,
-                                                owner, plain), self)
-        words3 = [int.from_bytes(plain.raw[128 * i + 96:128 * i + 128], "little") for i in range(n)]
-        return list(owner), plain.raw, [w & ((1 << 64) - 1) for w in words3], [w >> 64 for w in words3]
+        owner, plain = self._note_scan("owned_labeled_note", view_keys, spend_public_keys, records, commitments)
+        words3 = [int.from_bytes(plain[128 * i + 96:128 * i + 128], "little") for i in range(len(owner))]
+        return owner, plain, [w & ((1 << 64) - 1) for w in words3], [w >> 64 for w in words3]
 
     def owned_labeled_note_scan_dev(self, view_keys: bytes, spend_public_keys: bytes, d_records, d_commitments, n: int, d_out_owner,
                                     d_out_plaintexts):
         """og_owned_labeled_note_scan_dev: the keys on the host, every other buffer on the device, enqueued on the context's
         stream; the plaintexts keep word 3 = amount + 2^64 label."""
-        _need(len(view_keys) % 32 == 0 and len(spend_public_keys) == len(view_keys),
-              "owned_labeled_note_scan_dev: view keys and spend public keys must be equally long multiples of 32 bytes")
-        _check(lib().og_owned_labeled_note_scan_dev(self._h, view_keys, spend_public_keys, len(view_keys) // 32, _ptr(d_records),
-                                                    _ptr(d_commitments), n, _ptr(d_out_owner), _ptr(d_out_plaintexts)), self)
+        self._note_scan_dev("owned_labeled_note", view_keys, spend_public_keys, (d_records, d_commitments, n, d_out_owner,
+                                                                                 d_out_plaintexts))
 
     def msm_g1(self, points: bytes, scalars: bytes) -> bytes:
         _need(len(scalars) % 32 == 0, "msm_g1: scalars must be a multiple of 32 bytes")
@@ -826,25 +816,12 @@ class Context:
     # ---- labeled notes (DESIGN.md section 3, "Labeled withdrawals") --------------------------------------------------
     def labeled_precommitments(self, nullifiers: bytes, secrets: bytes) -> bytes:
         """MultiMiMC7([nullifier, secret], 2) of each note (32 bytes each in and out): what a depositor sends the node."""
-        _need(len(nullifiers) % 32 == 0 and len(secrets) == len(nullifiers),
-              "labeled_precommitments: nullifiers and secrets must be equally long multiples of 32 bytes")
-        n = len(nullifiers) // 32
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_labeled_precommitments(self._h, nullifiers, secrets, n, out), self)
-        return out.raw
+        return self._note_hash("labeled_precommitments", (nullifiers, secrets))
 
     def labeled_leaves(self, precommitments: bytes, tokens: bytes, amounts, labels) -> bytes:
         """MultiMiMC7([precommitment, token, amount, label], 2) of each deposit: precommitments and tokens 32 bytes each,
         amounts uint64 and labels uint32 (little-endian buffers, arrays or sequences of ints)."""
-        _need(len(precommitments) % 32 == 0 and len(tokens) == len(precommitments),
-              "labeled_leaves: precommitments and tokens must be equally long multiples of 32 bytes")
-        n = len(precommitments) // 32
-        am, la = _u64_array(amounts), _label_array(labels)
-        for name, buf, size in (("amounts", am, 8), ("labels", la, 4)):
-            _need((C.sizeof(buf) if isinstance(buf, C.Array) else _blen(buf)) == size * n, f"labeled_leaves: expected one {name[:-1]} per deposit")
-        out = C.create_string_buffer(32 * n)
-        _check(lib().og_labeled_leaves(self._h, precommitments, tokens, _ptr(am), _ptr(la), n, out), self)
-        return out.raw
+        return self._note_hash("labeled_leaves", (precommitments, tokens, amounts, labels))
 
     def labeled_witness(self, depth, tokens, recipients, withdrawn, nullifiers, secrets, amounts, labels, siblings, path_bits,
                         change_nullifiers, change_secrets, excl_low, excl_next, excl_siblings, excl_path_bits) -> bytes:

@@ -654,107 +654,62 @@ int32_t og_note_public_keys(og_ctx* ctx, const uint8_t* view_keys, uint32_t n, u
     return check_flag(ctx);
 }
 
-int32_t og_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
-                            const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals, uint64_t n,
-                            uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
-    OG_ENTER(ctx);
-    if (n && (!d_pk_x || !d_pk_is_odd || !d_nullifiers || !d_secrets || !d_tokens || !d_amounts || !d_ephemerals || !d_out_records ||
-              !d_out_commitments || !d_out_status)) return OG_E_INVALID;
-    return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts, d_ephemerals}, n,
-                            d_out_records, d_out_commitments, d_out_status);
+// One encrypt body and one scan body serve the three note kinds (NoteKind, mimc.cuh); every og_*note_encrypt* / og_*note_scan*
+// entry point packs its arguments and calls one of these.  Owned labeled notes add one label per note to the inputs of an
+// encryption; the owned kinds add one spend public key per view key to a scan's.
+static bool note_encrypt_null(NoteKind kind, const NoteEncryptInputs& in, const uint32_t* labels, const uint8_t* records,
+                              const uint8_t* commitments, const uint8_t* status) {
+    return !in.pk_x || !in.pk_odd || !in.nullifiers || !in.secrets || !in.tokens || !in.amounts || !in.ephemerals ||
+           (kind == NOTE_OWNED_LABELED && !labels) || !records || !commitments || !status;
 }
 
-int32_t og_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* nullifiers, const uint8_t* secrets,
-                        const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
-                        uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
+static int32_t note_encrypt_dev_entry(og_ctx* ctx, NoteKind kind, const NoteEncryptInputs& d_in, const uint32_t* d_labels, uint64_t n,
+                                      uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
     OG_ENTER(ctx);
-    if (n && (!pk_x || !pk_is_odd || !nullifiers || !secrets || !tokens || !amounts || !ephemerals || !out_records || !out_commitments ||
-              !out_status)) return OG_E_INVALID;
+    if (n && note_encrypt_null(kind, d_in, d_labels, d_out_records, d_out_commitments, d_out_status)) return OG_E_INVALID;
+    return note_encrypt_dev(ctx, d_in, n, d_out_records, d_out_commitments, d_out_status, kind, d_labels);
+}
+
+static int32_t note_encrypt_entry(og_ctx* ctx, NoteKind kind, const NoteEncryptInputs& in, const uint32_t* labels, uint64_t n,
+                                  uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
+    OG_ENTER(ctx);
+    if (n && note_encrypt_null(kind, in, labels, out_records, out_commitments, out_status)) return OG_E_INVALID;
     if (n == 0) return OG_OK;
-    // per note: 5 x 32 B inputs, 8 B amount, 1 B parity in; 160 B record, 32 B commitment, 1 B status out (u64s first: aligned)
-    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 362ull * n);
+    // per note: 5 x 32 B inputs, 8 B amount, 1 B parity (and a 4 B label) in; 160 B record, 32 B commitment, 1 B status out
+    // (the u64s first, then the labels: aligned)
+    const bool labeled = kind == NOTE_OWNED_LABELED;
+    const uint64_t lb = labeled ? 4 : 0;
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, (362 + lb) * n);
     uint64_t* da = reinterpret_cast<uint64_t*>(io);
-    uint8_t *dx = io + 8 * n, *dnu = dx + 32 * n, *dse = dnu + 32 * n, *dto = dse + 32 * n, *de = dto + 32 * n;
+    uint32_t* dla = reinterpret_cast<uint32_t*>(io + 8 * n);
+    uint8_t *dx = io + (8 + lb) * n, *dnu = dx + 32 * n, *dse = dnu + 32 * n, *dto = dse + 32 * n, *de = dto + 32 * n;
     uint8_t *drec = de + 32 * n, *dcm = drec + 160 * n, *dodd = dcm + 32 * n, *dst = dodd + n;
     OG_TRY(clear_flag(ctx));
-    H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dnu, nullifiers, 32 * n); H2D(ctx, dse, secrets, 32 * n);
-    H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n);
-    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dnu, dse, dto, da, de}, n, drec, dcm, dst));
+    H2D(ctx, da, in.amounts, 8 * n); H2D(ctx, dx, in.pk_x, 32 * n); H2D(ctx, dnu, in.nullifiers, 32 * n); H2D(ctx, dse, in.secrets, 32 * n);
+    H2D(ctx, dto, in.tokens, 32 * n); H2D(ctx, de, in.ephemerals, 32 * n); H2D(ctx, dodd, in.pk_odd, n);
+    if (labeled) H2D(ctx, dla, labels, 4 * n);
+    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dnu, dse, dto, da, de}, n, drec, dcm, dst, kind, labeled ? dla : nullptr));
     D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
     return check_flag(ctx);
 }
 
-// view keys are host memory in both variants: they are checked here, then staged to the device
-static int32_t note_stage_keys(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint32_t** d_keys) {
+static bool note_scan_null(NoteKind kind, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys, const uint8_t* records,
+                           const uint8_t* commitments, uint64_t n, const uint32_t* owner, const uint8_t* plaintexts) {
+    return (n_keys && (!view_keys || (kind != NOTE_TRANSFER && !spend_public_keys))) || (n && (!records || !commitments || !owner || !plaintexts));
+}
+
+// The keys are host memory in every scan: the view keys are checked (note_check_view_keys), and for the owned kinds so are the
+// spend public keys, one per view key, canonical (OG_E_ENCODING); then both are staged to the device.  *d_spend stays null
+// for transfer notes, which have no owner check.
+static int32_t note_stage_keys(og_ctx* ctx, NoteKind kind, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                               const uint32_t** d_keys, const uint32_t** d_spend) {
     if (n_keys > 65535) { snprintf(ctx->err, sizeof(ctx->err), "at most 65535 view keys per scan"); return OG_E_INVALID; }
     OG_TRY(note_check_view_keys(ctx, view_keys, n_keys));
     OG_SLOT(ctx, dk, uint32_t, S_NOTE_KEYS, 32ull * n_keys);
     if (n_keys) H2D(ctx, dk, view_keys, 32ull * n_keys);
     *d_keys = dk;
-    return OG_OK;
-}
-
-int32_t og_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments,
-                         uint64_t n, uint32_t* d_out_owner, uint8_t* d_out_plaintexts) {
-    OG_ENTER(ctx);
-    if ((n_keys && !view_keys) || (n && (!d_records || !d_commitments || !d_out_owner || !d_out_plaintexts))) return OG_E_INVALID;
-    const uint32_t* dk;
-    OG_TRY(note_stage_keys(ctx, view_keys, n_keys, &dk));
-    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts);
-}
-
-int32_t og_note_scan(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* records, const uint8_t* commitments, uint64_t n,
-                     uint32_t* out_owner, uint8_t* out_plaintexts) {
-    OG_ENTER(ctx);
-    if ((n_keys && !view_keys) || (n && (!records || !commitments || !out_owner || !out_plaintexts))) return OG_E_INVALID;
-    const uint32_t* dk;
-    OG_TRY(note_stage_keys(ctx, view_keys, n_keys, &dk));
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // 160 B record, 32 B commitment in; 4 B owner, 128 B plaintext out
-    uint32_t* downer = reinterpret_cast<uint32_t*>(io);
-    uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
-    H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
-    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl));
-    D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
-    OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return OG_OK;
-}
-
-// ---- spend-key notes: encryption and scanning (note_impl.cuh with commitment key 4 and the owner check) ---------------
-int32_t og_owned_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
-                                  const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals,
-                                  uint64_t n, uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
-    OG_ENTER(ctx);
-    if (n && (!d_pk_x || !d_pk_is_odd || !d_owners || !d_blindings || !d_tokens || !d_amounts || !d_ephemerals || !d_out_records ||
-              !d_out_commitments || !d_out_status)) return OG_E_INVALID;
-    return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals}, n,
-                            d_out_records, d_out_commitments, d_out_status, NOTE_OWNED);
-}
-
-int32_t og_owned_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners, const uint8_t* blindings,
-                              const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
-                              uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
-    OG_ENTER(ctx);
-    if (n && (!pk_x || !pk_is_odd || !owners || !blindings || !tokens || !amounts || !ephemerals || !out_records || !out_commitments ||
-              !out_status)) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    // og_note_encrypt's staging
-    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 362ull * n);
-    uint64_t* da = reinterpret_cast<uint64_t*>(io);
-    uint8_t *dx = io + 8 * n, *dow = dx + 32 * n, *dbl = dow + 32 * n, *dto = dbl + 32 * n, *de = dto + 32 * n;
-    uint8_t *drec = de + 32 * n, *dcm = drec + 160 * n, *dodd = dcm + 32 * n, *dst = dodd + n;
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
-    H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n);
-    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dow, dbl, dto, da, de}, n, drec, dcm, dst, NOTE_OWNED));
-    D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
-    return check_flag(ctx);
-}
-
-// the view keys as og_note_scan stages them, and one spend public key per view key, canonical (OG_E_ENCODING), staged beside
-static int32_t owned_note_stage_keys(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
-                                     const uint32_t** d_keys, const uint32_t** d_spend) {
-    OG_TRY(note_stage_keys(ctx, view_keys, n_keys, d_keys));
+    *d_spend = nullptr;
+    if (kind == NOTE_TRANSFER) return OG_OK;
     for (uint32_t j = 0; j < n_keys; j++) {
         uint32_t v[8];
         memcpy(v, spend_public_keys + 32ull * j, 32);
@@ -769,97 +724,104 @@ static int32_t owned_note_stage_keys(og_ctx* ctx, const uint8_t* view_keys, cons
     return OG_OK;
 }
 
-int32_t og_owned_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
-                               const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
-                               uint8_t* d_out_plaintexts) {
+static int32_t note_scan_dev_entry(og_ctx* ctx, NoteKind kind, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                                   const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
+                                   uint8_t* d_out_plaintexts) {
     OG_ENTER(ctx);
-    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!d_records || !d_commitments || !d_out_owner || !d_out_plaintexts)))
+    if (note_scan_null(kind, view_keys, spend_public_keys, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts))
         return OG_E_INVALID;
     const uint32_t *dk, *ds;
-    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
-    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, NOTE_OWNED, ds);
+    OG_TRY(note_stage_keys(ctx, kind, view_keys, spend_public_keys, n_keys, &dk, &ds));
+    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, kind, ds);
 }
 
-int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys, const uint8_t* records,
-                           const uint8_t* commitments, uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts) {
+static int32_t note_scan_entry(og_ctx* ctx, NoteKind kind, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                               const uint8_t* records, const uint8_t* commitments, uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts) {
     OG_ENTER(ctx);
-    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!records || !commitments || !out_owner || !out_plaintexts)))
-        return OG_E_INVALID;
+    if (note_scan_null(kind, view_keys, spend_public_keys, n_keys, records, commitments, n, out_owner, out_plaintexts)) return OG_E_INVALID;
     const uint32_t *dk, *ds;
-    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
+    OG_TRY(note_stage_keys(ctx, kind, view_keys, spend_public_keys, n_keys, &dk, &ds));
     if (n == 0) return OG_OK;
-    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // og_note_scan's staging
+    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // 160 B record, 32 B commitment in; 4 B owner, 128 B plaintext out
     uint32_t* downer = reinterpret_cast<uint32_t*>(io);
     uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
     H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
-    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, NOTE_OWNED, ds));
+    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, kind, ds));
     D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
     OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return OG_OK;
 }
 
-// ---- owned labeled notes: encryption and scanning (note_impl.cuh, NOTE_OWNED_LABELED) ----------------------------------
+int32_t og_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_nullifiers, const uint8_t* d_secrets,
+                            const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals, uint64_t n,
+                            uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
+    return note_encrypt_dev_entry(ctx, NOTE_TRANSFER, {d_pk_x, d_pk_is_odd, d_nullifiers, d_secrets, d_tokens, d_amounts, d_ephemerals}, nullptr,
+                                  n, d_out_records, d_out_commitments, d_out_status);
+}
+int32_t og_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* nullifiers, const uint8_t* secrets,
+                        const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
+                        uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
+    return note_encrypt_entry(ctx, NOTE_TRANSFER, {pk_x, pk_is_odd, nullifiers, secrets, tokens, amounts, ephemerals}, nullptr, n, out_records,
+                              out_commitments, out_status);
+}
+int32_t og_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments,
+                         uint64_t n, uint32_t* d_out_owner, uint8_t* d_out_plaintexts) {
+    return note_scan_dev_entry(ctx, NOTE_TRANSFER, view_keys, nullptr, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts);
+}
+int32_t og_note_scan(og_ctx* ctx, const uint8_t* view_keys, uint32_t n_keys, const uint8_t* records, const uint8_t* commitments, uint64_t n,
+                     uint32_t* out_owner, uint8_t* out_plaintexts) {
+    return note_scan_entry(ctx, NOTE_TRANSFER, view_keys, nullptr, n_keys, records, commitments, n, out_owner, out_plaintexts);
+}
+
+// ---- spend-key notes: encryption and scanning (NOTE_OWNED: the nullifier and secret fields carry owner and blinding) ---------
+int32_t og_owned_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
+                                  const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint8_t* d_ephemerals,
+                                  uint64_t n, uint8_t* d_out_records, uint8_t* d_out_commitments, uint8_t* d_out_status) {
+    return note_encrypt_dev_entry(ctx, NOTE_OWNED, {d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals}, nullptr, n,
+                                  d_out_records, d_out_commitments, d_out_status);
+}
+int32_t og_owned_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners, const uint8_t* blindings,
+                              const uint8_t* tokens, const uint64_t* amounts, const uint8_t* ephemerals, uint64_t n,
+                              uint8_t* out_records, uint8_t* out_commitments, uint8_t* out_status) {
+    return note_encrypt_entry(ctx, NOTE_OWNED, {pk_x, pk_is_odd, owners, blindings, tokens, amounts, ephemerals}, nullptr, n, out_records,
+                              out_commitments, out_status);
+}
+int32_t og_owned_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
+                               const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
+                               uint8_t* d_out_plaintexts) {
+    return note_scan_dev_entry(ctx, NOTE_OWNED, view_keys, spend_public_keys, n_keys, d_records, d_commitments, n, d_out_owner,
+                               d_out_plaintexts);
+}
+int32_t og_owned_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys, const uint8_t* records,
+                           const uint8_t* commitments, uint64_t n, uint32_t* out_owner, uint8_t* out_plaintexts) {
+    return note_scan_entry(ctx, NOTE_OWNED, view_keys, spend_public_keys, n_keys, records, commitments, n, out_owner, out_plaintexts);
+}
+
+// ---- owned labeled notes: encryption and scanning (NOTE_OWNED_LABELED) --------------------------------------------------
 int32_t og_owned_labeled_note_encrypt_dev(og_ctx* ctx, const uint8_t* d_pk_x, const uint8_t* d_pk_is_odd, const uint8_t* d_owners,
                                           const uint8_t* d_blindings, const uint8_t* d_tokens, const uint64_t* d_amounts,
                                           const uint32_t* d_labels, const uint8_t* d_ephemerals, uint64_t n, uint8_t* d_out_records,
                                           uint8_t* d_out_commitments, uint8_t* d_out_status) {
-    OG_ENTER(ctx);
-    if (n && (!d_pk_x || !d_pk_is_odd || !d_owners || !d_blindings || !d_tokens || !d_amounts || !d_labels || !d_ephemerals ||
-              !d_out_records || !d_out_commitments || !d_out_status)) return OG_E_INVALID;
-    return note_encrypt_dev(ctx, NoteEncryptInputs{d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals}, n,
-                            d_out_records, d_out_commitments, d_out_status, NOTE_OWNED_LABELED, d_labels);
+    return note_encrypt_dev_entry(ctx, NOTE_OWNED_LABELED, {d_pk_x, d_pk_is_odd, d_owners, d_blindings, d_tokens, d_amounts, d_ephemerals},
+                                  d_labels, n, d_out_records, d_out_commitments, d_out_status);
 }
-
 int32_t og_owned_labeled_note_encrypt(og_ctx* ctx, const uint8_t* pk_x, const uint8_t* pk_is_odd, const uint8_t* owners,
                                       const uint8_t* blindings, const uint8_t* tokens, const uint64_t* amounts, const uint32_t* labels,
                                       const uint8_t* ephemerals, uint64_t n, uint8_t* out_records, uint8_t* out_commitments,
                                       uint8_t* out_status) {
-    OG_ENTER(ctx);
-    if (n && (!pk_x || !pk_is_odd || !owners || !blindings || !tokens || !amounts || !labels || !ephemerals || !out_records ||
-              !out_commitments || !out_status)) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    // og_note_encrypt's staging with the labels after the amounts, where they stay 4-byte aligned
-    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 366ull * n);
-    uint64_t* da = reinterpret_cast<uint64_t*>(io);
-    uint32_t* dla = reinterpret_cast<uint32_t*>(io + 8 * n);
-    uint8_t *dx = io + 12 * n, *dow = dx + 32 * n, *dbl = dow + 32 * n, *dto = dbl + 32 * n, *de = dto + 32 * n;
-    uint8_t *drec = de + 32 * n, *dcm = drec + 160 * n, *dodd = dcm + 32 * n, *dst = dodd + n;
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, da, amounts, 8 * n); H2D(ctx, dx, pk_x, 32 * n); H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
-    H2D(ctx, dto, tokens, 32 * n); H2D(ctx, de, ephemerals, 32 * n); H2D(ctx, dodd, pk_is_odd, n); H2D(ctx, dla, labels, 4 * n);
-    OG_TRY(note_encrypt_dev(ctx, NoteEncryptInputs{dx, dodd, dow, dbl, dto, da, de}, n, drec, dcm, dst, NOTE_OWNED_LABELED, dla));
-    D2H(ctx, out_records, drec, 160 * n); D2H(ctx, out_commitments, dcm, 32 * n); D2H(ctx, out_status, dst, n);
-    return check_flag(ctx);
+    return note_encrypt_entry(ctx, NOTE_OWNED_LABELED, {pk_x, pk_is_odd, owners, blindings, tokens, amounts, ephemerals}, labels, n,
+                              out_records, out_commitments, out_status);
 }
-
 int32_t og_owned_labeled_note_scan_dev(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
                                        const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n, uint32_t* d_out_owner,
                                        uint8_t* d_out_plaintexts) {
-    OG_ENTER(ctx);
-    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!d_records || !d_commitments || !d_out_owner || !d_out_plaintexts)))
-        return OG_E_INVALID;
-    const uint32_t *dk, *ds;
-    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
-    return note_scan_dev(ctx, dk, n_keys, d_records, d_commitments, n, d_out_owner, d_out_plaintexts, NOTE_OWNED_LABELED, ds);
+    return note_scan_dev_entry(ctx, NOTE_OWNED_LABELED, view_keys, spend_public_keys, n_keys, d_records, d_commitments, n, d_out_owner,
+                               d_out_plaintexts);
 }
-
 int32_t og_owned_labeled_note_scan(og_ctx* ctx, const uint8_t* view_keys, const uint8_t* spend_public_keys, uint32_t n_keys,
                                    const uint8_t* records, const uint8_t* commitments, uint64_t n, uint32_t* out_owner,
                                    uint8_t* out_plaintexts) {
-    OG_ENTER(ctx);
-    if ((n_keys && (!view_keys || !spend_public_keys)) || (n && (!records || !commitments || !out_owner || !out_plaintexts)))
-        return OG_E_INVALID;
-    const uint32_t *dk, *ds;
-    OG_TRY(owned_note_stage_keys(ctx, view_keys, spend_public_keys, n_keys, &dk, &ds));
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, io, uint8_t, S_IO_NOTE, 324ull * n);          // og_note_scan's staging
-    uint32_t* downer = reinterpret_cast<uint32_t*>(io);
-    uint8_t *drec = io + 4 * n, *dcm = drec + 160 * n, *dpl = dcm + 32 * n;
-    H2D(ctx, drec, records, 160 * n); H2D(ctx, dcm, commitments, 32 * n);
-    OG_TRY(note_scan_dev(ctx, dk, n_keys, drec, dcm, n, downer, dpl, NOTE_OWNED_LABELED, ds));
-    D2H(ctx, out_owner, downer, 4 * n); D2H(ctx, out_plaintexts, dpl, 128 * n);
-    OG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return OG_OK;
+    return note_scan_entry(ctx, NOTE_OWNED_LABELED, view_keys, spend_public_keys, n_keys, records, commitments, n, out_owner, out_plaintexts);
 }
 
 // ---- MSM --------------------------------------------------------------------------------------------------
@@ -1064,6 +1026,32 @@ static int32_t statement_prove_dev(og_ctx* ctx, const og_pk* pk, Statement s, co
     return prove_statement_dev(ctx, pk, s, d_in, batch, d_rs, d_proofs, d_public_out);
 }
 
+// ---- the note hashes (the note-hash table, mimc.cuh) ------------------------------------------------------------------
+// Every og_* note hash packs its columns, in C ABI order, into a StatementInputs and calls this.  Column k is staged in slot
+// S_IO_A + k and the output in the slot after the last column.
+static int32_t note_hash_entry(og_ctx* ctx, NoteHash h, const StatementInputs& cols, uint64_t n, uint8_t* out) {
+    OG_ENTER(ctx);
+    const NoteHashDesc& H = NOTE_HASHES[h];
+    for (uint32_t k = 0; k < H.n_cols; k++) if (!cols.p[k]) return OG_E_INVALID;
+    if (!out) return OG_E_INVALID;
+    if (n == 0) return OG_OK;
+    uint8_t* d[NOTE_HASH_MAX_COLUMNS];
+    for (uint32_t k = 0; k < H.n_cols; k++) {
+        OG_SLOT(ctx, dk, uint8_t, S_IO_A + k, H.cols[k] * n);
+        d[k] = dk;
+    }
+    OG_SLOT(ctx, dout, uint8_t, S_IO_A + H.n_cols, 32 * n);
+    OG_TRY(clear_flag(ctx));
+    StatementInputs dc;
+    for (uint32_t k = 0; k < H.n_cols; k++) {
+        H2D(ctx, d[k], cols.p[k], H.cols[k] * n);
+        dc.p[k] = d[k];
+    }
+    OG_TRY(note_hash_dev(ctx, h, dc, n, dout));
+    D2H(ctx, out, dout, 32 * n);
+    return check_flag(ctx);
+}
+
 // ---- withdraw statement ----------------------------------------------------------------------------------------
 int32_t og_withdraw_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
     return statement_r1cs_info(ST_WITHDRAW, depth, n_constraints, n_vars, n_pub, log_m);
@@ -1134,33 +1122,11 @@ int32_t og_exclusion_witness(og_ctx* ctx, uint32_t depth, const uint8_t* nullifi
 
 // ---- labeled notes and the labeled withdraw statement --------------------------------------------------------------
 int32_t og_labeled_precommitments(og_ctx* ctx, const uint8_t* nullifiers, const uint8_t* secrets, uint64_t n, uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !nullifiers || !secrets || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dn, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, ds, uint8_t, S_IO_B, 32 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_C, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dn, nullifiers, 32 * n); H2D(ctx, ds, secrets, 32 * n);
-    OG_TRY(labeled_precommitments_dev(ctx, dn, ds, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_LABELED_PRECOMMITMENTS, {nullifiers, secrets}, n, out);
 }
 int32_t og_labeled_leaves(og_ctx* ctx, const uint8_t* precommitments, const uint8_t* tokens, const uint64_t* amounts, const uint32_t* labels,
                           uint64_t n, uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !precommitments || !tokens || !amounts || !labels || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dp, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, dt, uint8_t, S_IO_B, 32 * n);
-    OG_SLOT(ctx, da, uint64_t, S_IO_C, 8 * n);
-    OG_SLOT(ctx, dl, uint32_t, S_IO_D, 4 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_E, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dp, precommitments, 32 * n); H2D(ctx, dt, tokens, 32 * n); H2D(ctx, da, amounts, 8 * n); H2D(ctx, dl, labels, 4 * n);
-    OG_TRY(labeled_leaves_dev(ctx, dp, dt, da, dl, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_LABELED_LEAVES, {precommitments, tokens, amounts, labels}, n, out);
 }
 int32_t og_labeled_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
     return statement_r1cs_info(ST_LABELED, depth, n_constraints, n_vars, n_pub, log_m);
@@ -1198,47 +1164,15 @@ int32_t og_labeled_association_witness(og_ctx* ctx, uint32_t depth, const uint8_
 
 // ---- spend-key notes and the owned transfer statement ---------------------------------------------------------------
 int32_t og_owned_public_keys(og_ctx* ctx, const uint8_t* spend_keys, uint64_t n, uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !spend_keys || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dk, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_B, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dk, spend_keys, 32 * n);
-    OG_TRY(owned_public_keys_dev(ctx, dk, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_OWNED_PUBLIC_KEYS, {spend_keys}, n, out);
 }
 int32_t og_owned_commitments(og_ctx* ctx, const uint8_t* owners, const uint8_t* blindings, const uint8_t* tokens, const uint64_t* amounts,
                              uint64_t n, uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !owners || !blindings || !tokens || !amounts || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dow, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, dbl, uint8_t, S_IO_B, 32 * n);
-    OG_SLOT(ctx, dt, uint8_t, S_IO_C, 32 * n);
-    OG_SLOT(ctx, da, uint64_t, S_IO_D, 8 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_E, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n); H2D(ctx, dt, tokens, 32 * n); H2D(ctx, da, amounts, 8 * n);
-    OG_TRY(owned_commitments_dev(ctx, dow, dbl, dt, da, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_OWNED_COMMITMENTS, {owners, blindings, tokens, amounts}, n, out);
 }
 int32_t og_owned_nullifiers(og_ctx* ctx, const uint8_t* spend_keys, const uint8_t* commitments, const uint32_t* indices, uint64_t n,
                             uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !spend_keys || !commitments || !indices || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dk, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, dc, uint8_t, S_IO_B, 32 * n);
-    OG_SLOT(ctx, di, uint32_t, S_IO_C, 4 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_D, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dk, spend_keys, 32 * n); H2D(ctx, dc, commitments, 32 * n); H2D(ctx, di, indices, 4 * n);
-    OG_TRY(owned_nullifiers_dev(ctx, dk, dc, di, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_OWNED_NULLIFIERS, {spend_keys, commitments, indices}, n, out);
 }
 int32_t og_owned_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
     return statement_r1cs_info(ST_OWNED_TRANSFER, depth, n_constraints, n_vars, n_pub, log_m);
@@ -1257,33 +1191,11 @@ int32_t og_owned_transfer_witness(og_ctx* ctx, uint32_t depth, const uint8_t* ro
 
 // ---- owned labeled notes and the owned labeled transfer statement ----------------------------------------------------
 int32_t og_owned_labeled_precommitments(og_ctx* ctx, const uint8_t* owners, const uint8_t* blindings, uint64_t n, uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !owners || !blindings || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dow, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, dbl, uint8_t, S_IO_B, 32 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_C, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dow, owners, 32 * n); H2D(ctx, dbl, blindings, 32 * n);
-    OG_TRY(owned_labeled_precommitments_dev(ctx, dow, dbl, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_OWNED_LABELED_PRECOMMITMENTS, {owners, blindings}, n, out);
 }
 int32_t og_owned_labeled_leaves(og_ctx* ctx, const uint8_t* precommitments, const uint8_t* tokens, const uint64_t* amounts,
                                 const uint32_t* labels, uint64_t n, uint8_t* out) {
-    OG_ENTER(ctx);
-    if (!ctx || !precommitments || !tokens || !amounts || !labels || !out) return OG_E_INVALID;
-    if (n == 0) return OG_OK;
-    OG_SLOT(ctx, dp, uint8_t, S_IO_A, 32 * n);
-    OG_SLOT(ctx, dt, uint8_t, S_IO_B, 32 * n);
-    OG_SLOT(ctx, da, uint64_t, S_IO_C, 8 * n);
-    OG_SLOT(ctx, dl, uint32_t, S_IO_D, 4 * n);
-    OG_SLOT(ctx, dout, uint8_t, S_IO_E, 32 * n);
-    OG_TRY(clear_flag(ctx));
-    H2D(ctx, dp, precommitments, 32 * n); H2D(ctx, dt, tokens, 32 * n); H2D(ctx, da, amounts, 8 * n); H2D(ctx, dl, labels, 4 * n);
-    OG_TRY(owned_labeled_leaves_dev(ctx, dp, dt, da, dl, n, dout));
-    D2H(ctx, out, dout, 32 * n);
-    return check_flag(ctx);
+    return note_hash_entry(ctx, NH_OWNED_LABELED_LEAVES, {precommitments, tokens, amounts, labels}, n, out);
 }
 int32_t og_owned_labeled_transfer_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
     return statement_r1cs_info(ST_OWNED_LABELED_TRANSFER, depth, n_constraints, n_vars, n_pub, log_m);

@@ -1,5 +1,5 @@
 // owshen_b200/csrc/mimc.cu -- MiMC7 (circomlib flavour) on sm_90a: 2-to-1 node hash, batched Merkle
-// paths (BASELINE config 2), level-by-level tree build, the labeled-note and spend-key-note hashes, and the witness generators
+// paths (BASELINE config 2), level-by-level tree build, the note hashes (k_note_hash), and the witness generators
 // of the withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw and owned transfer
 // statements (every t^2, t^4, t^6, t^7 of every round is a circuit variable).
 //
@@ -13,7 +13,9 @@
 #include "host_math.hpp"
 #include "mimc.cuh"
 #include "mimc_core.cuh"
+#include <iterator>
 #include <stdlib.h>
+#include <utility>
 
 namespace og {
 
@@ -366,24 +368,27 @@ __device__ __forceinline__ Fr mimc7_multi_hash(const Fr (&xs)[N], const Fr& key,
     return r;
 }
 
-// Labeled notes (oracle/labeled_circuit.py), one thread per note: precommitment = MultiMiMC7([nullifier, secret], 2) for the
-// wallet, leaf = MultiMiMC7([precommitment, token, amount, label], 2) for the node
-__global__ void __launch_bounds__(64) k_labeled_precommitments(const uint8_t* __restrict__ nullifiers, const uint8_t* __restrict__ secrets,
-                                                               uint64_t n, uint8_t* __restrict__ out, int* flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const Fr xs[2] = {load_canonical<Fr>(nullifiers + 32 * i, flag), load_canonical<Fr>(secrets + 32 * i, flag)};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(LABELED_KEY), nullptr, 0));
+// item i of a note-hash column as a field element
+template <NoteColumn COL>
+__device__ __forceinline__ Fr note_column(const uint8_t* col, uint64_t i, int* flag) {
+    if (COL == COL_FR) return load_canonical<Fr>(col + 32 * i, flag);
+    if (COL == COL_U64) return fr_from_u64(reinterpret_cast<const uint64_t*>(col)[i]);
+    return Fr::from_u32(reinterpret_cast<const uint32_t*>(col)[i]);
 }
 
-__global__ void __launch_bounds__(64) k_labeled_leaves(const uint8_t* __restrict__ pre, const uint8_t* __restrict__ tokens,
-                                                       const uint64_t* __restrict__ amounts, const uint32_t* __restrict__ labels, uint64_t n,
-                                                       uint8_t* __restrict__ out, int* flag) {
+template <NoteHash H, size_t... K>
+__device__ __forceinline__ Fr note_hash_one(const StatementInputs& cols, uint64_t i, int* flag, std::index_sequence<K...>) {
+    const Fr xs[sizeof...(K)] = {note_column<NOTE_HASHES[H].cols[K]>(cols.p[K], i, flag)...};
+    return mimc7_multi_hash<false>(xs, Fr::from_u32(NOTE_HASHES[H].key), nullptr, 0);
+}
+
+// The note hash H (the note-hash table, mimc.cuh), one thread per item; the row's column count and types are template
+// constants, so each instance loads exactly its columns.
+template <NoteHash H>
+__global__ void __launch_bounds__(64) k_note_hash(StatementInputs cols, uint64_t n, uint8_t* __restrict__ out, int* flag) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const Fr xs[4] = {load_canonical<Fr>(pre + 32 * i, flag), load_canonical<Fr>(tokens + 32 * i, flag), fr_from_u64(amounts[i]),
-                      Fr::from_u32(labels[i])};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(LABELED_KEY), nullptr, 0));
+    store_canonical(out + 32 * i, note_hash_one<H>(cols, i, flag, std::make_index_sequence<NOTE_HASHES[H].n_cols>{}));
 }
 
 // The labeled note's part of the labeled and labeled association witnesses, whose layouts and inputs share the names it
@@ -493,34 +498,6 @@ __global__ void __launch_bounds__(96) k_labeled_association_witness(LabeledAssoc
     }
 }
 
-// Spend-key notes (oracle/owned_circuit.py), one thread per item: the spend public key MultiMiMC7([s], 3) and the commitment
-// MultiMiMC7([P, blinding, token, amount], 4) for wallets and nodes, the nullifier MultiMiMC7([s, cm, index], 5) for the wallet
-// that watches its notes being spent
-__global__ void __launch_bounds__(64) k_owned_public_keys(const uint8_t* __restrict__ keys, uint64_t n, uint8_t* __restrict__ out, int* flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const Fr xs[1] = {load_canonical<Fr>(keys + 32 * i, flag)};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_OWNER_KEY), nullptr, 0));
-}
-
-__global__ void __launch_bounds__(64) k_owned_commitments(const uint8_t* __restrict__ owners, const uint8_t* __restrict__ blindings,
-                                                          const uint8_t* __restrict__ tokens, const uint64_t* __restrict__ amounts, uint64_t n,
-                                                          uint8_t* __restrict__ out, int* flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const Fr xs[4] = {load_canonical<Fr>(owners + 32 * i, flag), load_canonical<Fr>(blindings + 32 * i, flag),
-                      load_canonical<Fr>(tokens + 32 * i, flag), fr_from_u64(amounts[i])};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_COMMITMENT_KEY), nullptr, 0));
-}
-
-__global__ void __launch_bounds__(64) k_owned_nullifiers(const uint8_t* __restrict__ keys, const uint8_t* __restrict__ commitments,
-                                                         const uint32_t* __restrict__ indices, uint64_t n, uint8_t* __restrict__ out, int* flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const Fr xs[3] = {load_canonical<Fr>(keys + 32 * i, flag), load_canonical<Fr>(commitments + 32 * i, flag), Fr::from_u32(indices[i])};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_NULLIFIER_KEY), nullptr, 0));
-}
-
 // An owned note block's first variable (an input's spend key, an output's owner), blinding, amount (< 2^64), its 64 bits and
 // the commitment MultiMiMC7([owner, blinding, token, amount], 4) with every round value, written into the block v.  Returns
 // the commitment.
@@ -594,26 +571,6 @@ __global__ void __launch_bounds__(128) k_owned_transfer_witness(OwnedTransferLay
         w[2] = a_out - a_in;
         w[10] = (w[5] - w[6]).inv();   // inv(0) = 0: two inputs with one nullifier leave the row unsatisfiable
     }
-}
-
-// Owned labeled notes (oracle/owned_labeled_circuit.py), one thread per item: the precommitment MultiMiMC7([P, blinding], 6)
-// for wallets and the leaf MultiMiMC7([pre, token, amount, label], 7) for nodes
-__global__ void __launch_bounds__(64) k_owned_labeled_precommitments(const uint8_t* __restrict__ owners, const uint8_t* __restrict__ blindings,
-                                                                     uint64_t n, uint8_t* __restrict__ out, int* flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const Fr xs[2] = {load_canonical<Fr>(owners + 32 * i, flag), load_canonical<Fr>(blindings + 32 * i, flag)};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_LABELED_PRE_KEY), nullptr, 0));
-}
-
-__global__ void __launch_bounds__(64) k_owned_labeled_leaves(const uint8_t* __restrict__ pre, const uint8_t* __restrict__ tokens,
-                                                             const uint64_t* __restrict__ amounts, const uint32_t* __restrict__ labels,
-                                                             uint64_t n, uint8_t* __restrict__ out, int* flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const Fr xs[4] = {load_canonical<Fr>(pre + 32 * i, flag), load_canonical<Fr>(tokens + 32 * i, flag), fr_from_u64(amounts[i]),
-                      Fr::from_u32(labels[i])};
-    store_canonical(out + 32 * i, mimc7_multi_hash<false>(xs, Fr::from_u32(OWNED_LABELED_LEAF_KEY), nullptr, 0));
 }
 
 // An owned labeled note block's first variable (an input's spend key, an output's owner), blinding, amount (< 2^64), its 64
@@ -738,50 +695,22 @@ int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_o
     return OG_OK;
 }
 
-int32_t labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_nullifiers, const uint8_t* d_secrets, uint64_t n, uint8_t* d_out) {
-    if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_labeled_precommitments, (unsigned)((n + 63) / 64), 64, 0, d_nullifiers, d_secrets, n, d_out, ctx->d_flag);
+template <NoteHash H>
+static int32_t note_hash_launch(og_ctx* ctx, const StatementInputs& cols, uint64_t n, uint8_t* d_out) {
+    OG_LAUNCHN(ctx, NOTE_HASHES[H].name, k_note_hash<H>, (unsigned)((n + 63) / 64), 64, 0, cols, n, d_out, ctx->d_flag);
     return OG_OK;
 }
 
-int32_t labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint32_t* d_labels,
-                           uint64_t n, uint8_t* d_out) {
-    if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_labeled_leaves, (unsigned)((n + 63) / 64), 64, 0, d_pre, d_tokens, d_amounts, d_labels, n, d_out, ctx->d_flag);
-    return OG_OK;
+template <size_t... H>
+static int32_t note_hash_dispatch(og_ctx* ctx, NoteHash h, const StatementInputs& cols, uint64_t n, uint8_t* d_out,
+                                  std::index_sequence<H...>) {
+    static constexpr int32_t (*launch[])(og_ctx*, const StatementInputs&, uint64_t, uint8_t*) = {note_hash_launch<NoteHash(H)>...};
+    return launch[h](ctx, cols, n, d_out);
 }
 
-int32_t owned_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint64_t n, uint8_t* d_out) {
+int32_t note_hash_dev(og_ctx* ctx, NoteHash h, const StatementInputs& cols, uint64_t n, uint8_t* d_out) {
     if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_owned_public_keys, (unsigned)((n + 63) / 64), 64, 0, d_keys, n, d_out, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t owned_commitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, const uint8_t* d_tokens,
-                              const uint64_t* d_amounts, uint64_t n, uint8_t* d_out) {
-    if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_owned_commitments, (unsigned)((n + 63) / 64), 64, 0, d_owners, d_blindings, d_tokens, d_amounts, n, d_out, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t owned_nullifiers_dev(og_ctx* ctx, const uint8_t* d_keys, const uint8_t* d_commitments, const uint32_t* d_indices, uint64_t n,
-                             uint8_t* d_out) {
-    if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_owned_nullifiers, (unsigned)((n + 63) / 64), 64, 0, d_keys, d_commitments, d_indices, n, d_out, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t owned_labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, uint64_t n, uint8_t* d_out) {
-    if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_owned_labeled_precommitments, (unsigned)((n + 63) / 64), 64, 0, d_owners, d_blindings, n, d_out, ctx->d_flag);
-    return OG_OK;
-}
-
-int32_t owned_labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts,
-                                 const uint32_t* d_labels, uint64_t n, uint8_t* d_out) {
-    if (n == 0) return OG_OK;
-    OG_LAUNCH(ctx, k_owned_labeled_leaves, (unsigned)((n + 63) / 64), 64, 0, d_pre, d_tokens, d_amounts, d_labels, n, d_out, ctx->d_flag);
-    return OG_OK;
+    return note_hash_dispatch(ctx, h, cols, n, d_out, std::make_index_sequence<std::size(NOTE_HASHES)>{});
 }
 
 // levels: Montgomery-form buffer holding n + n/2 + ... + 1 elements, level 0 already filled

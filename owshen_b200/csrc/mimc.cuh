@@ -451,25 +451,44 @@ struct StatementInputs {
     }
 };
 
+// ---- the note-hash table ------------------------------------------------------------------------------------------------
+// The batch hashes of the note families, one thread per item: MultiMiMC7(columns, key).  What the C ABI and api.py
+// (_NOTE_HASHES, which mirrors this table) know of a note hash.  Besides its row here a hash has its og_* forwarder (capi.cu);
+// mimc.cu's k_note_hash<H> and note_hash_dev serve every row.
+enum NoteHash : uint32_t { NH_LABELED_PRECOMMITMENTS, NH_LABELED_LEAVES, NH_OWNED_PUBLIC_KEYS, NH_OWNED_COMMITMENTS, NH_OWNED_NULLIFIERS,
+                           NH_OWNED_LABELED_PRECOMMITMENTS, NH_OWNED_LABELED_LEAVES };
+// a column's item: a 32-byte canonical field element, or an integer (u64, u32) taken as the field element it is
+enum NoteColumn : uint32_t { COL_FR = 32, COL_U64 = 8, COL_U32 = 4 };   // the value is the item's size in bytes
+constexpr uint32_t NOTE_HASH_MAX_COLUMNS = 4;
+
+struct NoteHashDesc {
+    const char* name;                                   // the kernel's og_profile name
+    uint32_t key;                                       // the MultiMiMC7 key
+    uint32_t n_cols;
+    NoteColumn cols[NOTE_HASH_MAX_COLUMNS];             // the input columns in C ABI order
+};
+
+constexpr NoteHashDesc NOTE_HASHES[] = {
+    // labeled notes (oracle/labeled_circuit.py): precommitment MultiMiMC7([nullifier, secret], 2), leaf MultiMiMC7([pre, token,
+    // amount, label], 2)
+    {"k_labeled_precommitments", LABELED_KEY, 2, {COL_FR, COL_FR}},
+    {"k_labeled_leaves", LABELED_KEY, 4, {COL_FR, COL_FR, COL_U64, COL_U32}},
+    // spend-key notes (oracle/owned_circuit.py): P = MultiMiMC7([s], 3), commitment MultiMiMC7([P, blinding, token, amount], 4),
+    // nullifier MultiMiMC7([s, cm, index], 5)
+    {"k_owned_public_keys", OWNED_OWNER_KEY, 1, {COL_FR}},
+    {"k_owned_commitments", OWNED_COMMITMENT_KEY, 4, {COL_FR, COL_FR, COL_FR, COL_U64}},
+    {"k_owned_nullifiers", OWNED_NULLIFIER_KEY, 3, {COL_FR, COL_FR, COL_U32}},
+    // owned labeled notes (oracle/owned_labeled_circuit.py): precommitment MultiMiMC7([P, blinding], 6), leaf MultiMiMC7([pre,
+    // token, amount, label], 7)
+    {"k_owned_labeled_precommitments", OWNED_LABELED_PRE_KEY, 2, {COL_FR, COL_FR}},
+    {"k_owned_labeled_leaves", OWNED_LABELED_LEAF_KEY, 4, {COL_FR, COL_FR, COL_U64, COL_U32}},
+};
+
 int32_t mimc_hash2_dev(og_ctx* ctx, const uint8_t* d_l, const uint8_t* d_r, uint64_t n, uint8_t* d_out);
 int32_t mimc_merkle_paths_dev(og_ctx* ctx, const uint8_t* d_leaves, const uint8_t* d_siblings, const uint32_t* d_bits,
                               uint32_t n_paths, uint32_t depth, uint8_t* d_out);
-// labeled notes (oracle/labeled_circuit.py): MultiMiMC7([nullifier, secret], 2) and MultiMiMC7([pre, token, amount, label], 2)
-int32_t labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_nullifiers, const uint8_t* d_secrets, uint64_t n, uint8_t* d_out);
-int32_t labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts, const uint32_t* d_labels,
-                           uint64_t n, uint8_t* d_out);
-// spend-key notes (oracle/owned_circuit.py): P = MultiMiMC7([s], 3), cm = MultiMiMC7([P, blinding, token, amount], 4) and
-// nullifier = MultiMiMC7([s, cm, index], 5)
-int32_t owned_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint64_t n, uint8_t* d_out);
-int32_t owned_commitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, const uint8_t* d_tokens,
-                              const uint64_t* d_amounts, uint64_t n, uint8_t* d_out);
-int32_t owned_nullifiers_dev(og_ctx* ctx, const uint8_t* d_keys, const uint8_t* d_commitments, const uint32_t* d_indices, uint64_t n,
-                             uint8_t* d_out);
-// owned labeled notes (oracle/owned_labeled_circuit.py): MultiMiMC7([P, blinding], 6) and MultiMiMC7([pre, token, amount,
-// label], 7)
-int32_t owned_labeled_precommitments_dev(og_ctx* ctx, const uint8_t* d_owners, const uint8_t* d_blindings, uint64_t n, uint8_t* d_out);
-int32_t owned_labeled_leaves_dev(og_ctx* ctx, const uint8_t* d_pre, const uint8_t* d_tokens, const uint64_t* d_amounts,
-                                 const uint32_t* d_labels, uint64_t n, uint8_t* d_out);
+// the note hash h of n items: cols.p[k] holds column k on the device
+int32_t note_hash_dev(og_ctx* ctx, NoteHash h, const StatementInputs& cols, uint64_t n, uint8_t* d_out);
 int32_t mimc_to_mont_dev(og_ctx* ctx, const uint8_t* d_in, uint64_t n, Fr* d_out);
 int32_t mimc_from_mont_dev(og_ctx* ctx, const Fr* d_in, uint64_t n, uint8_t* d_out);
 int32_t mimc_tree_build_dev(og_ctx* ctx, Fr* d_levels, uint64_t n_leaves);
@@ -504,8 +523,8 @@ int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uin
 enum NoteKind : uint32_t { NOTE_TRANSFER, NOTE_OWNED, NOTE_OWNED_LABELED };
 OG_HD constexpr uint32_t note_kind_key(NoteKind k) { return k == NOTE_TRANSFER ? 0 : k == NOTE_OWNED ? OWNED_COMMITMENT_KEY : OWNED_LABELED_LEAF_KEY; }
 int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status,
-                         NoteKind kind = NOTE_TRANSFER, const uint32_t* d_labels = nullptr);
+                         NoteKind kind, const uint32_t* d_labels);
 int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
-                      uint32_t* d_owner, uint8_t* d_plaintexts, NoteKind kind = NOTE_TRANSFER, const uint32_t* d_spend_keys = nullptr);
+                      uint32_t* d_owner, uint8_t* d_plaintexts, NoteKind kind, const uint32_t* d_spend_keys);
 
 }  // namespace og

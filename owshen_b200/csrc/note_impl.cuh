@@ -6,7 +6,7 @@
 //   k_note_prepare       one thread per record: parse, decompress E, E' = 8 E and the malformed checks, once for all keys;
 //                        writes E' (the only scratch) and seeds the owner word with NOT_OWNED or MALFORMED
 //   k_note_scan          one thread per (record, key); blockIdx.y is the key, so a warp shares one scalar and the
-//                        double-and-add (or the window digits) never diverge.  An owner is recorded with atomicMin, so the
+//                        window digits never diverge.  An owner is recorded with atomicMin, so the
 //                        lowest owning key index wins whatever the scheduling
 //   k_note_finish        one thread per record: zero plaintext, or the note decrypted again under the winning key
 // The encrypt, scan and finish kernels take the note kind: transfer notes (commitment key 0), spend-key notes (commitment key
@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(128) k_note_prepare(const uint8_t* __restrict_
     owner[i] = ok ? NOTE_NOT_OWNED : NOTE_MALFORMED;
 }
 
-template <bool WINDOW, NoteKind KIND>
+template <NoteKind KIND>
 __global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ spend_keys,
                                                   const uint8_t* __restrict__ records, const uint8_t* __restrict__ commitments,
                                                   const Fr* __restrict__ prepared, uint64_t n, uint32_t* owner) {
@@ -75,9 +75,9 @@ __global__ void __launch_bounds__(64) k_note_scan(const uint32_t* __restrict__ k
 #pragma unroll
     for (int k = 0; k < 8; k++) v[k] = keys[8 * key + k];
     Fr m[4];
-    if (note_decrypt_one<WINDOW, note_kind_key(KIND)>(prepared[2 * i], prepared[2 * i + 1], v,
-                                                      reinterpret_cast<const uint32_t*>(records + 160 * i),
-                                                      reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m) &&
+    if (note_decrypt_one<true, note_kind_key(KIND)>(prepared[2 * i], prepared[2 * i + 1], v,
+                                                    reinterpret_cast<const uint32_t*>(records + 160 * i),
+                                                    reinterpret_cast<const uint32_t*>(commitments + 32 * i), NoteC{}, m) &&
         (KIND == NOTE_TRANSFER || m[0] == Fr::from_canonical(spend_keys + 8 * key)))
         atomicMin(owner + i, key);
 }
@@ -131,46 +131,42 @@ int32_t note_public_keys_dev(og_ctx* ctx, const uint8_t* d_keys, uint32_t n, uin
     return OG_OK;
 }
 
+// the note kinds' og_profile names: the transfer-note kernels keep theirs, the other kinds' are k_owned_note_* and
+// k_owned_labeled_note_*
+struct NoteKernelNames { const char *encrypt, *scan, *finish; };
+constexpr NoteKernelNames NOTE_KERNEL_NAMES[] = {
+    {"k_note_encrypt", "k_note_scan", "k_note_finish"},
+    {"k_owned_note_encrypt", "k_owned_note_scan", "k_owned_note_finish"},
+    {"k_owned_labeled_note_encrypt", "k_owned_labeled_note_scan", "k_owned_labeled_note_finish"},
+};
+
+// f(std::integral_constant<NoteKind, kind>): the kernels' template argument from the kind a call names
+template <class F>
+static int32_t with_note_kind(NoteKind kind, F&& f) {
+    switch (kind) {
+    case NOTE_TRANSFER: return f(std::integral_constant<NoteKind, NOTE_TRANSFER>{});
+    case NOTE_OWNED: return f(std::integral_constant<NoteKind, NOTE_OWNED>{});
+    case NOTE_OWNED_LABELED: return f(std::integral_constant<NoteKind, NOTE_OWNED_LABELED>{});
+    }
+    return OG_E_INVALID;
+}
+
 int32_t note_encrypt_dev(og_ctx* ctx, const NoteEncryptInputs& in, uint64_t n, uint8_t* d_records, uint8_t* d_commitments, uint8_t* d_status,
                          NoteKind kind, const uint32_t* d_labels) {
     if (n == 0) return OG_OK;
     const Fr* tab;
     OG_TRY(bjj_table(ctx, &tab));
-    const unsigned blocks = (unsigned)((n + 63) / 64);
-    // profile names: the transfer-note kernels keep theirs, the other kinds' instances are named k_owned_note_* and
-    // k_owned_labeled_note_*
-    switch (kind) {
-    case NOTE_TRANSFER:
-        OG_LAUNCHN(ctx, "k_note_encrypt", k_note_encrypt<NOTE_TRANSFER>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status,
-                   ctx->d_flag, d_labels);
-        break;
-    case NOTE_OWNED:
-        OG_LAUNCHN(ctx, "k_owned_note_encrypt", k_note_encrypt<NOTE_OWNED>, blocks, 64, 0, tab, in, n, d_records, d_commitments, d_status,
-                   ctx->d_flag, d_labels);
-        break;
-    case NOTE_OWNED_LABELED:
-        OG_LAUNCHN(ctx, "k_owned_labeled_note_encrypt", k_note_encrypt<NOTE_OWNED_LABELED>, blocks, 64, 0, tab, in, n, d_records,
+    return with_note_kind(kind, [&](auto k) -> int32_t {
+        constexpr NoteKind KIND = decltype(k)::value;
+        OG_LAUNCHN(ctx, NOTE_KERNEL_NAMES[KIND].encrypt, k_note_encrypt<KIND>, (unsigned)((n + 63) / 64), 64, 0, tab, in, n, d_records,
                    d_commitments, d_status, ctx->d_flag, d_labels);
-        break;
-    }
-    return OG_OK;
-}
-
-// the scan and finish kernels of one note kind; names: the profile names of the window scan, the plain scan and finish
-template <NoteKind KIND>
-static int32_t note_scan_launch(og_ctx* ctx, const char* const names[3], bool window, dim3 grid, const uint32_t* d_keys, uint32_t n_keys,
-                                const uint32_t* d_spend_keys, const uint8_t* d_records, const uint8_t* d_commitments, const Fr* prep,
-                                uint64_t n, uint32_t* d_owner, uint8_t* d_plaintexts) {
-    if (n_keys) {
-        const auto kernel = window ? k_note_scan<true, KIND> : k_note_scan<false, KIND>;
-        OG_LAUNCHN(ctx, window ? names[0] : names[1], kernel, grid, 64, 0, d_keys, d_spend_keys, d_records, d_commitments, prep, n, d_owner);
-    }
-    OG_LAUNCHN(ctx, names[2], k_note_finish<KIND>, grid.x, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n, d_owner, d_plaintexts);
-    return OG_OK;
+        return OG_OK;
+    });
 }
 
 // d_keys: n_keys checked view keys (canonical limbs) in device memory, and d_spend_keys their checked spend public keys for
-// spend-key and owned labeled notes (unread for transfer notes); the prepared points go to a context slot
+// spend-key and owned labeled notes (unread for transfer notes); the prepared points go to a context slot.  The
+// variable-base multiplier is the 4-bit window (DESIGN.md section 5.6).
 int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, const uint8_t* d_records, const uint8_t* d_commitments, uint64_t n,
                       uint32_t* d_owner, uint8_t* d_plaintexts, NoteKind kind, const uint32_t* d_spend_keys) {
     if (n == 0) return OG_OK;
@@ -178,23 +174,15 @@ int32_t note_scan_dev(og_ctx* ctx, const uint32_t* d_keys, uint32_t n_keys, cons
     OG_SLOT(ctx, prep, Fr, S_NOTE_PREP, sizeof(Fr) * 2 * n);
     const unsigned blocks = (unsigned)((n + 63) / 64);
     OG_LAUNCH(ctx, k_note_prepare, (unsigned)((n + 127) / 128), 128, 0, d_records, d_commitments, n, prep, d_owner);
-    // the variable-base multiplier: the 4-bit window, or plain double-and-add with OG_NOTE_WINDOW=0 (DESIGN.md section 8:
-    // the window is 15 % faster at 2^20 records x 8 keys on an H100)
-    const char* w = getenv("OG_NOTE_WINDOW");
-    const bool window = !w || atoi(w) != 0;
-    const dim3 grid(blocks, n_keys);
-    static const char* const transfer[3] = {"k_note_scan<true>", "k_note_scan<false>", "k_note_finish"};
-    static const char* const owned[3] = {"k_owned_note_scan<true>", "k_owned_note_scan<false>", "k_owned_note_finish"};
-    static const char* const labeled[3] = {"k_owned_labeled_note_scan<true>", "k_owned_labeled_note_scan<false>", "k_owned_labeled_note_finish"};
-    const auto run = [&](auto launch, const char* const names[3]) {
-        return launch(ctx, names, window, grid, d_keys, n_keys, d_spend_keys, d_records, d_commitments, prep, n, d_owner, d_plaintexts);
-    };
-    switch (kind) {
-    case NOTE_TRANSFER: return run(note_scan_launch<NOTE_TRANSFER>, transfer);
-    case NOTE_OWNED: return run(note_scan_launch<NOTE_OWNED>, owned);
-    case NOTE_OWNED_LABELED: return run(note_scan_launch<NOTE_OWNED_LABELED>, labeled);
-    }
-    return OG_OK;
+    return with_note_kind(kind, [&](auto k) -> int32_t {
+        constexpr NoteKind KIND = decltype(k)::value;
+        if (n_keys)
+            OG_LAUNCHN(ctx, NOTE_KERNEL_NAMES[KIND].scan, k_note_scan<KIND>, dim3(blocks, n_keys), 64, 0, d_keys, d_spend_keys, d_records,
+                       d_commitments, prep, n, d_owner);
+        OG_LAUNCHN(ctx, NOTE_KERNEL_NAMES[KIND].finish, k_note_finish<KIND>, blocks, 64, 0, d_keys, n_keys, d_records, d_commitments, prep, n,
+                   d_owner, d_plaintexts);
+        return OG_OK;
+    });
 }
 
 }  // namespace og

@@ -1,12 +1,11 @@
 """Encrypted notes on the GPU: encryption and scanning rates with inputs resident in HBM (the `_dev` entry points), timed with
 CUDA events on the library's stream, median of --steps after --warmup; a per-kernel split from og_profile in a separate run;
 the scan's share of the carry-chain peak from the operation count below and og_int_pipe_peaks measured in the same run; the
-card's name and power limit from read-only nvidia-smi queries.  Both variable-base multipliers of the scan are timed
-(plain double-and-add, and the 4-bit window selected with OG_NOTE_WINDOW=1).
+card's name and power limit from read-only nvidia-smi queries.
 
 Operation count of one (record, key) pair in k_note_scan, in Fr products (one product = 64 + 64 = 128 carry-chain 32x32-bit
 multiply-adds: the 8x8-limb product and its Montgomery reduction):
-  v E' by double-and-add: 256 doublings x 8 + about 128 additions x 13 = 3712 (the window: 252 x 8 + 78 x 13 = 3030)
+  v E' by the 4-bit window: 252 doublings x 8 + at most 78 additions x 13 = 3030
   affine(S): one inversion by exponentiation, about 256 squarings + 128 products, and 2 products = 386
   MiMC7: k (2 permutations) and the 4 pads, 6 x 91 rounds x 4 products = 2184 (a foreign record stops there: its amount
   is not below 2^64, so the 4 permutations of the commitment run only for candidate notes)
@@ -21,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
-PRODUCTS_PER_PAIR = {"plain": 3712 + 386 + 2184, "window": 3030 + 386 + 2184}
+PRODUCTS_PER_PAIR = 3030 + 386 + 2184
 MADDS_PER_PRODUCT = 128
 
 
@@ -88,23 +87,18 @@ def main():
     encrypt(nmax)
     ctx.sync()
     assert bytes(d_st.cpu().numpy()) == b"\x01" * nmax
-    for variant in ("plain", "window"):
-        os.environ["OG_NOTE_WINDOW"] = "1" if variant == "window" else "0"
-        for n in (1 << 16, 1 << 20):
-            for k in (1, 8):
-                med, lo, hi = timed(lambda: ctx.note_scan_dev(kb[:32 * k], d_rec, d_cm, n, d_owner, d_plain))
-                pairs = n * k / med * 1e3
-                results["scan"].append({"variant": variant, "n": n, "keys": k, "ms": med, "ms_min": lo, "ms_max": hi,
-                                        "records_per_s": n / med * 1e3, "pairs_per_s": pairs,
-                                        "share_of_carry_chain_peak": pairs * PRODUCTS_PER_PAIR[variant] * MADDS_PER_PRODUCT / chain_peak})
-        # per-kernel split of one 2^20 x 8 scan and one 2^20 encryption, in a separate profiled run
-        ctx.profile(True)
-        ctx.note_scan_dev(kb, d_rec, d_cm, nmax, d_owner, d_plain)
-        if variant == "plain":
-            encrypt(nmax)
-        results["profile_" + variant] = ctx.profile_dump()
-        ctx.profile(False)
-    os.environ.pop("OG_NOTE_WINDOW")
+    for n in (1 << 16, 1 << 20):
+        for k in (1, 8):
+            med, lo, hi = timed(lambda: ctx.note_scan_dev(kb[:32 * k], d_rec, d_cm, n, d_owner, d_plain))
+            pairs = n * k / med * 1e3
+            results["scan"].append({"n": n, "keys": k, "ms": med, "ms_min": lo, "ms_max": hi, "records_per_s": n / med * 1e3,
+                                    "pairs_per_s": pairs, "share_of_carry_chain_peak": pairs * PRODUCTS_PER_PAIR * MADDS_PER_PRODUCT / chain_peak})
+    # per-kernel split of one 2^20 x 8 scan and one 2^20 encryption, in a separate profiled run
+    ctx.profile(True)
+    ctx.note_scan_dev(kb, d_rec, d_cm, nmax, d_owner, d_plain)
+    encrypt(nmax)
+    results["profile"] = ctx.profile_dump()
+    ctx.profile(False)
     found = int((d_owner != -1).sum().item())
     results["owned_in_last_scan"] = found
     print(json.dumps(results, indent=1))
