@@ -403,6 +403,22 @@ int32_t og_owned_labeled_transfer_witness(og_ctx* ctx, uint32_t depth, const uin
                                           const uint64_t* out_amounts, const uint8_t* assoc_siblings, const uint32_t* assoc_path_bits,
                                           uint32_t batch, uint8_t* witnesses);
 
+/* ---- the ragequit statement (DESIGN.md section 3): the public exit of an owned labeled note, with no provider approval ---- */
+/* Public inputs (root, token, amount, label, recipient, nullifier): one owned labeled note (P = MultiMiMC7([s], 3), blinding,
+ * token, amount, label) whose leaf reaches root, spent whole and paid to recipient; nullifier is og_owned_nullifiers' of
+ * (s, leaf, index), the one an owned labeled transfer of the note would publish.  depth 1..32; at depth 32: 27 076
+ * variables, 27 037 constraints, domain 2^15. */
+int32_t og_ragequit_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m);
+/* CSR of matrix `which` (0 = A, 1 = B, 2 = C); pass NULL arrays to query nnz only */
+int32_t og_ragequit_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz);
+/* full assignments (batch * n_vars * 32 B) computed on the GPU.  Per proof: root, token, recipient (32 B each), amount
+ * (uint64), label (uint32), spend_key, blinding (32 B each), siblings (depth x 32 B), path_bits (uint32; only the low depth
+ * bits count).  root is the caller's and the nullifier is derived: a wrong spend key, blinding, token, amount, label or path
+ * gives a witness that does not satisfy the R1CS. */
+int32_t og_ragequit_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                            const uint64_t* amounts, const uint32_t* labels, const uint8_t* spend_keys, const uint8_t* blindings,
+                            const uint8_t* siblings, const uint32_t* path_bits, uint32_t batch, uint8_t* witnesses);
+
 /* ---- Groth16 ------------------------------------------------------------------------------------ */
 /* Development ("toxic waste in the clear") setup for the withdraw statement, computed on the GPU.
  * toxic = tau || alpha || beta || gamma || delta (5 * 32 B).  Writes serialized pk / vk blobs;
@@ -557,6 +573,17 @@ int32_t og_groth16_prove_owned_labeled_transfer_dev(og_ctx* ctx, const og_pk* pk
                                                     const uint8_t* d_out_blindings, const uint64_t* d_out_amounts,
                                                     const uint8_t* d_assoc_siblings, const uint32_t* d_assoc_path_bits, uint32_t batch,
                                                     const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
+/* batch of ragequit proofs, witness generation on the GPU; inputs as in og_ragequit_witness.  OG_E_INVALID unless the key
+ * has a ragequit statement's shape (the depth is recognised from it).  public_out (optional): batch * 6 * 32 B = root,
+ * token, amount, label, recipient, nullifier. */
+int32_t og_groth16_prove_ragequit(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                  const uint64_t* amounts, const uint32_t* labels, const uint8_t* spend_keys, const uint8_t* blindings,
+                                  const uint8_t* siblings, const uint32_t* path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
+                                  uint8_t* public_out);
+int32_t og_groth16_prove_ragequit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens, const uint8_t* d_recipients,
+                                      const uint64_t* d_amounts, const uint32_t* d_labels, const uint8_t* d_spend_keys,
+                                      const uint8_t* d_blindings, const uint8_t* d_siblings, const uint32_t* d_path_bits, uint32_t batch,
+                                      const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out);
 /* debug/parity probe: the H-query scalars d_j = (a*b - c)(g w^j) for one witness, 2^log_m * 32 B */
 int32_t og_groth16_h_evals(og_ctx* ctx, const og_pk* pk, const uint8_t* witness, uint8_t* out);
 

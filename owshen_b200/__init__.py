@@ -1,6 +1,6 @@
 """owshen_b200 -- H100-native (sm_90a) Groth16 backend for privacy-pool deposit, withdraw, transfer, association-set
-withdraw, exclusion withdraw, labeled withdraw, labeled association withdraw, owned transfer and owned labeled transfer
-proofs over BN254, with encrypted delivery of the notes they create.
+withdraw, exclusion withdraw, labeled withdraw, labeled association withdraw, owned transfer, owned labeled transfer and
+ragequit proofs over BN254, with encrypted delivery of the notes they create.
 
 Python is the host language here because the reference's (Rust) toolchain is absent from this image;
 everything below is a thin ctypes veneer over the C ABI in include/owshen_b200.h, which is the real
@@ -19,6 +19,7 @@ from .api import (Context, ProvingKey, MerkleTree, OwshenB200Error, lib, build_l
                   setup_owned_transfer, owned_transfer_r1cs_info, owned_transfer_r1cs_export, ptau_prepare_owned_transfer,
                   deposit_owned_labeled, setup_owned_labeled_transfer, owned_labeled_transfer_r1cs_info,
                   owned_labeled_transfer_r1cs_export, ptau_prepare_owned_labeled_transfer,
+                  setup_ragequit, ragequit_r1cs_info, ragequit_r1cs_export, ptau_prepare_ragequit,
                   ptau_new, ptau_contribute, ptau_verify, ptau_prepare, ptau_prepare_withdraw, ptau_prepare_deposit,
                   ptau_prepare_transfer, phase2_contribute, phase2_verify, NOTE_SUBGROUP_ORDER, NOTE_NOT_OWNED, NOTE_MALFORMED)
 
@@ -35,4 +36,5 @@ __all__ = ["Context", "ProvingKey", "MerkleTree", "OwshenB200Error", "lib", "bui
            "setup_owned_transfer", "owned_transfer_r1cs_info", "owned_transfer_r1cs_export", "ptau_prepare_owned_transfer",
            "deposit_owned_labeled", "setup_owned_labeled_transfer", "owned_labeled_transfer_r1cs_info",
            "owned_labeled_transfer_r1cs_export", "ptau_prepare_owned_labeled_transfer",
+           "setup_ragequit", "ragequit_r1cs_info", "ragequit_r1cs_export", "ptau_prepare_ragequit",
            "NOTE_SUBGROUP_ORDER", "NOTE_NOT_OWNED", "NOTE_MALFORMED"]

@@ -137,6 +137,9 @@ _SIGS = {
     "og_owned_labeled_transfer_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
     "og_owned_labeled_transfer_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_owned_labeled_transfer_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 15 + [C.c_uint32, C.c_void_p]),
+    "og_ragequit_r1cs_info": (C.c_int32, [C.c_uint32] + [C.POINTER(C.c_uint32)] * 4),
+    "og_ragequit_r1cs_export": (C.c_int32, [C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "og_ragequit_witness": (C.c_int32, [C.c_void_p, C.c_uint32] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p]),
     "og_groth16_setup_withdraw": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
     "og_groth16_setup": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32] + [C.c_void_p] * 9
                          + [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.POINTER(C.c_uint64)]),
@@ -167,6 +170,8 @@ _SIGS = {
                                                 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_prove_owned_labeled_transfer_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 15
                                                     + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_ragequit": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "og_groth16_prove_ragequit_dev": (C.c_int32, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_pk_prover_plan": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "og_groth16_h_evals": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "og_groth16_verify": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -315,6 +320,9 @@ _STATEMENTS = {
                                       ("in_path_bits", 8, 0, _u32_array), ("out_owners", 64, 0, None), ("out_blindings", 64, 0, None),
                                       ("out_amounts", 16, 0, _u64_array), ("assoc_siblings", 0, 32, None),
                                       ("assoc_path_bits", 4, 0, _u32_array))),
+    "ragequit": (True, (("roots", 32, 0, None), ("tokens", 32, 0, None), ("recipients", 32, 0, None), ("amounts", 8, 0, _u64_array),
+                        ("labels", 4, 0, _label_array), ("spend_keys", 32, 0, None), ("blindings", 32, 0, None), ("siblings", 0, 32, None),
+                        ("path_bits", 4, 0, _u32_array))),
 }
 
 
@@ -862,6 +870,13 @@ class Context:
                                                                          in_blindings, in_amounts, in_siblings, in_path_bits, out_owners,
                                                                          out_blindings, out_amounts, assoc_siblings, assoc_path_bits))
 
+    def ragequit_witness(self, depth, roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings, path_bits) -> bytes:
+        """Full assignments of the depth-`depth` ragequit statement, n_vars * 32 bytes per proof, computed on the GPU.  Per
+        proof: root, token, recipient 32 bytes each; the note's amount one uint64 and its label one uint32; its spending key
+        and blinding 32 bytes each; siblings depth elements and path_bits one word, the note's pool path."""
+        return self._statement_witness("ragequit", depth, (roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings,
+                                                           path_bits))
+
 
 def mimc7_constants():
     out = C.create_string_buffer(32 * 91)
@@ -970,6 +985,15 @@ def owned_labeled_transfer_r1cs_export(depth: int, which: str):
     return _statement_r1cs_export("owned_labeled_transfer", depth, which)
 
 
+def ragequit_r1cs_info(depth: int) -> dict:
+    return _statement_r1cs_info("ragequit", depth)
+
+
+def ragequit_r1cs_export(depth: int, which: str):
+    """(row_ptr, col_idx, coeffs as ints) of matrix 'A' | 'B' | 'C' of the product's depth-`depth` ragequit R1CS."""
+    return _statement_r1cs_export("ragequit", depth, which)
+
+
 def _r1cs_args(A, B, C_):
     """(n_constraints, the nine CSR arguments of og_groth16_setup / og_ptau_prepare) after the length checks."""
     mats = []
@@ -1053,6 +1077,12 @@ def setup_owned_labeled_transfer(ctx: Context, depth: int, tau: int, alpha: int,
     """Development setup of the depth-`depth` owned labeled transfer statement -> (pk_bytes, vk_bytes): its exported R1CS
     through setup_r1cs.  The key records depth 0; the prover recognises it as an owned labeled transfer key by its shape."""
     return _setup_statement(ctx, "owned_labeled_transfer", depth, (tau, alpha, beta, gamma, delta))
+
+
+def setup_ragequit(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
+    """Development setup of the depth-`depth` ragequit statement -> (pk_bytes, vk_bytes): its exported R1CS through
+    setup_r1cs.  The key records depth 0; the prover recognises it as a ragequit key by its shape."""
+    return _setup_statement(ctx, "ragequit", depth, (tau, alpha, beta, gamma, delta))
 
 
 def setup_withdraw(ctx: Context, depth: int, tau: int, alpha: int, beta: int, gamma: int, delta: int):
@@ -1153,6 +1183,10 @@ def ptau_prepare_owned_transfer(ctx: Context, acc: bytes, depth: int):
 
 def ptau_prepare_owned_labeled_transfer(ctx: Context, acc: bytes, depth: int):
     return _ptau_prepare_statement(ctx, acc, "owned_labeled_transfer", depth)
+
+
+def ptau_prepare_ragequit(ctx: Context, acc: bytes, depth: int):
+    return _ptau_prepare_statement(ctx, acc, "ragequit", depth)
 
 
 def phase2_contribute(ctx: Context, pk: bytes, vk: bytes, delta=None, nonce=None):
@@ -1350,6 +1384,19 @@ class ProvingKey:
         return self._prove_statement("owned_labeled_transfer", self.owned_labeled_transfer_depth,
                                      (roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings, in_amounts, in_siblings,
                                       in_path_bits, out_owners, out_blindings, out_amounts, assoc_siblings, assoc_path_bits), rs,
+                                     want_public)
+
+    @property
+    def ragequit_depth(self):
+        """The depth d whose ragequit statement has this key's shape (ragequit_r1cs_info), or None."""
+        return self._shape_depth("ragequit")
+
+    def prove_ragequit(self, roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings, path_bits, rs,
+                       want_public=True):
+        """Batch of ragequit proofs from the notes (witness generation on the GPU).  Inputs as in Context.ragequit_witness;
+        returns (proofs, public_inputs) with public inputs (root, token, amount, label, recipient, nullifier) per proof."""
+        return self._prove_statement("ragequit", self.ragequit_depth,
+                                     (roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings, path_bits), rs,
                                      want_public)
 
     def prover_plan(self, batch: int) -> dict:

@@ -1215,6 +1215,20 @@ int32_t og_owned_labeled_transfer_witness(og_ctx* ctx, uint32_t depth, const uin
                                                                      out_amounts, assoc_siblings, assoc_path_bits}, batch, witnesses);
 }
 
+// ---- the ragequit statement --------------------------------------------------------------------------------------
+int32_t og_ragequit_r1cs_info(uint32_t depth, uint32_t* n_constraints, uint32_t* n_vars, uint32_t* n_pub, uint32_t* log_m) {
+    return statement_r1cs_info(ST_RAGEQUIT, depth, n_constraints, n_vars, n_pub, log_m);
+}
+int32_t og_ragequit_r1cs_export(uint32_t depth, int32_t which, uint32_t* row_ptr, uint32_t* col_idx, uint8_t* coeffs, uint64_t* nnz) {
+    return statement_r1cs_export(ST_RAGEQUIT, depth, which, row_ptr, col_idx, coeffs, nnz);
+}
+int32_t og_ragequit_witness(og_ctx* ctx, uint32_t depth, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                            const uint64_t* amounts, const uint32_t* labels, const uint8_t* spend_keys, const uint8_t* blindings,
+                            const uint8_t* siblings, const uint32_t* path_bits, uint32_t batch, uint8_t* witnesses) {
+    return statement_witness(ctx, ST_RAGEQUIT, depth, {roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings, path_bits},
+                             batch, witnesses);
+}
+
 // ---- Groth16 -------------------------------------------------------------------------------------------------------
 int32_t og_groth16_setup(og_ctx* ctx, uint32_t n_constraints, uint32_t n_vars, uint32_t n_pub,
                          const uint32_t* a_row_ptr, const uint32_t* a_col, const uint8_t* a_coeffs,
@@ -1435,6 +1449,22 @@ int32_t og_groth16_prove_owned_labeled_transfer(og_ctx* ctx, const og_pk* pk, co
     return statement_prove(ctx, pk, ST_OWNED_LABELED_TRANSFER, {roots, tokens, recipients, withdrawn, labels, in_spend_keys, in_blindings,
                                                                 in_amounts, in_siblings, in_path_bits, out_owners, out_blindings, out_amounts,
                                                                 assoc_siblings, assoc_path_bits}, batch, rs, proofs, public_out);
+}
+
+int32_t og_groth16_prove_ragequit_dev(og_ctx* ctx, const og_pk* pk, const uint8_t* d_roots, const uint8_t* d_tokens, const uint8_t* d_recipients,
+                                      const uint64_t* d_amounts, const uint32_t* d_labels, const uint8_t* d_spend_keys,
+                                      const uint8_t* d_blindings, const uint8_t* d_siblings, const uint32_t* d_path_bits, uint32_t batch,
+                                      const uint8_t* d_rs, uint8_t* d_proofs, uint8_t* d_public_out) {
+    return statement_prove_dev(ctx, pk, ST_RAGEQUIT, {d_roots, d_tokens, d_recipients, d_amounts, d_labels, d_spend_keys, d_blindings,
+                                                      d_siblings, d_path_bits}, batch, d_rs, d_proofs, d_public_out);
+}
+
+int32_t og_groth16_prove_ragequit(og_ctx* ctx, const og_pk* pk, const uint8_t* roots, const uint8_t* tokens, const uint8_t* recipients,
+                                  const uint64_t* amounts, const uint32_t* labels, const uint8_t* spend_keys, const uint8_t* blindings,
+                                  const uint8_t* siblings, const uint32_t* path_bits, uint32_t batch, const uint8_t* rs, uint8_t* proofs,
+                                  uint8_t* public_out) {
+    return statement_prove(ctx, pk, ST_RAGEQUIT, {roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings, path_bits},
+                           batch, rs, proofs, public_out);
 }
 
 int32_t og_pk_prover_plan(const og_pk* pk, uint32_t batch, uint32_t* chunk, uint32_t* lanes, uint64_t* scratch_bytes_per_lane) {

@@ -661,6 +661,54 @@ __global__ void __launch_bounds__(160) k_owned_labeled_transfer_witness(OwnedLab
     if (active && role == 0) w[11] = (w[6] - w[7]).inv();   // inv(0) = 0: two inputs with one nullifier leave the row unsatisfiable
 }
 
+// Witness of the ragequit statement, layout of DESIGN.md section 3 (== oracle/ragequit_circuit.py); row p starts at
+// W + p * w_stride, Montgomery form.  A CTA covers 32 proofs with two warps, one per independent hash chain of a proof, so no
+// warp diverges and a proof's critical path is the owner, precommitment, leaf and pool path (7 + 2 * depth permutations):
+//   warp 0   the spend key and blinding, the owner with its round values, the precommitment, the leaf, the depth pool levels
+//   warp 1   the owner, precommitment and leaf again in registers (no stores), the nullifier with its round values, and the
+//            scalars (ONE, root, token, amount, label, recipient, recipient_sq)
+// No warp reads what another wrote, so there is no barrier.  Only the low `depth` bits of the path word count, in the levels
+// and in the nullifier's index alike.
+__global__ void __launch_bounds__(64) k_ragequit_witness(RagequitLayout L, uint32_t w_stride, RagequitInputs in, uint32_t batch,
+                                                         Fr* __restrict__ W, int* flag) {
+    const uint32_t p = blockIdx.x * 32 + (threadIdx.x & 31);
+    if (p >= batch) return;
+    Fr* w = W + (uint64_t)p * w_stride;
+    const Fr token = load_canonical<Fr>(in.tokens + 32ull * p, flag);
+    const Fr am = fr_from_u64(in.amounts[p]);
+    const Fr la = Fr::from_u32(in.labels[p]);
+    const Fr s = load_canonical<Fr>(in.spend_keys + 32ull * p, flag);
+    const Fr bl = load_canonical<Fr>(in.blindings + 32ull * p, flag);
+    const uint32_t bits = in.path_bits[p];
+    const Fr s1[1] = {s};
+    const Fr k3 = Fr::from_u32(OWNED_OWNER_KEY), k6 = Fr::from_u32(OWNED_LABELED_PRE_KEY), k7 = Fr::from_u32(OWNED_LABELED_LEAF_KEY);
+    if (threadIdx.x < 32) {
+        w[8] = s; w[9] = bl;
+        const Fr owner = mimc7_multi_hash<true>(s1, k3, w + L.owner_perm, L.perm);
+        const Fr pre_in[2] = {owner, bl};
+        const Fr pre = mimc7_multi_hash<true>(pre_in, k6, w + L.pre, L.perm);
+        w[L.pre_out] = pre;
+        const Fr leaf_in[4] = {pre, token, am, la};
+        const Fr leaf = mimc7_multi_hash<true>(leaf_in, k7, w + L.leaf, L.perm);
+        w[L.leaf_out] = leaf;
+        witness_path(leaf, w + L.lvl_base, L.depth, L.lvl_size, L.perm, in.siblings + 32ull * L.depth * p, bits, flag);
+    } else {
+        const Fr owner = mimc7_multi_hash<false>(s1, k3, nullptr, 0);
+        const Fr pre_in[2] = {owner, bl};
+        const Fr pre = mimc7_multi_hash<false>(pre_in, k6, nullptr, 0);
+        const Fr leaf_in[4] = {pre, token, am, la};
+        const Fr leaf = mimc7_multi_hash<false>(leaf_in, k7, nullptr, 0);
+        const uint32_t mask = L.depth >= 32 ? 0xffffffffu : (1u << L.depth) - 1;
+        const Fr nf_in[3] = {s, leaf, Fr::from_u32(bits & mask)};
+        w[6] = mimc7_multi_hash<true>(nf_in, Fr::from_u32(OWNED_NULLIFIER_KEY), w + L.nf_perm, L.perm);
+        const Fr re = load_canonical<Fr>(in.recipients + 32ull * p, flag);
+        w[0] = Fr::one();
+        w[1] = load_canonical<Fr>(in.roots + 32ull * p, flag);
+        w[2] = token; w[3] = am; w[4] = la; w[5] = re;
+        w[7] = re.sqr();
+    }
+}
+
 // ---- host side ------------------------------------------------------------------------------------
 void mimc_constants_host(Fr* out91) { mimc7_round_constants(out91); }
 
@@ -738,8 +786,8 @@ int32_t mimc_tree_append_dev(og_ctx* ctx, uint32_t depth, uint64_t start, uint64
     return OG_OK;
 }
 
-// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion, labeled, labeled association and
-// owned transfer kernels give a proof more than one warp.
+// One CTA covers 32 proofs in every statement's kernel; the transfer, association, exclusion, labeled, labeled association,
+// owned transfer, owned labeled transfer and ragequit kernels give a proof more than one warp.
 int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t w_stride, const StatementInputs& in, uint32_t batch,
                               Fr* d_W) {
     if (batch == 0) return OG_OK;
@@ -796,6 +844,11 @@ int32_t statement_witness_dev(og_ctx* ctx, Statement s, uint32_t depth, uint32_t
                                            a[8], (const uint32_t*)a[9], a[10], a[11], (const uint64_t*)a[12], a[13], (const uint32_t*)a[14]};
         OG_LAUNCH(ctx, k_owned_labeled_transfer_witness, grid, 160, 0, OwnedLabeledTransferLayout::make(depth), w_stride, t, batch, d_W,
                   ctx->d_flag);
+        break;
+    }
+    case ST_RAGEQUIT: {
+        const RagequitInputs t{a[0], a[1], a[2], (const uint64_t*)a[3], (const uint32_t*)a[4], a[5], a[6], a[7], (const uint32_t*)a[8]};
+        OG_LAUNCH(ctx, k_ragequit_witness, grid, 64, 0, RagequitLayout::make(depth), w_stride, t, batch, d_W, ctx->d_flag);
         break;
     }
     }

@@ -1,9 +1,9 @@
 // owshen_b200/csrc/mimc.cuh -- declarations of the MiMC7 module and the variable layouts of the
-// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw, owned transfer and owned
-// labeled transfer statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
+// withdraw, deposit, transfer, association, exclusion, labeled and labeled association withdraw, owned transfer, owned
+// labeled transfer and ragequit statements (DESIGN.md section 3; must equal oracle/withdraw_circuit.py: Layout,
 // oracle/deposit_circuit.py: Layout, oracle/transfer_circuit.py: Layout, oracle/association_circuit.py: Layout,
 // oracle/exclusion_circuit.py: Layout, oracle/labeled_circuit.py: Layout, oracle/labeled_association_circuit.py: Layout,
-// oracle/owned_circuit.py: Layout and oracle/owned_labeled_circuit.py: Layout).
+// oracle/owned_circuit.py: Layout, oracle/owned_labeled_circuit.py: Layout and oracle/ragequit_circuit.py: Layout).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -383,12 +383,48 @@ struct OwnedLabeledTransferInputs {
     const uint32_t* assoc_bits;
 };
 
+constexpr uint32_t RAGEQUIT_N_PUB = 6;
+
+// 0 ONE | 1 root | 2 token | 3 amount | 4 label | 5 recipient | 6 nullifier | 7 recipient_sq | 8 spend_key | 9 blinding | the
+// owner permutation | the precommitment's two permutations and its output | the leaf's four permutations and its output |
+// depth pool levels | the nullifier's three permutations (oracle/ragequit_circuit.py).  The owned labeled family's note keys.
+struct RagequitLayout {
+    uint32_t depth, perm;
+    uint32_t owner_perm, pre, pre_out, leaf, leaf_out, lvl_base, lvl_size, nf_perm;
+    uint32_t n_vars, n_constraints;
+    static RagequitLayout make(uint32_t depth, uint32_t n_rounds = 91) {
+        RagequitLayout L;
+        L.depth = depth;
+        L.perm = 4 * n_rounds;
+        const uint32_t P = L.perm;
+        L.lvl_size = 2 * P + 4;
+        L.owner_perm = 10;
+        L.pre = 10 + P; L.pre_out = 10 + 3 * P;
+        L.leaf = 11 + 3 * P; L.leaf_out = 11 + 7 * P;
+        L.lvl_base = 12 + 7 * P;
+        L.nf_perm = L.lvl_base + depth * L.lvl_size;
+        L.n_vars = L.nf_perm + 3 * P;
+        L.n_constraints = 5 + 10 * P + depth * (2 * P + 3);
+        return L;
+    }
+};
+
+// the caller's inputs of a batch of ragequits (k_ragequit_witness's argument), in C ABI order; per proof: root, token,
+// recipient (32 B each), amount (u64), label (u32), spend key, blinding (32 B each), depth siblings and a path-bits word
+struct RagequitInputs {
+    const uint8_t *roots, *tokens, *recipients;
+    const uint64_t* amounts;
+    const uint32_t* labels;
+    const uint8_t *spend_keys, *blindings, *siblings;
+    const uint32_t* path_bits;
+};
+
 // ---- the statement table ------------------------------------------------------------------------------------------------
 // What the C ABI, the prover and api.py (_STATEMENTS, which mirrors this table) know of a statement.  Besides its row here a
 // statement has a layout (above), an R1CS builder (withdraw_circuit.hpp: statement_r1cs), a witness kernel (mimc.cu:
 // statement_witness_dev) and its og_* forwarders (capi.cu).
 enum Statement : uint32_t { ST_WITHDRAW, ST_DEPOSIT, ST_TRANSFER, ST_ASSOCIATION, ST_EXCLUSION, ST_LABELED, ST_LABELED_ASSOCIATION,
-                            ST_OWNED_TRANSFER, ST_OWNED_LABELED_TRANSFER };
+                            ST_OWNED_TRANSFER, ST_OWNED_LABELED_TRANSFER, ST_RAGEQUIT };
 constexpr uint32_t STATEMENT_MAX_INPUTS = 15;
 
 struct StatementShape { uint32_t n_vars, n_constraints; };
@@ -433,6 +469,8 @@ constexpr StatementDesc STATEMENTS[] = {
     // in_siblings, in_path_bits, out_owners, out_blindings, out_amounts, assoc_siblings, assoc_path_bits
     {OWNED_LABELED_TRANSFER_N_PUB, layout_shape<OwnedLabeledTransferLayout>, true, 15,
      {32, 32, 32, 8, 4, 64, 64, 16, 0, 8, 64, 64, 16, 0, 4}, {0, 0, 0, 0, 0, 0, 0, 0, 64, 0, 0, 0, 0, 32, 0}},
+    // ragequit: roots, tokens, recipients, amounts, labels, spend_keys, blindings, siblings, path_bits
+    {RAGEQUIT_N_PUB, layout_shape<RagequitLayout>, true, 9, {32, 32, 32, 8, 4, 32, 32, 0, 4}, {0, 0, 0, 0, 0, 0, 0, 32, 0}},
 };
 
 // the input arrays of a batch in the statement's C ABI order (host or device pointers)

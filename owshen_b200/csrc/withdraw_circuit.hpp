@@ -56,6 +56,12 @@
 //   amount, label], 7) with one label for all four notes; nullifier = MultiMiMC7([spend_key, leaf, leaf index], 5); label
 //   range-checked to 32 bits, withdrawn and the amounts to 64; in0 + in1 = out0 + out1 + withdrawn; nonzero inputs open
 //   under root; nf[0] != nf[1]; assoc_leaf = label + 1 reaching association_root; recipient^2 bound.
+// ragequit
+//   public : root, token, amount, label, recipient, nullifier
+//   private: spend_key, blinding, siblings[depth], bits[depth]
+//   the owned labeled transfer's owner, precommitment, leaf and nullifier for one note, spent whole; the leaf reaches root
+//   unconditionally; no range rows (the leaf binds amount and label, and every key-7 leaf in the pool was range-checked on
+//   its way in); no association path; recipient^2 bound.
 #pragma once
 #include <map>
 #include <vector>
@@ -503,6 +509,42 @@ struct OwnedLabeledTransferBuilder {
     }
 };
 
+struct RagequitBuilder {
+    static constexpr uint32_t V_ONE = 0, V_ROOT = 1, V_TOKEN = 2, V_AMOUNT = 3, V_LABEL = 4, V_RECIP = 5, V_NF = 6, V_RSQ = 7,
+                              V_KEY = 8, V_BLINDING = 9;
+
+    static R1cs build(uint32_t depth, uint32_t n_rounds = MIMC_ROUNDS) {
+        Mimc7Builder b(n_rounds);
+        RagequitLayout L = RagequitLayout::make(depth, n_rounds);
+        b.cs.n_vars = L.n_vars;
+        b.cs.n_pub = RAGEQUIT_N_PUB;
+        const uint32_t P = L.perm;
+        b.cs.add(lc_var(V_RECIP), lc_var(V_RECIP), lc_var(V_RSQ));
+        // owner P = MultiMiMC7([s], 3) = 3 + s + hash(s, 3), kept as a linear combination
+        LC s = lc_var(V_KEY), k3; k3[V_ONE] = Fr::from_u32(OWNED_OWNER_KEY);
+        LC h = b.perm(s, k3, L.owner_perm);
+        LC owner = lc_sum({&k3, &s, &h});
+        LC k6, k7; k6[V_ONE] = Fr::from_u32(OWNED_LABELED_PRE_KEY); k7[V_ONE] = Fr::from_u32(OWNED_LABELED_LEAF_KEY);
+        LC bl = lc_var(V_BLINDING), tok = lc_var(V_TOKEN), am = lc_var(V_AMOUNT), la = lc_var(V_LABEL);
+        b.multi_hash({&owner, &bl}, k6, {L.pre, L.pre + P}, L.pre_out);
+        LC vpre = lc_var(L.pre_out);
+        b.multi_hash({&vpre, &tok, &am, &la}, k7, {L.leaf, L.leaf + P, L.leaf + 2 * P, L.leaf + 3 * P}, L.leaf_out);
+        const uint32_t cur = b.merkle_path(L.leaf_out, L.lvl_base, L.lvl_size, depth);
+        // (root - node) * ONE = 0, unconditional: a zero-value note off the tree does not ragequit
+        LC vroot = lc_var(V_ROOT), ncur = lc_neg_var(cur);
+        b.cs.add(lc_sum({&vroot, &ncur}), lc_var(V_ONE), LC());
+        // nullifier = MultiMiMC7([s, leaf, index], 5), the owned labeled transfer's, bound to the public nullifier directly
+        LC vleaf = lc_var(L.leaf_out), index, k5; k5[V_ONE] = Fr::from_u32(OWNED_NULLIFIER_KEY);
+        Fr pow2 = Fr::one();
+        for (uint32_t l = 0; l < depth; l++) {
+            lc_add_term(index, L.lvl_base + l * L.lvl_size + 1, pow2);
+            pow2 = pow2 + pow2;
+        }
+        b.multi_hash({&s, &vleaf, &index}, k5, {L.nf_perm, L.nf_perm + P, L.nf_perm + 2 * P}, V_NF);
+        return b.cs;
+    }
+};
+
 // the statement's R1CS at `depth` (ignored by deposit)
 inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     switch (s) {
@@ -515,6 +557,7 @@ inline R1cs statement_r1cs(Statement s, uint32_t depth) {
     case ST_LABELED_ASSOCIATION: return LabeledAssociationBuilder::build(depth);
     case ST_OWNED_TRANSFER: return OwnedTransferBuilder::build(depth);
     case ST_OWNED_LABELED_TRANSFER: return OwnedLabeledTransferBuilder::build(depth);
+    case ST_RAGEQUIT: return RagequitBuilder::build(depth);
     }
     return R1cs();
 }

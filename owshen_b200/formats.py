@@ -89,6 +89,10 @@ SHIELDED_TRANSFER_KIND = "shielded-transfer"
 # the owned labeled notes of its outputs:
 #     ["shielded-labeled-transfer", proof (256 B), 9 public inputs (32 B LE each), record 0, record 1 (160 B each)]
 SHIELDED_LABELED_TRANSFER_KIND = "shielded-labeled-transfer"
+# A shielded ragequit (the public exit of an owned labeled note) has a kind of its own, 6 public inputs and no records: it
+# creates no note.
+#     ["shielded-ragequit", proof (256 B), 6 public inputs (32 B LE each)]
+SHIELDED_RAGEQUIT_KIND = "shielded-ragequit"
 
 
 def rlp_encode(item) -> bytes:
@@ -216,3 +220,23 @@ def shielded_labeled_transfer_from_rlp(msg: bytes):
             or any(len(r) != 160 for r in recs)):
         raise ValueError("Invalid tx!")
     return proof, b"".join(pub), b"".join(recs)
+
+
+def shielded_ragequit_to_rlp(proof: bytes, public_inputs: bytes) -> bytes:
+    """CustomTxMsg-shaped message for one ragequit proof: public_inputs = the 6 inputs of og_groth16_prove_ragequit's
+    `public_out` row (192 B: root, token, amount, label, recipient, nullifier)."""
+    if len(proof) != 256 or len(public_inputs) != 192:
+        raise ValueError("shielded_ragequit_to_rlp: proof must be 256 bytes, public inputs 192")
+    return rlp_encode([SHIELDED_RAGEQUIT_KIND, proof] + [public_inputs[32 * i:32 * i + 32] for i in range(6)])
+
+
+def shielded_ragequit_from_rlp(msg: bytes):
+    """-> (proof, public_inputs); raises ValueError("Invalid tx!") on anything that is not a well-formed shielded-ragequit
+    message."""
+    item = rlp_decode(msg)
+    if not isinstance(item, list) or len(item) != 8 or any(isinstance(x, list) for x in item):
+        raise ValueError("Invalid tx!")
+    kind, proof, pub = item[0], item[1], item[2:8]
+    if kind != SHIELDED_RAGEQUIT_KIND.encode() or len(proof) != 256 or any(len(x) != 32 for x in pub):
+        raise ValueError("Invalid tx!")
+    return proof, b"".join(pub)
